@@ -109,7 +109,10 @@ int32_t rapid_view_num_joiners(const rapid_view* v, int64_t* out);
  * bus.  Ids are renumbered densely (surviving members in order, then the admitted joiners; joiners not in the cut are
  * dropped); out_old_to_new[n + joiners] receives the mapping (-1 = gone) and may be NULL.  With NodeIds set
  * (rapid_view_set_node_ids) an admitted joiner whose NodeId is already in identifiersSeen -> RAPID_EUUID_SEEN
- * (UUIDAlreadySeenException, MembershipView.java:126-128) and NOTHING changes.  Detector handles created on the old view must be
+ * (UUIDAlreadySeenException, MembershipView.java:126-128) and NOTHING changes.  A cut that admits one endpoint twice (registered
+ * twice as a joiner) -> RAPID_EALREADY_IN_RING (the second ringAdd's NodeAlreadyInRingException); two different endpoints with
+ * equal keys on a ring -> RAPID_EHASH_COLLISION.  Every refusal leaves the view, identifiersSeen included, as it was, and
+ * out_old_to_new unwritten.  Detector handles created on the old view must be
  * destroyed and recreated (their receivers are ring-0 positions of that view). */
 int32_t rapid_view_apply_cut(rapid_view* v, const int32_t* cut_ids, int64_t n_cut, int32_t* out_old_to_new);
 /* identifiersSeen on the device (MembershipView.java:58-60): NodeIds of the current members (index = node id) seed it —

@@ -231,18 +231,21 @@ static int32_t upload_endpoints(View* v, int64_t count, const uint8_t* hb, const
     return RAPID_OK;
 }
 
-// error reporting only: are the endpoints with ids a and b the same (hostname, port)?  Fetched from the device.
-static bool same_endpoint(const View* v, int64_t a, int64_t b) {
+// error reporting only: are the endpoints with ids a and b of a device endpoint table the same (hostname, port)?
+static bool same_endpoint(const uint8_t* hb, const int32_t* off, const int32_t* port, int64_t a, int64_t b) {
     int32_t oa[2], ob[2], pa = 0, pb = 0;
-    if (cudaMemcpy(oa, v->host_off.p + a, sizeof(oa), cudaMemcpyDeviceToHost) != cudaSuccess) return false;
-    if (cudaMemcpy(ob, v->host_off.p + b, sizeof(ob), cudaMemcpyDeviceToHost) != cudaSuccess) return false;
-    cudaMemcpy(&pa, v->port.p + a, sizeof(pa), cudaMemcpyDeviceToHost);
-    cudaMemcpy(&pb, v->port.p + b, sizeof(pb), cudaMemcpyDeviceToHost);
+    if (cudaMemcpy(oa, off + a, sizeof(oa), cudaMemcpyDeviceToHost) != cudaSuccess) return false;
+    if (cudaMemcpy(ob, off + b, sizeof(ob), cudaMemcpyDeviceToHost) != cudaSuccess) return false;
+    cudaMemcpy(&pa, port + a, sizeof(pa), cudaMemcpyDeviceToHost);
+    cudaMemcpy(&pb, port + b, sizeof(pb), cudaMemcpyDeviceToHost);
     const int32_t la = oa[1] - oa[0], lb = ob[1] - ob[0];
     if (la != lb || pa != pb) return false;
     std::vector<uint8_t> ba((size_t)std::max(la, 1)), bb((size_t)std::max(lb, 1));
-    if (la) { cudaMemcpy(ba.data(), v->host_bytes.p + oa[0], (size_t)la, cudaMemcpyDeviceToHost); cudaMemcpy(bb.data(), v->host_bytes.p + ob[0], (size_t)lb, cudaMemcpyDeviceToHost); }
+    if (la) { cudaMemcpy(ba.data(), hb + oa[0], (size_t)la, cudaMemcpyDeviceToHost); cudaMemcpy(bb.data(), hb + ob[0], (size_t)lb, cudaMemcpyDeviceToHost); }
     return memcmp(ba.data(), bb.data(), (size_t)la) == 0;
+}
+static bool same_endpoint(const View* v, int64_t a, int64_t b) {
+    return same_endpoint(v->host_bytes.p, v->host_off.p, v->port.p, a, b);
 }
 
 static int32_t build_rings(View* v) {
@@ -528,6 +531,10 @@ __global__ void k_cut_joiner_keys(int K, int64_t n, int64_t tot, size_t stride, 
     jk[(size_t)k * m + j] = (uint64_t)key[(size_t)k * stride + id] ^ 0x8000000000000000ULL;
     jv[(size_t)k * m + j] = newid[id];
 }
+// collision[0] = ring of the first equal-key pair found (-1: none), collision[1..2] = the pair's new ids
+__device__ __forceinline__ void cut_collision(int32_t* collision, int k, int32_t a, int32_t b) {
+    if (atomicCAS(&collision[0], -1, k) == -1) { collision[1] = a; collision[2] = b; }
+}
 // the (few) joiners of every ring sorted by key: rank = number of joiners with a smaller key, all pairs through shared memory;
 // two joiners with the same key on a ring -> collision (TreeSet.add would silently drop one)
 __global__ void __launch_bounds__(256) k_cut_joiner_rank(int32_t m, const uint64_t* __restrict__ jk, const int32_t* __restrict__ jv,
@@ -535,6 +542,7 @@ __global__ void __launch_bounds__(256) k_cut_joiner_rank(int32_t m, const uint64
     __shared__ uint64_t s_k[256];
     const int k = blockIdx.y;
     const uint64_t* mk = jk + (size_t)k * m;
+    const int32_t* mv = jv + (size_t)k * m;
     const int32_t i = blockIdx.x * 256 + threadIdx.x;
     const uint64_t key = i < m ? mk[i] : 0ull;
     int32_t rank = 0;
@@ -546,10 +554,18 @@ __global__ void __launch_bounds__(256) k_cut_joiner_rank(int32_t m, const uint64
         for (int32_t j = 0; j < lim; ++j) {
             const uint64_t o = s_k[j];
             rank += o < key ? 1 : 0;
-            if (o == key && b + j != i && i < m) atomicCAS(&collision[0], -1, k);
+            if (o == key && b + j != i && i < m) cut_collision(collision, k, mv[i], mv[b + j]);
         }
     }
-    if (i < m) { jk2[(size_t)k * m + rank] = key; jv2[(size_t)k * m + rank] = jv[(size_t)k * m + i]; }
+    if (i < m) { jk2[(size_t)k * m + rank] = key; jv2[(size_t)k * m + rank] = mv[i]; }
+}
+// after the per-ring radix sorts of the joiners: equal keys are adjacent (as k_unflip_and_check finds them for build_rings)
+__global__ void k_cut_joiner_adjacent(int K, int32_t m, const uint64_t* __restrict__ jk2, const int32_t* __restrict__ jv2,
+                                      int32_t* __restrict__ collision) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (int64_t)K * m) return;
+    const int32_t j = (int32_t)(t % m);
+    if (j + 1 < m && jk2[t] == jk2[t + 1]) cut_collision(collision, (int)(t / m), jv2[t], jv2[t + 1]);
 }
 // merge of every ring (blockIdx.y): survivors keep their order, every joiner slots in by its key (TreeSet order of the new membership)
 __global__ void k_cut_merge(int64_t n, int32_t n_surv, int32_t m, const int32_t* __restrict__ ring, const int64_t* __restrict__ sorted_key,
@@ -570,9 +586,10 @@ __global__ void k_cut_merge(int64_t n, int32_t n_surv, int32_t m, const int32_t*
         const uint64_t u = (uint64_t)sk[t] ^ 0x8000000000000000ULL;
         int32_t lo = 0, hi = m;                               // joiners with a smaller key
         while (lo < hi) { const int32_t mid = (lo + hi) >> 1; if (jk[mid] < u) lo = mid + 1; else hi = mid; }
-        if (lo < m && jk[lo] == u) atomicCAS(&collision[0], -1, k);
+        const int32_t me = newid[ring[(size_t)k * n + t]];
+        if (lo < m && jk[lo] == u) cut_collision(collision, k, me, jv[lo]);
         const int32_t out = (ps[t] - base) + lo;
-        ring2[(size_t)k * n2 + out] = newid[ring[(size_t)k * n + t]];
+        ring2[(size_t)k * n2 + out] = me;
         sorted_key2[(size_t)k * n2 + out] = sk[t];
     } else if (t < n + m) {
         const int32_t i = (int32_t)(t - n);
@@ -580,7 +597,7 @@ __global__ void k_cut_merge(int64_t n, int32_t n_surv, int32_t m, const int32_t*
         int64_t lo = 0, hi = n;                               // first old position whose key is >= the joiner's
         while (lo < hi) { const int64_t mid = (lo + hi) >> 1; if (sk[mid] < key) lo = mid + 1; else hi = mid; }
         const int32_t before = n == 0 ? 0 : (lo < n ? ps[lo] - base : ps[n - 1] + fl[n - 1] - base);
-        if (lo < n && sk[lo] == key && fl[lo]) atomicCAS(&collision[0], -1, k);
+        if (lo < n && sk[lo] == key && fl[lo]) cut_collision(collision, k, jv[i], newid[ring[(size_t)k * n + lo]]);
         const int32_t out = before + i;
         ring2[(size_t)k * n2 + out] = jv[i];
         sorted_key2[(size_t)k * n2 + out] = key;
@@ -645,8 +662,9 @@ __global__ void k_ids_merge(const int64_t* __restrict__ ah, const int64_t* __res
     }
 }
 
-// identifiersSeen := merge(identifiersSeen, sorted(add));  RAPID_EUUID_SEEN (nothing changed) if a NodeId would be there twice
-static int32_t seen_add(View* v, const int64_t* add_hi_dev, const int64_t* add_lo_dev, int64_t n_add) {
+// merge(identifiersSeen, sorted(add)) into the id scratch, leaving the view alone; RAPID_EUUID_SEEN if a NodeId would be there
+// twice.  seen_commit swaps the merged set in: a caller that can still refuse does so in between and the view stays unchanged.
+static int32_t seen_merge(View* v, const int64_t* add_hi_dev, const int64_t* add_lo_dev, int64_t n_add) {
     if (n_add <= 0) return RAPID_OK;
     cudaStream_t s = v->stream;
     IdScratch& c = scratch(v)->ids;
@@ -661,10 +679,14 @@ static int32_t seen_add(View* v, const int64_t* add_hi_dev, const int64_t* add_l
     RAPID_CUDA(cudaMemcpyAsync(&f, c.dup.p, sizeof(f), cudaMemcpyDeviceToHost, s));
     RAPID_CUDA(cudaStreamSynchronize(s));
     if (f >= 0) { set_error("a NodeId was seen before (UUIDAlreadySeenException)"); return RAPID_EUUID_SEEN; }
+    return RAPID_OK;
+}
+static void seen_commit(View* v, int64_t n_add) {
+    if (n_add <= 0) return;
+    IdScratch& c = scratch(v)->ids;
     std::swap(v->seen_hi.p, c.oh.p); std::swap(v->seen_hi.cap, c.oh.cap);
     std::swap(v->seen_lo.p, c.ol.p); std::swap(v->seen_lo.cap, c.ol.cap);
-    v->n_seen = tot;
-    return RAPID_OK;
+    v->n_seen += n_add;
 }
 
 template <typename T>
@@ -721,15 +743,16 @@ static int32_t apply_cut_device(View* v, const int32_t* cut_ids, int64_t n_cut, 
         k_cut_keys<<<(unsigned)ceil_div<int64_t>((int64_t)K * tot, TB), TB, 0, s>>>(K, tot, v->key_stride, stride2, c.kept.p, c.newid.p, v->key.p, c.key2.p);
         RAPID_KERNEL_CHECK();
     }
-    // ---- UUID rule for the joiners that come in (:126-128), before anything is swapped in ---------------------------------------
-    if (v->has_node_ids && m > 0) {
+    // ---- UUID rule for the joiners that come in (:126-128): merged beside identifiersSeen, committed at the swap-in --------------
+    const int64_t n_seen_add = v->has_node_ids ? m : 0;
+    if (n_seen_add > 0) {
         // the joiners' NodeIds are the last m entries of the new NodeId arrays (joiners follow the surviving members)
-        const int32_t rc = seen_add(v, c.nhi2.p + n_surv, c.nlo2.p + n_surv, m);
+        const int32_t rc = seen_merge(v, c.nhi2.p + n_surv, c.nlo2.p + n_surv, n_seen_add);
         if (rc != RAPID_OK) return rc;                                       // UUIDAlreadySeenException: the view is unchanged
     }
     // ---- rings: all K at once ------------------------------------------------------------------------------------------------------
-    RAPID_CHECK(c.collision.reserve(1));
-    RAPID_CUDA(cudaMemsetAsync(c.collision.p, 0xff, sizeof(int32_t), s));
+    RAPID_CHECK(c.collision.reserve(3));
+    RAPID_CUDA(cudaMemsetAsync(c.collision.p, 0xff, 3 * sizeof(int32_t), s));
     const size_t kn = (size_t)K * (size_t)std::max<int64_t>(n, 1), km = (size_t)K * (size_t)std::max(m, 1);
     RAPID_CHECK(c.flag.reserve(kn)); RAPID_CHECK(c.pos.reserve(kn));
     RAPID_CHECK(c.jk.reserve(km)); RAPID_CHECK(c.jk2.reserve(km)); RAPID_CHECK(c.jv.reserve(km)); RAPID_CHECK(c.jv2.reserve(km));
@@ -748,6 +771,8 @@ static int32_t apply_cut_device(View* v, const int32_t* cut_ids, int64_t n_cut, 
         } else {
             for (int k = 0; k < K; ++k)
                 RAPID_CHECK(sort_pairs(v, c.jk.p + (size_t)k * m, c.jk2.p + (size_t)k * m, c.jv.p + (size_t)k * m, c.jv2.p + (size_t)k * m, m, s));
+            k_cut_joiner_adjacent<<<(unsigned)ceil_div<int64_t>((int64_t)K * m, TB), TB, 0, s>>>(K, m, c.jk2.p, c.jv2.p, c.collision.p);
+            RAPID_KERNEL_CHECK();
         }
     }
     if (n + m > 0) {
@@ -755,12 +780,21 @@ static int32_t apply_cut_device(View* v, const int32_t* cut_ids, int64_t n_cut, 
                                                                                             c.jk2.p, c.jv2.p, c.ring2.p, c.sk2.p, c.collision.p);
         RAPID_KERNEL_CHECK();
     }
-    int32_t coll = -1;
-    RAPID_CUDA(cudaMemcpyAsync(&coll, c.collision.p, sizeof(coll), cudaMemcpyDeviceToHost, s));
-    if (out_old_to_new && tot) RAPID_CUDA(cudaMemcpyAsync(out_old_to_new, c.map.p, (size_t)tot * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    int32_t coll[3] = {-1, -1, -1};
+    RAPID_CUDA(cudaMemcpyAsync(coll, c.collision.p, sizeof(coll), cudaMemcpyDeviceToHost, s));
     RAPID_CUDA(cudaStreamSynchronize(s));
-    if (coll >= 0) { set_error("ring-%d key collision while adding joiners (TreeSet would silently drop one)", coll); return RAPID_EHASH_COLLISION; }
-    // ---- swap in ------------------------------------------------------------------------------------------------------------------
+    if (coll[0] >= 0) {                                                      // the pair's ids index the new endpoint table
+        if (same_endpoint(c.hb2.p, c.off2.p, c.port2.p, coll[1], coll[2])) {
+            set_error("the cut adds one endpoint twice (new ids %d and %d): NodeAlreadyInRingException", coll[1], coll[2]);
+            return RAPID_EALREADY_IN_RING;
+        }
+        set_error("ring-%d key collision between new ids %d and %d while adding joiners (TreeSet would silently drop one)",
+                  coll[0], coll[1], coll[2]);
+        return RAPID_EHASH_COLLISION;
+    }
+    if (out_old_to_new && tot) RAPID_CUDA(cudaMemcpy(out_old_to_new, c.map.p, (size_t)tot * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    // ---- swap in: nothing can refuse the cut past this point ----------------------------------------------------------------------
+    seen_commit(v, n_seen_add);
     swap_buf(v->host_bytes, c.hb2); swap_buf(v->host_off, c.off2); swap_buf(v->port, c.port2);
     swap_buf(v->key, c.key2); swap_buf(v->ring, c.ring2); swap_buf(v->sorted_key, c.sk2);
     if (v->has_node_ids) { swap_buf(v->node_hi, c.nhi2); swap_buf(v->node_lo, c.nlo2); }
@@ -809,8 +843,9 @@ int32_t rapid_view_set_node_ids(rapid_view* v, const int64_t* id_high, const int
     }
     RAPID_CUDA(cudaStreamSynchronize(v->stream));
     v->n_seen = 0;
-    const int32_t rc = seen_add(v, v->node_hi.p, v->node_lo.p, v->n);
+    const int32_t rc = seen_merge(v, v->node_hi.p, v->node_lo.p, v->n);
     if (rc != RAPID_OK) return rc;
+    seen_commit(v, v->n);
     v->has_node_ids = true;
     return RAPID_OK;
 }

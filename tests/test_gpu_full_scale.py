@@ -138,6 +138,37 @@ def test_c3_ten_thousand_nodes_correlated_partition(orc):
     assert t.decided and t.length == 500 and t.count == rb.quorum(n)
 
 
+@pytest.mark.parametrize("n", [63 * 1024, 70_000])
+def test_c3_partition_on_both_sides_of_the_invalidation_split(orc, n):
+    """k_inval_finalize2 splits a tile's work list over several blocks below 64 tiles of 1024 receivers and gives every tile one
+    block from 64 tiles on: a C3 partition at 63 tiles and at 69, checked receiver by receiver on windows that straddle a tile
+    edge and windows inside the partitioned arc"""
+    import rapid_b200 as rb
+    v = _view(rb, n)
+    obs, _ = v.tables()
+    ring0 = v.getRing(0)
+    b = W.c3_correlated_partition(obs, ring0, n, 0.05)
+    hi, lo = W.node_ids(0, n)
+    cfg = v.getCurrentConfigurationId(hi, lo)
+    blocked = W.blocked_by_receiver(b.blocked, ring0, 0, n)
+    cl = rb.VirtualCluster(v, H, L)
+    res, _ = _check_converged(rb, v, cl, b, cfg, blocked)
+    assert cl.debugStats()[1] > 0                                   # the cut came out of invalidateFailingEdges
+    start, count = b.meta["arc_start"], len(b.expected_cut)
+    # receivers are ring-0 positions, so the arc is receivers start .. start + count: one window across its edge, two inside it
+    inside = [(start + d) % n for d in (-SAMPLE // 2, SAMPLE, count // 2)]
+    windows = [1024 * 31 - SAMPLE // 2, 1024 * 62 - SAMPLE // 3] + [w0 for w0 in inside if w0 + SAMPLE <= n]
+    assert len(windows) >= 3
+    _, oview = _oracle_view(orc, n)
+    for w0 in windows:
+        _sampled_oracle_check(orc, rb, oview, cl, res, w0, b, cfg, blocked)
+    fp = rb.FastPaxos(cfg, n)
+    cl.clear()
+    cl.handleBatch(cfg, None, b.dst, b.ring, b.status, blocked=blocked, read_outputs=False)
+    t = fp.tallyCluster(cl)
+    assert t.decided and t.length == count and t.count == rb.quorum(n)
+
+
 def test_c4_hundred_thousand_nodes_flip_flop_stream(orc):
     import rapid_b200 as rb
     n = 100_000

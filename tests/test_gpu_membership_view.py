@@ -215,7 +215,7 @@ def test_apply_cut_with_node_ids_uuid_rule_and_device_config_id(orc, rb):
 
 @pytest.mark.parametrize("n", [1, 2, 4095, 4096, 4097, 20_000])
 def test_rings_from_the_hand_written_radix_sort(orc, rb, n):
-    """ring order = signed 64-bit key order, sizes around the sort's 4096-pair tile and several tiles (decoupled look-back)"""
+    """ring order = signed 64-bit key order, sizes around the sort's 4096-pair tile and several tiles"""
     w = OracleWorld(orc, n, K)
     v = rb.MembershipView.from_packed(K, *w.member_packed())
     for k in (0, K - 1):
