@@ -378,6 +378,24 @@ int32_t rapid_px_phase1b_from_acceptors(rapid_px* px, const rapid_pxa* a, uint64
 int32_t rapid_px_phase2b_from_acceptors(rapid_px* px, const rapid_pxa* a, uint64_t perm_seed, int32_t* decided,
                                         int64_t* decided_index, uint64_t* decided_hash, uint64_t* decided_hash2,
                                         int32_t* decided_len);
+/* The same over acceptor SHARDS: the answers of the n_shards handles listed (1..64 per rank, any order) and, with comm != NULL,
+ * of every other rank's shards, delivered as if one handle held the union of their acceptors: in ascending sender
+ * (perm_seed == 0) or in ascending splitmix64(perm_seed ^ sender) order.  Outputs, and the state the px keeps for later
+ * calls, are bit-identical to rapid_px_phase1b_from_acceptors / rapid_px_phase2b_from_acceptors on that one handle.
+ * comm == NULL: this process only.  comm != NULL: a collective call; every rank calls it with its own shards and every rank
+ * gets the same outputs (each holds a replica of the coordinator's / learner's tallies; O(N) bytes cross ranks: 32 B per
+ * Phase1b answer, 4 B per Phase2b answer).
+ * RAPID_EINVAL, on every rank alike and before any answer moves, if: a shard is NULL or n_shards is outside [1, 64]; acceptor
+ * ranges overlap; a shard has no answers of the wanted kind pending (last broadcast dropped for its configuration, or the
+ * other phase); shards answered different broadcasts (rank, configuration or Phase2a value); a shard lives on a device other
+ * than the px's.  A NULL px or a comm on another device than the px's is refused on that rank alone, without entering any
+ * collective.  A refused call leaves the px unchanged. */
+int32_t rapid_px_phase1b_from_acceptor_shards(rapid_px* px, const rapid_pxa* const* shards, int32_t n_shards, rapid_comm* comm,
+                                              uint64_t perm_seed, int32_t* proposed, int64_t* trigger_index, uint64_t* cval_hash,
+                                              uint64_t* cval_hash2, int32_t* cval_len, int64_t* n_messages);
+int32_t rapid_px_phase2b_from_acceptor_shards(rapid_px* px, const rapid_pxa* const* shards, int32_t n_shards, rapid_comm* comm,
+                                              uint64_t perm_seed, int32_t* decided, int64_t* decided_index, uint64_t* decided_hash,
+                                              uint64_t* decided_hash2, int32_t* decided_len);
 /* State of one acceptor: ranks[4] = rnd.round, rnd.node_index, vrnd.round, vrnd.node_index; its vval triple. */
 int32_t rapid_pxa_read(const rapid_pxa* a, int64_t acceptor, int32_t* ranks, uint64_t* hash, uint64_t* hash2, int32_t* len);
 

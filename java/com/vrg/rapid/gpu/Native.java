@@ -94,6 +94,9 @@ public final class Native {
     public static native long pxaPhase2a(long pxa, long msgCfg, int round, int nodeIndex, long hash, long hash2, int len);
     public static native int pxPhase1bFromAcceptors(long px, long pxa, long permSeed, long[] out6);
     public static native int pxPhase2bFromAcceptors(long px, long pxa, long permSeed, long[] out5);
+    /** the same over this rank's acceptor shards (and, comm != 0, every rank's: a collective call); outputs as above */
+    public static native int pxPhase1bFromAcceptorShards(long px, long[] pxaShards, long comm, long permSeed, long[] out6);
+    public static native int pxPhase2bFromAcceptorShards(long px, long[] pxaShards, long comm, long permSeed, long[] out5);
 
     // ---- wire-format ingest (rapid.proto bytes -> cells on the device) ----
     public static native long wireCreate(long view);

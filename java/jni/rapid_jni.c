@@ -437,6 +437,43 @@ JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_pxPhase2bFromAcceptors(JNIE
     (*env)->SetLongArrayRegion(env, out5, 0, 5, v);
     return rc;
 }
+/* jlong[] of handles -> rapid_pxa* array (malloc'ed; NULL if out of memory, which the entry point refuses as a NULL list) */
+static const rapid_pxa** shard_list(JNIEnv* env, jlongArray shards, jint* n) {
+    *n = (*env)->GetArrayLength(env, shards);
+    const rapid_pxa** out = (const rapid_pxa**)malloc(sizeof(rapid_pxa*) * (size_t)(*n > 0 ? *n : 1));
+    jlong* h = (*env)->GetLongArrayElements(env, shards, NULL);
+    for (jint i = 0; out && i < *n; ++i) out[i] = H(rapid_pxa, h[i]);
+    (*env)->ReleaseLongArrayElements(env, shards, h, JNI_ABORT);
+    return out;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_pxPhase1bFromAcceptorShards(JNIEnv* env, jclass c, jlong px, jlongArray shards, jlong comm,
+                                                                                  jlong seed, jlongArray out6) {
+    int32_t proposed = 0, clen = 0;
+    int64_t trigger = -1, total = 0;
+    uint64_t ca = 0, cb = 0;
+    jint n = 0;
+    const rapid_pxa** list = shard_list(env, shards, &n);
+    const int32_t rc = rapid_px_phase1b_from_acceptor_shards(H(rapid_px, px), list, n, H(rapid_comm, comm), (uint64_t)seed, &proposed,
+                                                             &trigger, &ca, &cb, &clen, &total);
+    free(list);
+    const jlong v[6] = {proposed, (jlong)trigger, (jlong)ca, (jlong)cb, clen, (jlong)total};
+    (*env)->SetLongArrayRegion(env, out6, 0, 6, v);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_pxPhase2bFromAcceptorShards(JNIEnv* env, jclass c, jlong px, jlongArray shards, jlong comm,
+                                                                                  jlong seed, jlongArray out5) {
+    int32_t decided = 0, dlen = 0;
+    int64_t at = -1;
+    uint64_t da = 0, db = 0;
+    jint n = 0;
+    const rapid_pxa** list = shard_list(env, shards, &n);
+    const int32_t rc = rapid_px_phase2b_from_acceptor_shards(H(rapid_px, px), list, n, H(rapid_comm, comm), (uint64_t)seed, &decided, &at,
+                                                             &da, &db, &dlen);
+    free(list);
+    const jlong v[5] = {decided, (jlong)at, (jlong)da, (jlong)db, dlen};
+    (*env)->SetLongArrayRegion(env, out5, 0, 5, v);
+    return rc;
+}
 
 /* ---------------------------------------------------------------- wire-format ingest (rapid.proto) */
 JNIEXPORT jlong JNICALL Java_com_vrg_rapid_gpu_Native_wireCreate(JNIEnv* env, jclass c, jlong view) {

@@ -1,11 +1,13 @@
 """Measure the classic-Paxos fallback (SURVEY.md §8 f2) at full size: one recovery round over N virtual nodes.
 
-    python profiles/bench_classic_paxos.py [--nodes 1000000] [--cpu-nodes 20000]
+    python profiles/bench_classic_paxos.py [--nodes 1000000] [--cpu-nodes 20000] [--shards W]
 
 GPU side: rapid_b200.PaxosAcceptors / Paxos through the C ABI (wall time of each call, which includes its host
 synchronisation, and the device time of the tally calls).  CPU side: the oracle's literal Paxos instances driven
 message by message (one acceptor object per node, one coordinator, one learner), on a smaller N, reported per message.
-Prints one JSON object."""
+--shards W also splits the N acceptors into W uneven local shards on the same GPU and reports the sharded tallies
+(Paxos.handlePhase1bFromAcceptorShards / handlePhase2bFromAcceptorShards, comm-less) next to the single-handle ones, each
+checked to give the single-handle result.  --cpu-nodes 0 skips the CPU side.  Prints one JSON object."""
 import argparse
 import json
 import os
@@ -18,13 +20,25 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def gpu_round(n, perm_seed):
+def gpu_round(n, perm_seed, n_shards=0):
     import rapid_b200 as rb
     acc = rb.PaxosAcceptors(9, n)
     ids = np.arange(n, dtype=np.int64)
     h = np.where(ids % 10 < 7, np.uint64(111), np.uint64(222)).astype(np.uint64)
     ln = np.full(n, 3, np.int32)
     out = {}
+    shards = []
+    if n_shards:
+        # uneven pieces (sizes proportional to 1, 2, ..., W), listed last piece first
+        w = np.arange(1, n_shards + 1, dtype=np.float64)
+        edges = np.concatenate([[0], np.round(np.cumsum(w) / w.sum() * n)]).astype(np.int64)
+        for a, b in zip(edges[:-1], edges[1:]):
+            s = rb.PaxosAcceptors(9, int(b - a), acceptor_begin=int(a))
+            s.registerFastRoundVotes(ids[a:b] - a, h[a:b], ln[a:b])
+            shards.append(s)
+        shards.reverse()
+        out["shard_sizes"] = [int(s.R) for s in shards]
+        sco, sle = rb.Paxos(9, n, message_capacity=n), rb.Paxos(9, n, message_capacity=n)
 
     def timed(name, fn):
         t0 = time.perf_counter()
@@ -46,6 +60,17 @@ def gpu_round(n, perm_seed):
         d = timed("learner_phase2b", lambda: le.handlePhase2bFromAcceptors(acc, perm_seed))
         out["learner_phase2b_device_ms"] = le.lastDeviceMs()
         assert d.decided and d.decided_index == n // 2 and d.decision == p.cval
+        if shards:
+            sco.reset(9); sle.reset(9)
+            sco.startPhase1a(2 + rep, 1)
+            assert sum(s.handlePhase1aMessage((2 + rep, 1)) for s in shards) == n
+            sp = timed("sharded_coordinator_phase1b", lambda: sco.handlePhase1bFromAcceptorShards(shards, perm_seed=perm_seed))
+            out["sharded_coordinator_phase1b_device_ms"] = sco.lastDeviceMs()
+            assert (sp.proposed, sp.trigger_index, sp.cval, sp.n_messages) == (p.proposed, p.trigger_index, p.cval, p.n_messages)
+            assert sum(s.handlePhase2aMessage((2 + rep, 1), p.cval) for s in shards) == n
+            sd = timed("sharded_learner_phase2b", lambda: sle.handlePhase2bFromAcceptorShards(shards, perm_seed=perm_seed))
+            out["sharded_learner_phase2b_device_ms"] = sle.lastDeviceMs()
+            assert (sd.decided, sd.decided_index, sd.decision) == (d.decided, d.decided_index, d.decision)
     out["round_ms"] = sum(out[k] for k in ("acceptors_phase1a_ms", "coordinator_phase1b_ms", "acceptors_phase2a_ms", "learner_phase2b_ms"))
     out["messages"] = 4 * n                                    # N x (1a delivery, 1b, 2a delivery, 2b at one learner)
     out["messages_per_s"] = out["messages"] / (out["round_ms"] * 1e-3)
@@ -88,9 +113,12 @@ def main():
     ap.add_argument("--nodes", type=int, default=1_000_000)
     ap.add_argument("--cpu-nodes", type=int, default=20_000)
     ap.add_argument("--perm-seed", type=int, default=12345)
+    ap.add_argument("--shards", type=int, default=0)
     args = ap.parse_args()
-    res = {"nodes": args.nodes, "gpu": gpu_round(args.nodes, args.perm_seed), "gpu_acceptor_order": gpu_round(args.nodes, 0),
-           "cpu_oracle": cpu_round(args.cpu_nodes)}
+    res = {"nodes": args.nodes, "shards": args.shards, "gpu": gpu_round(args.nodes, args.perm_seed, args.shards),
+           "gpu_acceptor_order": gpu_round(args.nodes, 0, args.shards)}
+    if args.cpu_nodes > 0:
+        res["cpu_oracle"] = cpu_round(args.cpu_nodes)
     print(json.dumps(res, indent=1))
 
 

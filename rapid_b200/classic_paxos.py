@@ -4,7 +4,9 @@ by librapid_b200.so on the GPU (csrc/classic_paxos.cu).
 Paxos            one node's coordinator + learner tallies (handlePhase1bMessage :159-191, handlePhase2bMessage :223-236,
                  selectProposalUsingCoordinatorRule :271-328), batches of messages in arrival order.
 PaxosAcceptors   the acceptor registers (rnd, vrnd, vval) of R virtual nodes (handlePhase1aMessage :120-151,
-                 handlePhase2aMessage :198-216, registerFastRoundVote :244-257).
+                 handlePhase2aMessage :198-216, registerFastRoundVote :244-257).  Several of them with disjoint
+                 acceptor_begin ranges, on one GPU or on every rank of an NcclComm, feed one Paxos through
+                 Paxos.handlePhase1bFromAcceptorShards / handlePhase2bFromAcceptorShards, as one handle over their union would.
 
 A value (List<Endpoint>) is an opaque (hash, hash2, len) triple; len == 0 is the empty list.  A rank is (round, nodeIndex).
 """
@@ -140,6 +142,27 @@ class Paxos:
     def handlePhase2bFromAcceptors(self, acceptors, perm_seed=0):
         o = self._p2_outs()
         N.check(N.lib().rapid_px_phase2b_from_acceptors(self._h, acceptors._h, int(perm_seed), *[C.byref(x) for x in o]))
+        return self._p2_result(o)
+
+    @staticmethod
+    def _shard_handles(shards):
+        return (C.c_void_p * max(len(shards), 1))(*[s._h.value for s in shards])
+
+    def handlePhase1bFromAcceptorShards(self, shards, comm=None, perm_seed=0):
+        """handlePhase1bFromAcceptors over the union of several PaxosAcceptors shards (any order, disjoint ranges); with an
+        NcclComm, a collective call over every rank's shards that gives every rank the same result"""
+        o = self._p1_outs()
+        N.check(N.lib().rapid_px_phase1b_from_acceptor_shards(self._h, self._shard_handles(shards), len(shards),
+                                                              None if comm is None else comm._h, int(perm_seed),
+                                                              *[C.byref(x) for x in o]))
+        return self._p1_result(o)
+
+    def handlePhase2bFromAcceptorShards(self, shards, comm=None, perm_seed=0):
+        """handlePhase2bFromAcceptors over the union of several PaxosAcceptors shards, as handlePhase1bFromAcceptorShards"""
+        o = self._p2_outs()
+        N.check(N.lib().rapid_px_phase2b_from_acceptor_shards(self._h, self._shard_handles(shards), len(shards),
+                                                              None if comm is None else comm._h, int(perm_seed),
+                                                              *[C.byref(x) for x in o]))
         return self._p2_result(o)
 
     def lastDeviceMs(self):

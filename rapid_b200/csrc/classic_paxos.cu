@@ -4,14 +4,18 @@
 //   * the coordinator rule (selectProposalUsingCoordinatorRule :271-328): max rank -> collect -> distinct values ->
 //     "first value whose (N/4+1)-th occurrence comes earliest in arrival order" -> first non-empty fallback;
 //   * the coordinator's Phase1b list (:159-191) and the learner's Phase2b sets (:223-236), one node's worth (rapid_px);
-//   * the acceptor registers rnd / vrnd / vval of R virtual nodes (:120-151, :198-216, :244-257) (rapid_pxa).
+//   * the acceptor registers rnd / vrnd / vval of R virtual nodes (:120-151, :198-216, :244-257) (rapid_pxa), whose answers
+//     feed the tallies from one handle or, gathered in ascending acceptor_begin, from several shards on one GPU or across ranks.
 // "k-th occurrence of a key in arrival order" is the one shared primitive: stable radix sort of (key, arrival index),
 // then the element at offset k of each key's run.  Everything is exact; nothing depends on thread scheduling.
 #include <limits.h>
 
 
+#include <algorithm>
+
 #include "cd_internal.cuh"
 #include "common.cuh"
+#include "nccl_api.cuh"
 #include "radix.cuh"
 #include "scan.cuh"
 
@@ -355,6 +359,8 @@ __global__ void k_px_gather(int64_t n, const int32_t* __restrict__ order, const 
 }
 
 // ------------------------------------------------------------------ handles
+struct PxSeg;
+struct PxRankHdr;
 struct PX {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -393,6 +399,17 @@ struct PX {
     DevBuf<uint64_t> pkey, spkey, g_h1, g_h2;
     DevBuf<int64_t> g_vr;
     DevBuf<int32_t> g_len, g_sender;
+    // answers gathered from acceptor shards (ascending sender), and the exchange that brings them
+    DevBuf<int32_t> sh_sender, sh_len;
+    DevBuf<int64_t> sh_vr;
+    DevBuf<uint64_t> sh_h1, sh_h2;
+    DevBuf<unsigned char> stage, recv;     // this rank's packed answers / every rank's
+    DevBuf<PxSeg> seg;
+    PinnedBuf<PxSeg> h_seg;
+    DevBuf<PxRankHdr> d_hdr;
+    PinnedBuf<PxRankHdr> h_hdr;
+    DevBuf<int32_t> d_ok;
+    PinnedBuf<int32_t> h_ok;
 };
 
 struct PXA {
@@ -568,22 +585,111 @@ static int32_t check_device(int32_t device) {
     return RAPID_OK;
 }
 
-// arrival order of the acceptors' answers: order[i] = answer position delivered i-th (NULL = as compacted)
-static int32_t px_arrival_order(PX* px, const PXA* a, uint64_t perm_seed, const int32_t** order) {
+// arrival order of n compacted answers (sender ascending): order[i] = answer position delivered i-th (NULL = as compacted);
+// with an order, px->g_sender holds the senders in arrival order
+static int32_t px_arrival_order(PX* px, const int32_t* sender, int64_t n, uint64_t perm_seed, const int32_t** order) {
     *order = nullptr;
-    const int64_t n = a->n_out;
     if (perm_seed == 0 || n <= 1) return RAPID_OK;
     cudaStream_t s = px->stream;
     RAPID_CHECK(px->pkey.reserve((size_t)n)); RAPID_CHECK(px->spkey.reserve((size_t)n));
     RAPID_CHECK(px->idx.reserve((size_t)n)); RAPID_CHECK(px->sidx.reserve((size_t)n));
-    k_px_perm_keys<<<grid_for(n), TB, 0, s>>>(n, a->o_sender.p, perm_seed, px->pkey.p, px->idx.p);
+    k_px_perm_keys<<<grid_for(n), TB, 0, s>>>(n, sender, perm_seed, px->pkey.p, px->idx.p);
     RAPID_KERNEL_CHECK();
     RAPID_CHECK(radix_sort_pairs<uint64_t>(px->rs, px->pkey.p, px->idx.p, px->spkey.p, px->sidx.p, n, 0, 64, s, false));
     RAPID_CHECK(px->g_sender.reserve((size_t)n));
-    k_px_gather<int32_t><<<grid_for(n), TB, 0, s>>>(n, px->sidx.p, a->o_sender.p, px->g_sender.p);
+    k_px_gather<int32_t><<<grid_for(n), TB, 0, s>>>(n, px->sidx.p, sender, px->g_sender.p);
     RAPID_KERNEL_CHECK();
     *order = px->sidx.p;      // NOTE: valid until the next sort on this handle; callers gather before tallying
     return RAPID_OK;
+}
+
+// handlePhase1bMessage for n compacted Phase1b answers (sender ascending) to the broadcast of `rank`, delivered in acceptor
+// order or in the perm_seed order
+static int32_t px_answers_1b(PX* px, int64_t n, int64_t rank, const int32_t* sender, const int64_t* vr, const uint64_t* h1,
+                             const uint64_t* h2, const int32_t* len, uint64_t perm_seed, int32_t* proposed, int64_t* trigger_index,
+                             uint64_t* cval_hash, uint64_t* cval_hash2, int32_t* cval_len, int64_t* n_messages) {
+    cudaStream_t s = px->stream;
+    if (n > 0) {
+        const int32_t* order = nullptr;
+        RAPID_CHECK(px_arrival_order(px, sender, n, perm_seed, &order));
+        if (order) {
+            RAPID_CHECK(px->g_vr.reserve((size_t)n)); RAPID_CHECK(px->g_h1.reserve((size_t)n));
+            RAPID_CHECK(px->g_h2.reserve((size_t)n)); RAPID_CHECK(px->g_len.reserve((size_t)n));
+            k_px_gather<int64_t><<<grid_for(n), TB, 0, s>>>(n, order, vr, px->g_vr.p);
+            k_px_gather<uint64_t><<<grid_for(n), TB, 0, s>>>(n, order, h1, px->g_h1.p);
+            k_px_gather<uint64_t><<<grid_for(n), TB, 0, s>>>(n, order, h2, px->g_h2.p);
+            k_px_gather<int32_t><<<grid_for(n), TB, 0, s>>>(n, order, len, px->g_len.p);
+            RAPID_KERNEL_CHECK();
+            vr = px->g_vr.p; h1 = px->g_h1.p; h2 = px->g_h2.p; len = px->g_len.p;
+        }
+    }
+    return px_phase1b_device(px, n, nullptr, nullptr, rank, vr, h1, h2, len, proposed, trigger_index, cval_hash, cval_hash2, cval_len,
+                             n_messages);
+}
+
+// handlePhase2bMessage for n compacted Phase2b broadcasts (sender ascending) of the value (h1, h2, len) in round `rank`
+static int32_t px_answers_2b(PX* px, int64_t n, int64_t rank, const int32_t* sender, uint64_t h1, uint64_t h2, int32_t len,
+                             uint64_t perm_seed, int32_t* decided, int64_t* decided_index, uint64_t* decided_hash,
+                             uint64_t* decided_hash2, int32_t* decided_len) {
+    if (n > 0) {
+        const int32_t* order = nullptr;
+        RAPID_CHECK(px_arrival_order(px, sender, n, perm_seed, &order));
+        if (order) sender = px->g_sender.p;
+    }
+    return px_phase2b_device(px, n, nullptr, nullptr, rank, sender, nullptr, nullptr, nullptr, h1, h2, len, decided, decided_index,
+                             decided_hash, decided_hash2, decided_len);
+}
+
+// ------------------------------------------------------------------ answers of several acceptor shards
+// Every shard (on every rank) contributes one fixed header; the gathered table is validated identically everywhere before any
+// answer moves, then the compacted answers are packed, all-gathered and unpacked in ascending acceptor_begin, which for
+// disjoint shards is exactly the compaction order (ascending sender) of one handle over their union.
+static const int PX_MAX_SHARDS = 64;        // per rank: the header exchange has a fixed size
+
+struct PxShardHdr {
+    int64_t begin, R, n_out, last_rank, cfg;
+    uint64_t h1, h2;                        // the Phase2a value (Phase2b answers only)
+    int32_t len, kind, on_px_device, pad_;
+};
+struct PxRankHdr {
+    int32_t n_shards, bad, want, pad_;      // bad: NULL shard or n_shards outside [1, PX_MAX_SHARDS]; want: 1 Phase1b, 2 Phase2b
+    PxShardHdr s[PX_MAX_SHARDS];
+};
+struct __align__(16) Px1bRec {              // one Phase1b answer in the exchange: 32 B
+    int32_t sender, len;
+    int64_t vr;
+    uint64_t h1, h2;
+};
+struct PxSeg { int64_t dst, src, n; };     // answers [dst, dst + n) of the gathered arrays come from records [src, src + n)
+
+__global__ void k_px_pack1b(int64_t n, const int32_t* __restrict__ sender, const int64_t* __restrict__ vr, const uint64_t* __restrict__ h1,
+                            const uint64_t* __restrict__ h2, const int32_t* __restrict__ len, Px1bRec* __restrict__ out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Px1bRec r;
+    r.sender = sender[i]; r.len = len[i]; r.vr = vr[i]; r.h1 = h1[i]; r.h2 = h2[i];
+    out[i] = r;
+}
+__device__ __forceinline__ int32_t px_seg_of(const PxSeg* __restrict__ seg, int32_t nseg, int64_t j) {
+    int32_t lo = 0, hi = nseg - 1;                           // last segment with dst <= j (segments are non-empty and ascending)
+    while (lo < hi) { const int32_t mid = (lo + hi + 1) >> 1; if (seg[mid].dst <= j) lo = mid; else hi = mid - 1; }
+    return lo;
+}
+__global__ void k_px_unpack1b(int64_t n, const PxSeg* __restrict__ seg, int32_t nseg, const Px1bRec* __restrict__ in,
+                              int32_t* __restrict__ sender, int64_t* __restrict__ vr, uint64_t* __restrict__ h1,
+                              uint64_t* __restrict__ h2, int32_t* __restrict__ len) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const PxSeg g = seg[px_seg_of(seg, nseg, j)];
+    const Px1bRec r = in[g.src + (j - g.dst)];
+    sender[j] = r.sender; vr[j] = r.vr; h1[j] = r.h1; h2[j] = r.h2; len[j] = r.len;
+}
+__global__ void k_px_unpack2b(int64_t n, const PxSeg* __restrict__ seg, int32_t nseg, const int32_t* __restrict__ in,
+                              int32_t* __restrict__ sender) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const PxSeg g = seg[px_seg_of(seg, nseg, j)];
+    sender[j] = in[g.src + (j - g.dst)];
 }
 
 static int32_t px_clear_tables(PX* px) {
@@ -598,6 +704,136 @@ using namespace rapid;
 
 struct rapid_px : rapid::PX {};
 struct rapid_pxa : rapid::PXA {};
+
+// Gather the pending answers of `want` kind (1 Phase1b, 2 Phase2b) of this rank's shards and, with a comm, of every rank's into
+// px->sh_* in ascending sender.  Every refusal that depends on the shards is decided from the gathered header table, which is
+// the same on every rank, so either every rank returns it or every rank goes on to the data exchange.  Outputs: the number of
+// answers, the rank of the broadcast they answer and (Phase2b) its value.
+static int32_t px_gather_shards(rapid_px* px, const rapid_pxa* const* shards, int32_t n_shards, rapid_comm* comm, int want,
+                                int64_t* n_total, int64_t* rank, uint64_t* h1, uint64_t* h2, int32_t* len) {
+    cudaStream_t s = px->stream;
+    const int world = comm ? comm->world : 1, me = comm ? comm->rank : 0;
+    if (comm && !g_nccl.AllGather) { set_error("libnccl lacks ncclAllGather"); return RAPID_ENCCL; }
+    // 1. headers
+    RAPID_CHECK(px->h_hdr.reserve((size_t)world));
+    PxRankHdr& mine = px->h_hdr.p[me];
+    memset(&mine, 0, sizeof(mine));
+    mine.want = want;
+    if (!shards || n_shards < 1 || n_shards > PX_MAX_SHARDS) mine.bad = 1;
+    else {
+        mine.n_shards = n_shards;
+        for (int32_t i = 0; i < n_shards; ++i) {
+            const rapid_pxa* a = shards[i];
+            if (!a) { mine.bad = 1; break; }
+            PxShardHdr& h = mine.s[i];
+            h.begin = a->begin; h.R = a->R; h.n_out = a->n_out; h.last_rank = a->last_rank; h.cfg = a->cfg;
+            h.kind = a->last_kind; h.on_px_device = a->device == px->device ? 1 : 0;
+            if (a->last_kind == 2) { h.h1 = a->last_h1; h.h2 = a->last_h2; h.len = a->last_len; }
+        }
+    }
+    if (comm) {
+        RAPID_CHECK(px->d_hdr.reserve((size_t)world)); RAPID_CHECK(px->d_ok.reserve(1)); RAPID_CHECK(px->h_ok.reserve(1));
+        RAPID_CUDA(cudaMemcpyAsync(px->d_hdr.p + me, &mine, sizeof(PxRankHdr), cudaMemcpyHostToDevice, s));
+        RAPID_NCCL(g_nccl.AllGather(px->d_hdr.p + me, px->d_hdr.p, sizeof(PxRankHdr), NCCL_UINT8, comm->comm, s));
+        RAPID_CUDA(cudaMemcpyAsync(px->h_hdr.p, px->d_hdr.p, (size_t)world * sizeof(PxRankHdr), cudaMemcpyDeviceToHost, s));
+        RAPID_CUDA(cudaStreamSynchronize(s));
+    }
+    // 2. validate the gathered table (identical on every rank) and place every shard's answers
+    struct Ent { int64_t begin, R, n_out, src; int r; };
+    std::vector<Ent> all;
+    std::vector<int64_t> rank_total((size_t)world, 0);
+    const PxShardHdr* ref = nullptr;
+    for (int r = 0; r < world; ++r) {
+        const PxRankHdr& h = px->h_hdr.p[r];
+        if (h.bad) { set_error("rank %d passed a NULL shard or n_shards outside [1, %d]", r, PX_MAX_SHARDS); return RAPID_EINVAL; }
+        if (h.want != want) { set_error("ranks disagree on the tally: rank %d asked for Phase%db answers", r, h.want); return RAPID_EINVAL; }
+        for (int32_t i = 0; i < h.n_shards; ++i) {
+            const PxShardHdr& x = h.s[i];
+            if (!x.on_px_device) { set_error("shard %d of rank %d lives on a device other than the px's", i, r); return RAPID_EINVAL; }
+            if (x.kind != want) {
+                if (want == 1) set_error("no Phase1b answers pending on shard %d of rank %d (call rapid_pxa_phase1a first)", i, r);
+                else set_error("no Phase2b broadcasts pending on shard %d of rank %d (call rapid_pxa_phase2a first)", i, r);
+                return RAPID_EINVAL;
+            }
+            if (!ref) ref = &x;
+            else if (x.last_rank != ref->last_rank || x.cfg != ref->cfg || x.h1 != ref->h1 || x.h2 != ref->h2 || x.len != ref->len) {
+                set_error("shard %d of rank %d answered a different broadcast (rank, configuration or Phase2a value)", i, r);
+                return RAPID_EINVAL;
+            }
+            all.push_back({x.begin, x.R, x.n_out, rank_total[(size_t)r], r});
+            rank_total[(size_t)r] += x.n_out;
+        }
+    }
+    std::sort(all.begin(), all.end(), [](const Ent& a, const Ent& b) { return a.begin < b.begin; });
+    for (size_t k = 1; k < all.size(); ++k)
+        if (all[k - 1].begin + all[k - 1].R > all[k].begin) {
+            set_error("acceptor ranges overlap: [%lld, %lld) and [%lld, %lld)", (long long)all[k - 1].begin,
+                      (long long)(all[k - 1].begin + all[k - 1].R), (long long)all[k].begin, (long long)(all[k].begin + all[k].R));
+            return RAPID_EINVAL;
+        }
+    const int64_t per_rank = *std::max_element(rank_total.begin(), rank_total.end());   // padded block of every rank
+    int64_t n = 0;
+    for (const Ent& e : all) n += e.n_out;
+    const size_t rec = want == 1 ? sizeof(Px1bRec) : sizeof(int32_t);
+    // 3. scratch for the gathered sizes; with a comm every rank learns whether every rank has it before the data moves
+    const size_t nn = (size_t)std::max<int64_t>(n, 1), nseg = std::max<size_t>(all.size(), 1);
+    const size_t block = (size_t)std::max<int64_t>(per_rank, 1) * rec;
+    int32_t rc = px->stage.reserve(block);
+    if (!rc && comm) rc = px->recv.reserve((size_t)world * block);
+    if (!rc) rc = px->sh_sender.reserve(nn);
+    if (!rc && want == 1) rc = px->sh_vr.reserve(nn);
+    if (!rc && want == 1) rc = px->sh_h1.reserve(nn);
+    if (!rc && want == 1) rc = px->sh_h2.reserve(nn);
+    if (!rc && want == 1) rc = px->sh_len.reserve(nn);
+    if (!rc) rc = px->seg.reserve(nseg);
+    if (!rc) rc = px->h_seg.reserve(nseg);
+    if (comm) {
+        *px->h_ok.p = rc == RAPID_OK ? 1 : 0;
+        RAPID_CUDA(cudaMemcpyAsync(px->d_ok.p, px->h_ok.p, sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        RAPID_NCCL(g_nccl.AllReduce(px->d_ok.p, px->d_ok.p, 1, NCCL_INT32, NCCL_MIN, comm->comm, s));
+        RAPID_CUDA(cudaMemcpyAsync(px->h_ok.p, px->d_ok.p, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+        RAPID_CUDA(cudaStreamSynchronize(s));
+        if (rc == RAPID_OK && !*px->h_ok.p) { set_error("another rank could not allocate the exchange buffers"); return RAPID_ENOMEM; }
+    }
+    RAPID_CHECK(rc);
+    // 4. pack this rank's answers (list order), exchange, unpack in ascending acceptor_begin
+    int64_t off = 0;
+    for (int32_t i = 0; i < n_shards; ++i) {
+        const rapid_pxa* a = shards[i];
+        const int64_t m = a->n_out;
+        if (m > 0 && want == 1) {
+            k_px_pack1b<<<grid_for(m), TB, 0, s>>>(m, a->o_sender.p, a->o_vr.p, a->o_h1.p, a->o_h2.p, a->o_len.p, (Px1bRec*)px->stage.p + off);
+            RAPID_KERNEL_CHECK();
+        } else if (m > 0) {                                  // Phase2b: the sender is the whole answer
+            RAPID_CUDA(cudaMemcpyAsync((int32_t*)px->stage.p + off, a->o_sender.p, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+        }
+        off += m;
+    }
+    const unsigned char* in = px->stage.p;
+    if (comm && per_rank > 0) {
+        RAPID_NCCL(g_nccl.AllGather(px->stage.p, px->recv.p, (size_t)per_rank * rec, NCCL_UINT8, comm->comm, s));
+        in = px->recv.p;
+    }
+    int32_t k = 0;
+    int64_t dst = 0;
+    for (const Ent& e : all) {
+        if (e.n_out == 0) continue;
+        px->h_seg.p[k++] = PxSeg{dst, (comm ? (int64_t)e.r * per_rank : 0) + e.src, e.n_out};
+        dst += e.n_out;
+    }
+    if (n > 0) {
+        RAPID_CUDA(cudaMemcpyAsync(px->seg.p, px->h_seg.p, (size_t)k * sizeof(PxSeg), cudaMemcpyHostToDevice, s));
+        if (want == 1)
+            k_px_unpack1b<<<grid_for(n), TB, 0, s>>>(n, px->seg.p, k, (const Px1bRec*)in, px->sh_sender.p, px->sh_vr.p, px->sh_h1.p,
+                                                      px->sh_h2.p, px->sh_len.p);
+        else
+            k_px_unpack2b<<<grid_for(n), TB, 0, s>>>(n, px->seg.p, k, (const int32_t*)in, px->sh_sender.p);
+        RAPID_KERNEL_CHECK();
+    }
+    *n_total = n;
+    *rank = ref->last_rank; *h1 = ref->h1; *h2 = ref->h2; *len = ref->len;
+    return RAPID_OK;
+}
 
 extern "C" {
 
@@ -872,24 +1108,8 @@ int32_t rapid_px_phase1b_from_acceptors(rapid_px* px, const rapid_pxa* a, uint64
     DeviceGuard g(px->device);
     cudaStream_t s = px->stream;
     RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    const int64_t n = a->n_out;
-    const int32_t* order = nullptr;
-    const int64_t* vr = a->o_vr.p; const uint64_t* h1 = a->o_h1.p; const uint64_t* h2 = a->o_h2.p; const int32_t* len = a->o_len.p;
-    if (n > 0) {
-        RAPID_CHECK(px_arrival_order(px, a, perm_seed, &order));
-        if (order) {
-            RAPID_CHECK(px->g_vr.reserve((size_t)n)); RAPID_CHECK(px->g_h1.reserve((size_t)n));
-            RAPID_CHECK(px->g_h2.reserve((size_t)n)); RAPID_CHECK(px->g_len.reserve((size_t)n));
-            k_px_gather<int64_t><<<grid_for(n), TB, 0, s>>>(n, order, a->o_vr.p, px->g_vr.p);
-            k_px_gather<uint64_t><<<grid_for(n), TB, 0, s>>>(n, order, a->o_h1.p, px->g_h1.p);
-            k_px_gather<uint64_t><<<grid_for(n), TB, 0, s>>>(n, order, a->o_h2.p, px->g_h2.p);
-            k_px_gather<int32_t><<<grid_for(n), TB, 0, s>>>(n, order, a->o_len.p, px->g_len.p);
-            RAPID_KERNEL_CHECK();
-            vr = px->g_vr.p; h1 = px->g_h1.p; h2 = px->g_h2.p; len = px->g_len.p;
-        }
-    }
-    const int32_t rc = px_phase1b_device(px, n, nullptr, nullptr, a->last_rank, vr, h1, h2, len, proposed, trigger_index, cval_hash, cval_hash2,
-                                         cval_len, n_messages);
+    const int32_t rc = px_answers_1b(px, a->n_out, a->last_rank, a->o_sender.p, a->o_vr.p, a->o_h1.p, a->o_h2.p, a->o_len.p, perm_seed,
+                                     proposed, trigger_index, cval_hash, cval_hash2, cval_len, n_messages);
     if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
     return rc;
 }
@@ -902,15 +1122,44 @@ int32_t rapid_px_phase2b_from_acceptors(rapid_px* px, const rapid_pxa* a, uint64
     DeviceGuard g(px->device);
     cudaStream_t s = px->stream;
     RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    const int64_t n = a->n_out;
-    const int32_t* order = nullptr;
-    const int32_t* sender = a->o_sender.p;
-    if (n > 0) {
-        RAPID_CHECK(px_arrival_order(px, a, perm_seed, &order));
-        if (order) sender = px->g_sender.p;
-    }
-    const int32_t rc = px_phase2b_device(px, n, nullptr, nullptr, a->last_rank, sender, nullptr, nullptr, nullptr, a->last_h1, a->last_h2,
-                                         a->last_len, decided, decided_index, decided_hash, decided_hash2, decided_len);
+    const int32_t rc = px_answers_2b(px, a->n_out, a->last_rank, a->o_sender.p, a->last_h1, a->last_h2, a->last_len, perm_seed, decided,
+                                     decided_index, decided_hash, decided_hash2, decided_len);
+    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
+    return rc;
+}
+
+int32_t rapid_px_phase1b_from_acceptor_shards(rapid_px* px, const rapid_pxa* const* shards, int32_t n_shards, rapid_comm* comm,
+                                              uint64_t perm_seed, int32_t* proposed, int64_t* trigger_index, uint64_t* cval_hash,
+                                              uint64_t* cval_hash2, int32_t* cval_len, int64_t* n_messages) {
+    if (!px) { set_error("NULL handle"); return RAPID_EINVAL; }
+    if (comm && comm->device != px->device) { set_error("comm and px live on different devices"); return RAPID_EINVAL; }
+    DeviceGuard g(px->device);
+    cudaStream_t s = px->stream;
+    RAPID_CUDA(cudaEventRecord(px->ev0, s));
+    int64_t n = 0, rank = 0;
+    uint64_t h1 = 0, h2 = 0;
+    int32_t len = 0;
+    RAPID_CHECK(px_gather_shards(px, shards, n_shards, comm, 1, &n, &rank, &h1, &h2, &len));
+    const int32_t rc = px_answers_1b(px, n, rank, px->sh_sender.p, px->sh_vr.p, px->sh_h1.p, px->sh_h2.p, px->sh_len.p, perm_seed, proposed,
+                                     trigger_index, cval_hash, cval_hash2, cval_len, n_messages);
+    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
+    return rc;
+}
+
+int32_t rapid_px_phase2b_from_acceptor_shards(rapid_px* px, const rapid_pxa* const* shards, int32_t n_shards, rapid_comm* comm,
+                                              uint64_t perm_seed, int32_t* decided, int64_t* decided_index, uint64_t* decided_hash,
+                                              uint64_t* decided_hash2, int32_t* decided_len) {
+    if (!px) { set_error("NULL handle"); return RAPID_EINVAL; }
+    if (comm && comm->device != px->device) { set_error("comm and px live on different devices"); return RAPID_EINVAL; }
+    DeviceGuard g(px->device);
+    cudaStream_t s = px->stream;
+    RAPID_CUDA(cudaEventRecord(px->ev0, s));
+    int64_t n = 0, rank = 0;
+    uint64_t h1 = 0, h2 = 0;
+    int32_t len = 0;
+    RAPID_CHECK(px_gather_shards(px, shards, n_shards, comm, 2, &n, &rank, &h1, &h2, &len));
+    const int32_t rc = px_answers_2b(px, n, rank, px->sh_sender.p, h1, h2, len, perm_seed, decided, decided_index, decided_hash,
+                                     decided_hash2, decided_len);
     if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
     return rc;
 }

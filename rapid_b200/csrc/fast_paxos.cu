@@ -15,6 +15,7 @@
 #include <cstdlib>
 
 #include "cd_internal.cuh"
+#include "nccl_api.cuh"
 #include "scan.cuh"
 
 namespace cg = cooperative_groups;
@@ -76,21 +77,10 @@ struct FP {
     int32_t last_launches = 0;
 };
 
-// ------------------------------------------------------------------ NCCL through dlopen
-typedef struct { char internal[128]; } nccl_uid;
-typedef void* nccl_comm;
-struct NcclApi {
-    void* lib = nullptr;
-    int (*GetUniqueId)(nccl_uid*) = nullptr;
-    int (*CommInitRank)(nccl_comm*, int, nccl_uid, int) = nullptr;
-    int (*CommDestroy)(nccl_comm) = nullptr;
-    int (*AllReduce)(const void*, void*, size_t, int, int, nccl_comm, cudaStream_t) = nullptr;
-    const char* (*GetErrorString)(int) = nullptr;
-};
-static NcclApi g_nccl;
-static const int NCCL_INT32 = 2, NCCL_UINT64 = 5, NCCL_SUM = 0, NCCL_MAX = 2;
+// ------------------------------------------------------------------ NCCL through dlopen (nccl_api.cuh)
+NcclApi g_nccl;
 
-static int32_t load_nccl() {
+int32_t load_nccl() {
     if (g_nccl.lib) return RAPID_OK;
     const char* names[] = {"libnccl.so.2", "libnccl.so"};
     void* h = nullptr;
@@ -102,22 +92,12 @@ static int32_t load_nccl() {
     a.CommInitRank = (int (*)(nccl_comm*, int, nccl_uid, int))dlsym(h, "ncclCommInitRank");
     a.CommDestroy = (int (*)(nccl_comm))dlsym(h, "ncclCommDestroy");
     a.AllReduce = (int (*)(const void*, void*, size_t, int, int, nccl_comm, cudaStream_t))dlsym(h, "ncclAllReduce");
+    a.AllGather = (int (*)(const void*, void*, size_t, int, nccl_comm, cudaStream_t))dlsym(h, "ncclAllGather");
     a.GetErrorString = (const char* (*)(int))dlsym(h, "ncclGetErrorString");
     if (!a.GetUniqueId || !a.CommInitRank || !a.CommDestroy || !a.AllReduce) { set_error("libnccl lacks required symbols"); return RAPID_ENCCL; }
     g_nccl = a;
     return RAPID_OK;
 }
-
-struct Comm {
-    int device = 0, rank = 0, world = 1;
-    nccl_comm comm = nullptr;
-};
-
-#define RAPID_NCCL(call)                                                                                              \
-    do {                                                                                                              \
-        int _r = (call);                                                                                              \
-        if (_r != 0) { set_error("NCCL error %d (%s): %s", _r, g_nccl.GetErrorString ? g_nccl.GetErrorString(_r) : "?", #call); return RAPID_ENCCL; } \
-    } while (0)
 
 // ------------------------------------------------------------------ kernels
 // a new FastPaxos instance on the same buffers, one launch
@@ -901,7 +881,6 @@ static int32_t read_result(FP* fp, int32_t* decided, uint64_t* dh1, uint64_t* dh
 using namespace rapid;
 
 struct rapid_fp : rapid::FP {};
-struct rapid_comm : rapid::Comm {};
 
 extern "C" {
 
