@@ -248,6 +248,9 @@ int32_t rapid_cd_last_path(const rapid_cd* cd, int32_t* path, int32_t* n_kernel_
  * invalidation work list, distinct subjects and valid cells of the batch. */
 int32_t rapid_cd_debug_stats(const rapid_cd* cd, int32_t* n_mixed, int32_t* n_inval_pairs, int32_t* n_batch_subjects,
                              int32_t* n_valid_cells);
+/* Bucketed handles, last batch: the subject chunks of the apply kernel's grid (RAPID_B200_CHUNKS overrides the host's choice)
+ * and the blocks of k_prepare's cooperative grid (RAPID_B200_PREP_GRID).  A sweep handle reports 0 chunks. */
+int32_t rapid_cd_debug_grid(const rapid_cd* cd, int32_t* apply_chunks, int32_t* prepare_blocks);
 
 /* RAW mode (RAPID_CD_RAW handles): the bare detector API the reference's CutDetectionTest drives.
  * aggregateForProposal(AlertMessage) :76-82 for every receiver (no filter, no announced gating); returns the

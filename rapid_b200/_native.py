@@ -75,6 +75,7 @@ SIGNATURES = {
     "rapid_view_set_joiner_ids": [_vp, _i32, _i64, _p, _p],
     "rapid_view_current_config_id": [_vp, _p],
     "rapid_cd_debug_stats": [_vp, _p, _p, _p, _p],
+    "rapid_cd_debug_grid": [_vp, _p, _p],
     "rapid_cd_create": [_pp, _vp, _i32, _i32, _i64, _i64, _u32, _i64],
     "rapid_cd_destroy": [_vp],
     "rapid_cd_apply_batch": [_vp, _i64, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p],

@@ -95,16 +95,24 @@ constexpr uint32_t MX_TIME = 16u;     // PERMUTED delivery: the classification n
 constexpr uint32_t PF_SEEN = 1u;      // a valid DOWN cell was delivered
 constexpr uint32_t PF_NEGINF = 2u;    // a subject already in the unstable band stayed there (its t_L is "before the batch")
 
+// Counts are full 32-bit words wherever they sum over more than one stage of subjects: a chunk (or a whole batch) can hold
+// 65,536 subjects or more.  The 16-bit halves of StageAcc only ever hold the sum over one stage (at most STAGE subjects).
 struct ChunkAcc {                     // what the FRESH subjects of a chunk contribute to EVERY active receiver
-    uint32_t nLH, tpUn, fl, minTH, minTLun, pad_;
+    uint32_t nL, nH, tp, nUn, fl, minTH, minTLun, pad_;
     uint64_t h1, h2;
     // sequences of batches: the prefix part (batches before the last one)
-    uint32_t nLHp, tpc, minBHp, minBLlong;
+    uint32_t nLp, nHp, tpc, minBHp, minBLlong, pad2_;
     uint64_t h1p, h2p;
 };
 
+// Partials::cnt.z holds touched_pre in its low 30 bits and the PF_* flags above them: a chunk holds fewer than 2^30 subjects
+// (the slot count is bounded far below that by the mask rows, 4 * Rpad bytes per slot)
+constexpr int PF_SHIFT = 30;
+constexpr uint32_t TP_MASK = (1u << PF_SHIFT) - 1u;
+
 struct Partials {                     // [n_chunks][Rpad] structure of arrays
-    uint4* cnt;                       // x = nL | nH << 16, y = touched_pre | nUn << 16, z = flags | tpc << 16, w = nLp | nHp << 16
+    uint4* cnt;                       // x = nL, y = nH, z = touched_pre | flags << PF_SHIFT, w = nUn
+    uint4* cntp;                      // sequences only: x = nLp, y = nHp, z = tpc (touched and in the band before the call)
     uint64_t* minTH;
     uint64_t* minTLun;
     uint64_t* h1;
@@ -127,7 +135,7 @@ struct Bucketed {
     DevBuf<uint8_t> s_ring, s_status;         // per sorted cell
     DevBuf<int32_t> p_flag;
     DevBuf<ChunkAcc> p_chunk;
-    DevBuf<uint4> p_cnt;
+    DevBuf<uint4> p_cnt, p_cntp;
     DevBuf<uint64_t> p_minTH, p_minTLun, p_h1, p_h2, p_h1p, p_h2p;
     DevBuf<uint2> p_seq;
     DevBuf<SubjWalk> pwalk;                   // sequences: prefix walks
@@ -345,7 +353,8 @@ __device__ __forceinline__ void note_unresolved(const ApplyArgs& a, int tile, in
 // the thread's own slice of the global partial arrays.
 template <bool SEQ>
 __device__ __forceinline__ void part_store(const Partials& p, size_t at, const Acc& a) {
-    p.cnt[at] = make_uint4(a.nL | (a.nH << 16), a.tp | (a.nUn << 16), a.flags | (SEQ ? a.tpc << 16 : 0u), SEQ ? (a.nLp | (a.nHp << 16)) : 0u);
+    p.cnt[at] = make_uint4(a.nL, a.nH, a.tp | (a.flags << PF_SHIFT), a.nUn);
+    if (SEQ) p.cntp[at] = make_uint4(a.nLp, a.nHp, a.tpc, 0u);
     p.minTH[at] = a.minTH == T32_NONE ? T64_NONE : (uint64_t)a.minTH;
     p.minTLun[at] = a.minTLun == T32_NONE ? T64_NONE : (uint64_t)a.minTLun;
     p.h1[at] = a.h1;
@@ -355,9 +364,9 @@ __device__ __forceinline__ void part_store(const Partials& p, size_t at, const A
 template <bool SEQ>
 __device__ __forceinline__ void part_merge(const Partials& p, size_t at, const Acc& a) {      // add `a` to what the slot holds
     uint4 c = p.cnt[at];
-    c.x += a.nL | (a.nH << 16); c.y += a.tp | (a.nUn << 16); c.z |= a.flags;
-    if (SEQ) { c.z += a.tpc << 16; c.w += a.nLp | (a.nHp << 16); }
+    c.x += a.nL; c.y += a.nH; c.z = (c.z + a.tp) | (a.flags << PF_SHIFT); c.w += a.nUn;
     p.cnt[at] = c;
+    if (SEQ && (a.nLp | a.nHp | a.tpc)) { uint4 cp = p.cntp[at]; cp.x += a.nLp; cp.y += a.nHp; cp.z += a.tpc; p.cntp[at] = cp; }
     if (a.minTH != T32_NONE) { const uint64_t o = p.minTH[at]; if ((uint64_t)a.minTH < o) p.minTH[at] = a.minTH; }
     if (a.minTLun != T32_NONE) { const uint64_t o = p.minTLun[at]; if ((uint64_t)a.minTLun < o) p.minTLun[at] = a.minTLun; }
     if (a.nH) { p.h1[at] += a.h1; p.h2[at] += a.h2; }
@@ -373,7 +382,7 @@ __device__ __forceinline__ void part_merge(const Partials& p, size_t at, const A
 // read, the new word is the batch's ring mask under the thread's activity mask, and their contribution to the
 // per-receiver accumulators is the same for every active receiver — it is reduced once per stage by warp 0 and added
 // at the end.  Only carried subjects (reports from earlier batches) take the load / compare / visit path.
-struct StageAcc {
+struct StageAcc {                     // one subject or one stage: the counts fit 16-bit halves (at most STAGE each)
     uint32_t nLH, tpUn, fl, minTH, minTLun;
     uint64_t h1, h2;
     uint32_t nLHp, tpc, minBHp, minBLlong;
@@ -411,6 +420,22 @@ __device__ __forceinline__ StageAcc stage_reduce(StageAcc s) {
         }
     }
     return s;
+}
+// c += the packed contribution of a whole stage (the chunk's sum needs the full 32-bit counts)
+template <bool SEQ>
+__device__ __forceinline__ void chunk_add(ChunkAcc& c, const StageAcc& m) {
+    c.nL += m.nLH & 0xFFFFu; c.nH += m.nLH >> 16; c.tp += m.tpUn & 0xFFFFu; c.nUn += m.tpUn >> 16; c.fl |= m.fl;
+    c.minTH = min(c.minTH, m.minTH); c.minTLun = min(c.minTLun, m.minTLun); c.h1 += m.h1; c.h2 += m.h2;
+    if (SEQ) {
+        c.nLp += m.nLHp & 0xFFFFu; c.nHp += m.nLHp >> 16; c.tpc += m.tpc; c.minBHp = min(c.minBHp, m.minBHp);
+        c.minBLlong = min(c.minBLlong, m.minBLlong); c.h1p += m.h1p; c.h2p += m.h2p;
+    }
+}
+__device__ __forceinline__ ChunkAcc chunk_zero() {
+    ChunkAcc c;
+    c.nL = 0; c.nH = 0; c.tp = 0; c.nUn = 0; c.fl = 0; c.minTH = T32_NONE; c.minTLun = T32_NONE; c.pad_ = 0; c.h1 = 0; c.h2 = 0;
+    c.nLp = 0; c.nHp = 0; c.tpc = 0; c.minBHp = T32_NONE; c.minBLlong = T32_NONE; c.pad2_ = 0; c.h1p = 0; c.h2p = 0;
+    return c;
 }
 // a += the packed contribution of one subject (or of a whole stage)
 template <bool SEQ>
@@ -483,7 +508,7 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
     __shared__ uint16_t* s_dst[STAGE];
     __shared__ uint32_t s_nw[STAGE];          // (rings reported by the call) replicated in both half-words
     __shared__ int s_unres[STAGE];
-    __shared__ StageAcc s_facc;               // fresh-subject accumulators of this block's chunk (same for every receiver)
+    __shared__ ChunkAcc s_facc;               // fresh-subject accumulators of this block's chunk (same for every receiver)
     __shared__ int s_heavy;                   // staged subjects that are NOT plain fresh ones (carried, or with dictionary observers)
     // SEQ: the dictionary observers ("edges") of the staged subjects — their pre-call rows (nullptr: fresh, state 0) and batch index
     __shared__ uint8_t s_ne[SEQ ? STAGE : 1];
@@ -530,10 +555,7 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
     uint32_t am[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) am[q] = (((act >> (2 * q)) & 1u) ? 0x0000FFFFu : 0u) | (((act >> (2 * q + 1)) & 1u) ? 0xFFFF0000u : 0u);
-    if (t == 0) {
-        s_facc.nLH = 0; s_facc.tpUn = 0; s_facc.fl = 0; s_facc.minTH = T32_NONE; s_facc.minTLun = T32_NONE; s_facc.h1 = 0; s_facc.h2 = 0;
-        s_facc.nLHp = 0; s_facc.tpc = 0; s_facc.minBHp = T32_NONE; s_facc.minBLlong = T32_NONE; s_facc.h1p = 0; s_facc.h2p = 0;
-    }
+    if (t == 0) s_facc = chunk_zero();
     if (MEMO) {                                     // the tile's first active receiver
         const int mine = act ? t * 8 + __ffs(act) - 1 : INT_MAX;
         const int wmin = __reduce_min_sync(0xffffffffu, mine);
@@ -614,14 +636,7 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
             }
             // warp reduction of the fresh subjects' contribution
             const StageAcc fr = stage_reduce<SEQ>(stage_pack<SEQ>(f));
-            if (t == 0) {
-                s_facc.nLH += fr.nLH; s_facc.tpUn += fr.tpUn; s_facc.fl |= fr.fl; s_facc.minTH = min(s_facc.minTH, fr.minTH);
-                s_facc.minTLun = min(s_facc.minTLun, fr.minTLun); s_facc.h1 += fr.h1; s_facc.h2 += fr.h2;
-                if (SEQ) {
-                    s_facc.nLHp += fr.nLHp; s_facc.tpc += fr.tpc; s_facc.minBHp = min(s_facc.minBHp, fr.minBHp);
-                    s_facc.minBLlong = min(s_facc.minBLlong, fr.minBLlong); s_facc.h1p += fr.h1p; s_facc.h2p += fr.h2p;
-                }
-            }
+            if (t == 0) chunk_add<SEQ>(s_facc, fr);
             if (MEMO) {
                 const unsigned mm = __ballot_sync(0xffffffffu, memo);
                 if (mm) {                                 // (warp-uniform)
@@ -764,13 +779,7 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
     const int need = __syncthreads_or((carried || had_exc) ? 1 : 0);
     if (t == 0) {
         a.part.flag[(size_t)chunk * a.part.n_tiles + tile] = need;
-        if (tile == 0) {
-            const StageAcc f = s_facc;
-            ChunkAcc c;
-            c.nLH = f.nLH; c.tpUn = f.tpUn; c.fl = f.fl; c.minTH = f.minTH; c.minTLun = f.minTLun; c.pad_ = 0; c.h1 = f.h1; c.h2 = f.h2;
-            c.nLHp = f.nLHp; c.tpc = f.tpc; c.minBHp = f.minBHp; c.minBLlong = f.minBLlong; c.h1p = f.h1p; c.h2p = f.h2p;
-            a.part.chunk[chunk] = c;
-        }
+        if (tile == 0) a.part.chunk[chunk] = s_facc;
     }
     if (!need) return;
     const Acc zero;
@@ -950,15 +959,11 @@ __global__ void __launch_bounds__(GEN_THREADS, 4) k_apply_generic(const ApplyArg
     }
     if (t == 0) {
         if ((blockIdx.x * GEN_THREADS) % TILE_R == 0) a.part.flag[(size_t)chunk * a.part.n_tiles + tile] = 1;
-        if (blockIdx.x == 0) {
-            ChunkAcc c;
-            c.nLH = 0; c.tpUn = 0; c.fl = 0; c.minTH = T32_NONE; c.minTLun = T32_NONE; c.pad_ = 0; c.h1 = 0; c.h2 = 0;
-            a.part.chunk[chunk] = c;
-        }
+        if (blockIdx.x == 0) a.part.chunk[chunk] = chunk_zero();
     }
     if (r < (int64_t)a.Rpad) {
         const size_t p = (size_t)chunk * a.Rpad + (size_t)r;
-        a.part.cnt[p] = make_uint4(nL | (nH << 16), tp | (nUn << 16), fl, 0u);
+        a.part.cnt[p] = make_uint4(nL, nH, tp | (fl << PF_SHIFT), nUn);
         a.part.minTH[p] = minTH;
         a.part.minTLun[p] = minTLun;
         a.part.h1[p] = h1;
@@ -1049,13 +1054,12 @@ __device__ __forceinline__ void reduce_fresh(const ResolveArgs& a, ChunkAcc* s_f
         uint64_t h1p = 0, h2p = 0;
         for (int c = threadIdx.x; c < a.n_chunks; c += 32) {
             const ChunkAcc k = ap.part.chunk[c];
-            const uint32_t cH = k.nLH >> 16, cUn = k.tpUn >> 16;
-            nL += k.nLH & 0xFFFFu; nH += cH; tp += k.tpUn & 0xFFFFu; nUn += cUn; fl |= k.fl;
-            if (cH) mTH = min(mTH, k.minTH);
-            if (cUn) mTL = min(mTL, k.minTLun);
+            nL += k.nL; nH += k.nH; tp += k.tp; nUn += k.nUn; fl |= k.fl;
+            if (k.nH) mTH = min(mTH, k.minTH);
+            if (k.nUn) mTL = min(mTL, k.minTLun);
             h1 += k.h1; h2 += k.h2;
             if (a.seq) {
-                nLp += k.nLHp & 0xFFFFu; nHp += k.nLHp >> 16; tpc += k.tpc; mBH = min(mBH, k.minBHp); mBL = min(mBL, k.minBLlong);
+                nLp += k.nLp; nHp += k.nHp; tpc += k.tpc; mBH = min(mBH, k.minBHp); mBL = min(mBL, k.minBLlong);
                 h1p += k.h1p; h2p += k.h2p;
             }
         }
@@ -1073,8 +1077,8 @@ __device__ __forceinline__ void reduce_fresh(const ResolveArgs& a, ChunkAcc* s_f
         }
         if (threadIdx.x == 0) {
             ChunkAcc f;
-            f.nLH = nL | (nH << 16); f.tpUn = tp | (nUn << 16); f.fl = fl; f.minTH = mTH; f.minTLun = mTL; f.pad_ = 0; f.h1 = h1; f.h2 = h2;
-            f.nLHp = nLp | (nHp << 16); f.tpc = tpc; f.minBHp = mBH; f.minBLlong = mBL; f.h1p = h1p; f.h2p = h2p;
+            f.nL = nL; f.nH = nH; f.tp = tp; f.nUn = nUn; f.fl = fl; f.minTH = mTH; f.minTLun = mTL; f.pad_ = 0; f.h1 = h1; f.h2 = h2;
+            f.nLp = nLp; f.nHp = nHp; f.tpc = tpc; f.minBHp = mBH; f.minBLlong = mBL; f.pad2_ = 0; f.h1p = h1p; f.h2p = h2p;
             *s_fresh = f;
             *s_fhave = (nH ? 1 : 0) | (nUn ? 2 : 0);
         }
@@ -1097,9 +1101,9 @@ __device__ void phase_finalize1(const ResolveArgs& a, int32_t* s_red) {
         const bool active = !(flags & RF_ANNOUNCED) && !((ap.dl.flags & RAPID_DELIVERY_BLOCKED) && ap.dl.blocked[r]);
         if (!active) { a.rflags[r] = flags; a.out_ann[r] = (flags & RF_ANNOUNCED) ? 1 : 0; continue; }
         flags |= RF_ACTIVE;
-        uint32_t nL = s_fresh.nLH & 0xFFFFu, nH = s_fresh.nLH >> 16, tp = s_fresh.tpUn & 0xFFFFu, nUn = s_fresh.tpUn >> 16, fl = s_fresh.fl;
+        uint32_t nL = s_fresh.nL, nH = s_fresh.nH, tp = s_fresh.tp, nUn = s_fresh.nUn, fl = s_fresh.fl;
         uint64_t minTH = s_fresh.minTH, minTLun = s_fresh.minTLun, h1 = s_fresh.h1, h2 = s_fresh.h2;
-        uint32_t nLp = s_fresh.nLHp & 0xFFFFu, nHp = s_fresh.nLHp >> 16;                  // sequences: what the prefix did
+        uint32_t nLp = s_fresh.nLp, nHp = s_fresh.nHp;                                      // sequences: what the prefix did
         uint64_t h1p = s_fresh.h1p, h2p = s_fresh.h2p;
         bool haveTH = s_fhave & 1, haveTL = (s_fhave & 2) != 0;
         const int tile = (int)(r / TILE_R);
@@ -1108,7 +1112,7 @@ __device__ void phase_finalize1(const ResolveArgs& a, int32_t* s_red) {
             int on[4];
 #pragma unroll
             for (int q = 0; q < 4; ++q) on[q] = c0 + q < a.n_chunks ? ap.part.flag[(size_t)(c0 + q) * ap.part.n_tiles + tile] : 0;
-            uint4 q4[4];
+            uint4 q4[4], p4[4];
             uint64_t th[4], tl[4], a1[4], a2[4], b1[4], b2[4];
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
@@ -1116,19 +1120,19 @@ __device__ void phase_finalize1(const ResolveArgs& a, int32_t* s_red) {
                 const size_t p = (size_t)(c0 + q) * ap.Rpad + (size_t)r;
                 q4[q] = ap.part.cnt[p]; a1[q] = ap.part.h1[p]; a2[q] = ap.part.h2[p];
                 if (!a.counts_only) { th[q] = ap.part.minTH[p]; tl[q] = ap.part.minTLun[p]; }
-                if (a.seq) { b1[q] = ap.part.h1p[p]; b2[q] = ap.part.h2p[p]; }
+                if (a.seq) { p4[q] = ap.part.cntp[p]; b1[q] = ap.part.h1p[p]; b2[q] = ap.part.h2p[p]; }
             }
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 if (!on[q]) continue;
-                const uint32_t cH = q4[q].x >> 16, cUn = q4[q].y >> 16;
-                nL += q4[q].x & 0xFFFFu; nH += cH; tp += q4[q].y & 0xFFFFu; nUn += cUn; fl |= q4[q].z & 0xFFFFu;
+                const uint32_t cH = q4[q].y, cUn = q4[q].w;
+                nL += q4[q].x; nH += cH; tp += q4[q].z & TP_MASK; nUn += cUn; fl |= q4[q].z >> PF_SHIFT;
                 if (!a.counts_only) {
                     if (cH && (!haveTH || th[q] < minTH)) { minTH = th[q]; haveTH = true; }
                     if (cUn && (!haveTL || tl[q] < minTLun)) { minTLun = tl[q]; haveTL = true; }
                 }
                 h1 += a1[q]; h2 += a2[q];
-                if (a.seq) { nLp += q4[q].w & 0xFFFFu; nHp += q4[q].w >> 16; h1p += b1[q]; h2p += b2[q]; }
+                if (a.seq) { nLp += p4[q].x; nHp += p4[q].y; h1p += b1[q]; h2p += b2[q]; }
             }
         }
         // every valid cell reaches every active receiver unless there is a per-receiver bitmap
@@ -1714,7 +1718,7 @@ __global__ void __launch_bounds__(GEN_THREADS) k_seq_check(const ResolveArgs* __
             for (int c = 0; c < a.n_chunks; ++c) {
                 if (!ap.part.flag[(size_t)c * ap.part.n_tiles + tile]) continue;
                 const size_t p = (size_t)c * ap.Rpad + (size_t)r;
-                tpc += ap.part.cnt[p].z >> 16;
+                tpc += ap.part.cntp[p].z;
                 const uint2 q = ap.part.seq[p];
                 mBH = min(mBH, q.x); mBL = min(mBL, q.y);
             }
@@ -2060,10 +2064,14 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
         }
         if (const char* ov = getenv("RAPID_B200_CHUNKS")) n_chunks = std::max(1, std::min(Sb, atoi(ov)));   // tuning aid
     }
+    cd->last_chunks = n_chunks;
     const size_t pn = (size_t)n_chunks * cd->Rpad;
     RAPID_CHECK(b->p_cnt.reserve(pn)); RAPID_CHECK(b->p_minTH.reserve(pn)); RAPID_CHECK(b->p_minTLun.reserve(pn));
     RAPID_CHECK(b->p_h1.reserve(pn)); RAPID_CHECK(b->p_h2.reserve(pn));
-    if (seq) { RAPID_CHECK(b->p_h1p.reserve(pn)); RAPID_CHECK(b->p_h2p.reserve(pn)); RAPID_CHECK(b->p_seq.reserve(pn)); }
+    if (seq) {
+        RAPID_CHECK(b->p_cntp.reserve(pn)); RAPID_CHECK(b->p_h1p.reserve(pn)); RAPID_CHECK(b->p_h2p.reserve(pn));
+        RAPID_CHECK(b->p_seq.reserve(pn));
+    }
     RAPID_CHECK(b->mx_fl.reserve(cd->Rpad)); RAPID_CHECK(b->mx_a.reserve(cd->Rpad)); RAPID_CHECK(b->mx_cand.reserve(cd->Rpad));
     RAPID_CHECK(b->mx_emax.reserve(cd->Rpad)); RAPID_CHECK(b->mx_p1.reserve(cd->Rpad)); RAPID_CHECK(b->mx_p2.reserve(cd->Rpad));
     RAPID_CHECK(b->mx_pc.reserve(cd->Rpad)); RAPID_CHECK(b->estar.reserve(cd->Rpad));
@@ -2079,7 +2087,7 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
     }
     RAPID_CHECK(b->p_flag.reserve((size_t)n_chunks * std::max(b->n_tiles, 1)));
     RAPID_CHECK(b->p_chunk.reserve((size_t)n_chunks));
-    Partials part{b->p_cnt.p, b->p_minTH.p, b->p_minTLun.p, b->p_h1.p, b->p_h2.p, b->p_h1p.p, b->p_h2p.p, b->p_seq.p, b->p_flag.p, b->p_chunk.p, b->n_tiles};
+    Partials part{b->p_cnt.p, b->p_cntp.p, b->p_minTH.p, b->p_minTLun.p, b->p_h1.p, b->p_h2.p, b->p_h1p.p, b->p_h2p.p, b->p_seq.p, b->p_flag.p, b->p_chunk.p, b->n_tiles};
 
     ApplyArgs ap;
     ap.masks = cd->masks.p; ap.cur = cd->cur.p; ap.Rpad = cd->Rpad;

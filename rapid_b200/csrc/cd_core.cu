@@ -1215,6 +1215,15 @@ int32_t rapid_cd_debug_stats(const rapid_cd* cd, int32_t* n_mixed, int32_t* n_in
     return RAPID_OK;
 }
 
+int32_t rapid_cd_debug_grid(const rapid_cd* cd, int32_t* apply_chunks, int32_t* prepare_blocks) {
+    if (!cd) { set_error("NULL handle"); return RAPID_EINVAL; }
+    DeviceGuard g(cd->device);
+    RAPID_CHECK(cd_wait(cd, false));
+    if (apply_chunks) *apply_chunks = cd->bucketed ? cd->last_chunks : 0;
+    if (prepare_blocks) *prepare_blocks = cd->last_prep_grid;
+    return RAPID_OK;
+}
+
 int32_t rapid_cd_last_path(const rapid_cd* cd, int32_t* path, int32_t* n_kernel_launches) {
     if (!cd) { set_error("NULL handle"); return RAPID_EINVAL; }
     DeviceGuard g(cd->device);

@@ -128,6 +128,7 @@ struct CD {
     void* bucketed_state = nullptr;
 
     int32_t last_path = 0, last_launches = 0;
+    int32_t last_chunks = 0, last_prep_grid = 0;   // grid of the last batch: subject chunks of the apply kernel, k_prepare blocks
     float last_ms = 0.f, last_main_ms = 0.f;
     int64_t last_A = 0;
 };

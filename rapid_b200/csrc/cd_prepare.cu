@@ -392,6 +392,7 @@ int32_t prepare_batch(CD* cd, int64_t cfg, int64_t A, const int32_t* dst_dev, co
     }
     int G = (int)std::max<int64_t>(1, std::min<int64_t>(cd->prep_grid_max, ceil_div<int64_t>(A, PREP_THREADS * 2)));
     if (const char* ov = getenv("RAPID_B200_PREP_GRID")) G = std::max(1, std::min(cd->prep_grid_max, atoi(ov)));   // tuning aid
+    cd->last_prep_grid = G;
     RAPID_CHECK(cd->scan_sums.reserve(8));
     PrepArgs a;
     a.A = A; a.dst = dst_dev; a.ring = ring_dev; a.status = status_dev; a.cell_cfg = cfg_dev; a.cfg = cfg;

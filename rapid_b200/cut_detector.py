@@ -287,6 +287,12 @@ class VirtualCluster:
         N.check(N.lib().rapid_cd_debug_stats(self._h, C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
         return a.value, b.value, c.value, d.value
 
+    def debugGrid(self):
+        """(subject chunks of the last batch's apply kernel, blocks of its k_prepare grid)"""
+        a, b = C.c_int32(0), C.c_int32(0)
+        N.check(N.lib().rapid_cd_debug_grid(self._h, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
     def lastPath(self):
         a, b = C.c_int32(0), C.c_int32(0)
         N.check(N.lib().rapid_cd_last_path(self._h, C.byref(a), C.byref(b)))

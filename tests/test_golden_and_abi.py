@@ -98,6 +98,7 @@ def test_library_exports_every_declared_symbol():
     assert not missing, missing
     # the Python binding knows every entry point it may call
     assert set(_native.SIGNATURES) | {"rapid_version"} <= declared
+    assert "rapid_cd_debug_grid" in declared and "rapid_cd_debug_grid" in _native.SIGNATURES
     _native.lib()
     assert b"sm_90a" in _native.lib().rapid_version()
 

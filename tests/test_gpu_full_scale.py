@@ -199,3 +199,93 @@ def test_c4_hundred_thousand_nodes_flip_flop_stream(orc):
             decided = t
             break
     assert decided is not None and (decided.hash, decided.hash2) == want and decided.count == rb.quorum(n)
+
+
+class _Cells:
+    """a slice of a workload batch, shaped like one for _sampled_oracle_check"""
+
+    def __init__(self, b, sl):
+        self.src, self.dst, self.ring, self.status = b.src[sl], b.dst[sl], b.ring[sl], b.status[sl]
+
+    def __len__(self):
+        return len(self.dst)
+
+
+def test_c5_carried_halves_as_the_benchmark_runs_them(orc):
+    """bench.py's roofline_carried path: the C5 batch delivered as two halves with no clear() in between, so the second half
+    read-modify-writes the rows the first wrote (memo, L2 prefetch).  The same oracle instances follow both halves on a window
+    across a tile edge and a window holding blocked receivers; then the fast round decides the cut."""
+    import rapid_b200 as rb
+    n = 1_000_000
+    nj = n // 200
+    v = _view(rb, n, nj)
+    obs, _ = v.tables()
+    b = W.c5_churn(obs, v.joinerTables(), n, n // 200, nj)
+    hi, lo = W.node_ids(0, n)
+    cfg = v.getCurrentConfigurationId(hi, lo)
+    blocked = W.blocked_by_receiver(b.blocked, v.getRing(0), 0, n)
+    cl = rb.VirtualCluster(v, H, L, max_subjects=len(b.expected_cut) + 64)
+    half = len(b) // 2
+    first = np.nonzero(blocked)[0]
+    windows = (1024 * 500 - 100, int(min(max(first[len(first) // 2] - SAMPLE // 2, 0), n - SAMPLE)))
+    assert blocked[windows[1]: windows[1] + SAMPLE].any()
+    _, oview = _oracle_view(orc, n, nj)
+    sims = {}
+    for sl in (slice(0, half), slice(half, len(b))):
+        part = _Cells(b, sl)
+        res = cl.handleBatch(cfg, None, part.dst, part.ring, part.status, blocked=blocked)
+        assert cl.lastPath()[0] == 2
+        for w0 in windows:
+            sims[w0] = _sampled_oracle_check(orc, rb, oview, cl, res, w0, part, cfg, blocked, sim=sims.get(w0))
+    live = blocked == 0
+    assert (res.announced[live] == 1).all() and (res.announced[~live] == 0).all()
+    want = rb.proposal_fingerprint(b.expected_cut)
+    fp = rb.FastPaxos(cfg, n)
+    t = fp.tallyCluster(cl)
+    assert t.decided and (t.hash, t.hash2, t.length) == (want[0], want[1], len(b.expected_cut))
+
+
+def test_c4_as_one_sequence_call(orc):
+    """bench.py's default C4 stream: ONE rapid_cd_apply_batches call over 100,000 receivers (the SEQ kernels and k_seq_check at
+    98 tiles), served in one pass, against the oracle handling every batch on its own on two windows"""
+    import rapid_b200 as rb
+    n = 100_000
+    v = _view(rb, n)
+    obs, _ = v.tables()
+    ring0 = v.getRing(0)
+    batches = W.c4_flip_flop_stream(obs, n, 0.01, T=8)
+    hi, lo = W.node_ids(0, n)
+    cfg = v.getCurrentConfigurationId(hi, lo)
+    blocked = W.blocked_by_receiver(batches[0].blocked, ring0, 0, n)
+    src = np.concatenate([x.src for x in batches]); dst = np.concatenate([x.dst for x in batches])
+    ring = np.concatenate([x.ring for x in batches]); status = np.concatenate([x.status for x in batches])
+    off = np.concatenate([[0], np.cumsum([len(x) for x in batches])]).astype(np.int64)
+    perm = batches[0].meta["perm_seed"]
+    cl = rb.VirtualCluster(v, H, L)
+    res, ain = cl.handleBatches(cfg, None, dst, ring, status, off, blocked=blocked, perm_seed=perm)
+    assert cl.sequenceStats() == (1, 0), cl.sequenceRefusal()
+    _, oview = _oracle_view(orc, n)
+    for w0 in (1024 * 40 - 128, 77_777):
+        sl = slice(w0, w0 + SAMPLE)
+        sim = orc.ClusterSim(oview, K, H, L, SAMPLE, receiver_base=w0)
+        want_in, want_len = np.full(SAMPLE, -1, np.int32), np.zeros(SAMPLE, np.int32)
+        want_h1, want_h2 = np.zeros(SAMPLE, np.uint64), np.zeros(SAMPLE, np.uint64)
+        for t in range(len(batches)):
+            c = slice(int(off[t]), int(off[t + 1]))
+            o_len, o_ann, o_ids, o_off = sim.apply_batch(src[c], dst[c], ring[c], status[c], np.full(c.stop - c.start, cfg, np.int64),
+                                                         blocked=blocked[sl], perm_seed=perm + t, threads=8)
+            e1, e2 = fingerprints_from_oracle(rb, o_len, o_ids, o_off)
+            now = o_len > 0
+            want_in[now], want_len[now], want_h1[now], want_h2[now] = t, o_len[now], e1[now], e2[now]
+        np.testing.assert_array_equal(ain[sl], want_in)
+        np.testing.assert_array_equal(res.proposal_len[sl], want_len)
+        np.testing.assert_array_equal(res.proposal_hash[sl], want_h1)
+        np.testing.assert_array_equal(res.proposal_hash2[sl], want_h2)
+        np.testing.assert_array_equal(res.announced[sl], o_ann)
+        quiet = np.nonzero(o_ann == 0)[0]
+        for r in quiet[:: max(1, len(quiet) // 3)][:3]:
+            for subj, m in cl.debugMasks(int(w0 + r)).items():
+                assert sim.reportMask(int(r), int(subj)) == m, "mask of subject %d at receiver %d" % (subj, w0 + r)
+            assert cl.debugCounters(int(w0 + r))[0] == sim.updatesInProgress(int(r))
+    live = blocked == 0
+    assert (ain[live] == len(batches) - 1).all()
