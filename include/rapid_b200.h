@@ -279,7 +279,10 @@ int32_t rapid_fp_reset(rapid_fp* fp, int64_t cfg_id, int64_t membership_size);
  * (:145-150).  A proposal is identified by (hash, hash2, len) = rapid_proposal_fingerprint + size.
  * vote_cfg / proposal_hash2 / proposal_len may be NULL (= cfg / 0 / 0).
  * Outputs: decided, the decided fingerprint, its vote count at the moment of decision (== quorum) and
- * votesReceived.size() at that moment (or the running totals if undecided). */
+ * votesReceived.size() at that moment (or the running totals if undecided).
+ * A call is refused as a whole, and changes nothing, if a sender lies outside [0, sender_capacity) (RAPID_EINVAL) or if
+ * more than 8 proposals reach the quorum within it (RAPID_EUNSUPPORTED).  Once decided, a call returns the decision
+ * without looking at its votes. */
 int32_t rapid_fp_tally(rapid_fp* fp, int64_t n_votes, const int32_t* sender, const int64_t* vote_cfg,
                        const uint64_t* proposal_hash, const uint64_t* proposal_hash2, const int32_t* proposal_len,
                        int32_t* decided, uint64_t* decided_hash, uint64_t* decided_hash2, int32_t* decided_len,

@@ -3,10 +3,12 @@
 //
 // The Java keeps HashMap<List<Endpoint>, AtomicInteger> and hashes the whole endpoint list for every vote
 // (O(#cut) per vote).  Here a proposal is its 128-bit order-independent fingerprint + length (computed once
-// per proposer by the cut-detection kernels); votes are de-duplicated per sender with an atomicMin
-// "first index" table, counted in an open-addressing table with warp-aggregated atomics, and the exact
-// decision point (the vote at which a count reaches N - floor((N-1)/4)) is recovered with a prefix scan so
-// that votesReceived / count at the moment of decision match the sequential reference.
+// per proposer by the cut-detection kernels).  One cooperative kernel tallies the votes of a call, whether they
+// come from host arrays or straight from a detector's outputs: votes are de-duplicated per sender with an
+// atomicMin "first index" table, counted in an open-addressing table with warp-aggregated atomics, and the
+// exact decision point (the vote at which a count reaches N - floor((N-1)/4)) is recovered with per-block
+// counts and in-block scans so that votesReceived / count at the moment of decision match the sequential
+// reference.
 #include <cooperative_groups.h>
 #include <dlfcn.h>
 
@@ -16,7 +18,6 @@
 
 #include "cd_internal.cuh"
 #include "nccl_api.cuh"
-#include "scan.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -26,23 +27,21 @@ struct FPState {
     int32_t decided;
     int32_t decided_entry;
     int32_t votes_received;
-    int32_t n_valid_call;
     int32_t n_cand;
     int32_t cand[8];
     int32_t i_star;
-    int32_t bad_sender;
+    int32_t bad_sender;     // largest index of a vote whose sender is outside [0, sender_cap) (-1: none)
     int32_t n_entries;      // table entries created since the last reset (listed in FP::entries)
     int32_t n_call;         // entries that received votes in the call in flight (listed in FP::call_list)
-    int32_t ticket;         // "last block done" counter of k_fp_tally_cd
-    int32_t too_many;       // more than 8 proposals reached the quorum in one call
+    int32_t ticket;         // "last block done" counter of k_fp_tally
     int32_t calls;          // rapid_fp_tally_cd[_async] calls since the last reset
     int32_t decided_call;   // index of the call that decided (-1: undecided)
 };
 
 struct FPResult {
-    int32_t decided, len, count, received;
+    int32_t decided, len, count, received;   // decided = -1: refused, more than 8 proposals reached the quorum
     uint64_t h1, h2;
-    int32_t decided_call, pad;
+    int32_t decided_call, bad_sender;         // bad_sender >= 0: refused, FPState::bad_sender
 };
 struct FP {
     int device = 0;
@@ -55,9 +54,9 @@ struct FP {
     DevBuf<int32_t> seen;                 // [sender_cap] INT_MAX = not voted, -1 = voted, else first index in the call
     DevBuf<int32_t> t_state, t_len, t_count, t_call;
     DevBuf<uint64_t> t_h1, t_h2;
-    DevBuf<int32_t> ent, scan, scan_sums; // per-vote scratch
+    DevBuf<int32_t> ent;                  // per-vote scratch
     DevBuf<int32_t> entries, call_list;   // [T] created entries / entries voted for in the call in flight
-    DevBuf<int32_t> blk_cnt;              // [8][grid] per-block vote counts of the quorum candidates (k_fp_tally_cd)
+    DevBuf<int32_t> blk_cnt;              // [8][grid] per-block vote counts of the quorum candidates (k_fp_tally)
     int tally_grid = 0;                   // co-resident blocks of the cooperative tally kernel
     rapid_comm* pending_comm = nullptr;   // what the last enqueued rapid_fp_tally_cd[_async] was called with
     const rapid_cd* pending_cd = nullptr;
@@ -115,238 +114,13 @@ __global__ void k_fp_reset(int64_t sender_cap, int32_t* __restrict__ seen, uint3
     if (i < sender_cap) seen[i] = INT_MAX;
     if (i < (int64_t)T) { t_state[i] = 0; t_count[i] = 0; t_call[i] = 0; }
     if (i == 0) {
-        st->decided = 0; st->decided_entry = 0; st->votes_received = 0; st->n_valid_call = 0; st->n_cand = 0; st->i_star = INT_MAX; st->bad_sender = -1;
-        st->n_entries = 0; st->n_call = 0; st->ticket = 0; st->too_many = 0; st->calls = 0; st->decided_call = -1;
+        st->decided = 0; st->decided_entry = 0; st->votes_received = 0; st->n_cand = 0; st->i_star = INT_MAX; st->bad_sender = -1;
+        st->n_entries = 0; st->n_call = 0; st->ticket = 0; st->calls = 0; st->decided_call = -1;
     }
-}
-
-// first vote of every sender in this call (votesReceived.contains(sender), :134)
-__global__ void k_fp_first(int64_t n, const int32_t* __restrict__ sender, const int64_t* __restrict__ vcfg, int64_t cfg,
-                           int64_t sender_cap, int allow_skip, int32_t* __restrict__ seen, FPState* __restrict__ st) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int32_t s = sender[i];
-    if (s < 0 || s >= sender_cap) { if (!(allow_skip && s < 0)) atomicMax(&st->bad_sender, (int32_t)i); return; }
-    if (vcfg && vcfg[i] != cfg) return;                     // :126
-    atomicMin(&seen[s], (int32_t)i);                         // -1 (already voted) stays
 }
 
 __device__ __forceinline__ uint32_t fp_slot_hash(uint64_t h1, uint64_t h2, int32_t len) {
     return (uint32_t)(splitmix64(h1 ^ rotl64(h2, 21) ^ (uint64_t)(uint32_t)len) >> 32);
-}
-
-// find-or-insert the proposal of every valid vote; count per entry for this call (warp-aggregated)
-__global__ void k_fp_insert(int64_t n, const int32_t* __restrict__ sender, const int64_t* __restrict__ vcfg, int64_t cfg,
-                            int64_t sender_cap, const uint64_t* __restrict__ h1v, const uint64_t* __restrict__ h2v,
-                            const int32_t* __restrict__ lenv, int32_t* __restrict__ seen, uint32_t T,
-                            int32_t* __restrict__ t_state, uint64_t* __restrict__ t_h1, uint64_t* __restrict__ t_h2,
-                            int32_t* __restrict__ t_len, int32_t* __restrict__ t_call, int32_t* __restrict__ ent,
-                            FPState* __restrict__ st, int unique_senders, int direct, int32_t* __restrict__ entries) {
-    // direct (sharded tally of a detector's own votes): no arrival-order bookkeeping is needed, so the counts go straight
-    // to t_count (the caller passes it as t_call), the senders are marked as having voted and votesReceived grows here
-    __shared__ int32_t s_key[16], s_val[16];
-    if (threadIdx.x < 16) { s_key[threadIdx.x] = -1; s_val[threadIdx.x] = 0; }
-    __syncthreads();
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    bool valid = false;
-    uint64_t h1 = 0, h2 = 0;
-    int32_t len = 0;
-    if (i < n) {
-        const int32_t s = sender[i];
-        // unique_senders: every sender appears at most once in this call (votes of a detector's own receivers), so the
-        // first-vote pass was skipped and "has not voted yet" is all there is to check
-        if (s >= 0 && s < sender_cap && !(vcfg && vcfg[i] != cfg) && (unique_senders ? seen[s] != -1 : seen[s] == (int32_t)i)) {
-            valid = true;
-            h1 = h1v[i];
-            h2 = h2v ? h2v[i] : 0;
-            len = lenv ? lenv[i] : 0;
-        }
-    }
-    int32_t e = -1;
-    // one leader per distinct fingerprint in the warp does the table probe
-    const unsigned active = __ballot_sync(0xffffffffu, valid);
-    if (valid) {
-        const unsigned same = __match_any_sync(active, h1 ^ rotl64(h2, 21) ^ ((uint64_t)(uint32_t)len << 1));
-        const int leader = __ffs(same) - 1;
-        const int lane = threadIdx.x & 31;
-        if (lane == leader) {
-            uint32_t pos = fp_slot_hash(h1, h2, len) & (T - 1);
-            for (;;) {
-                int32_t state = *(volatile int32_t*)&t_state[pos];         // published entries need no atomic
-                if (state == 0) state = atomicCAS(&t_state[pos], 0, 1);
-                if (state == 0) {                            // claimed an empty entry: publish the key
-                    t_h1[pos] = h1; t_h2[pos] = h2; t_len[pos] = len;
-                    __threadfence();
-                    atomicExch(&t_state[pos], 2);
-                    entries[atomicAdd(&st->n_entries, 1)] = (int32_t)pos;
-                    e = (int32_t)pos;
-                    break;
-                }
-                while (state == 1) state = atomicAdd(&t_state[pos], 0);     // another warp is publishing
-                __threadfence();
-                if (t_h1[pos] == h1 && t_h2[pos] == h2 && t_len[pos] == len) { e = (int32_t)pos; break; }
-                pos = (pos + 1) & (T - 1);
-            }
-            {   // warp -> block aggregation of the per-call count (a handful of distinct proposals per block)
-                const int c = __popc(same);
-                int slot = -1;
-                for (int q = 0; q < 16; ++q) {
-                    const int32_t k = atomicCAS(&s_key[q], -1, e);
-                    if (k == -1 || k == e) { slot = q; break; }
-                }
-                if (slot >= 0) atomicAdd(&s_val[slot], c);
-                else atomicAdd(&t_call[e], c);
-            }
-        }
-        // NOTE: __match_any groups by the XOR-folded key; distinct fingerprints that fold equal are split below
-        e = __shfl_sync(same, e, leader);
-        const uint64_t lh1 = __shfl_sync(same, h1, leader), lh2 = __shfl_sync(same, h2, leader);
-        const int32_t llen = __shfl_sync(same, len, leader);
-        if (lh1 != h1 || lh2 != h2 || llen != len) {
-            // folded-key collision inside the warp (astronomically rare): undo the leader's count for me, probe myself
-            atomicSub(&t_call[e], 1);
-            uint32_t pos = fp_slot_hash(h1, h2, len) & (T - 1);
-            for (;;) {
-                int32_t state = atomicCAS(&t_state[pos], 0, 1);
-                if (state == 0) {
-                    t_h1[pos] = h1; t_h2[pos] = h2; t_len[pos] = len;
-                    __threadfence();
-                    atomicExch(&t_state[pos], 2);
-                    entries[atomicAdd(&st->n_entries, 1)] = (int32_t)pos;
-                    break;
-                }
-                while (state == 1) state = atomicAdd(&t_state[pos], 0);
-                if (t_h1[pos] == h1 && t_h2[pos] == h2 && t_len[pos] == len) break;
-                pos = (pos + 1) & (T - 1);
-            }
-            e = (int32_t)pos;
-            atomicAdd(&t_call[e], 1);
-        }
-    }
-    if (i < n) ent[i] = e;
-    if (direct && valid) seen[sender[i]] = -1;
-    const unsigned cnt = __popc(active);
-    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(direct ? &st->votes_received : &st->n_valid_call, (int32_t)cnt);
-    __syncthreads();
-    if (threadIdx.x < 16 && s_key[threadIdx.x] >= 0) atomicAdd(&t_call[s_key[threadIdx.x]], s_val[threadIdx.x]);
-}
-
-// entries whose count reaches the quorum within this call
-__global__ void k_fp_candidates(uint32_t T, const int32_t* __restrict__ t_count, const int32_t* __restrict__ t_call,
-                                int32_t Q, FPState* __restrict__ st) {
-    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= T) return;
-    const int32_t c = t_call[e];
-    if (c > 0 && t_count[e] + c >= Q) {
-        const int32_t at = atomicAdd(&st->n_cand, 1);
-        if (at < 8) st->cand[at] = (int32_t)e;
-    }
-}
-
-__global__ void k_fp_flag(int64_t n, const int32_t* __restrict__ ent, int32_t e, int32_t* __restrict__ flag) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) flag[i] = ent[i] == e ? 1 : 0;
-}
-
-__global__ void k_fp_scan(int32_t* __restrict__ data, int64_t n) {          // single block exclusive scan
-    __shared__ int32_t part[1024];
-    const int T = blockDim.x, t = threadIdx.x;
-    const int64_t per = (n + T - 1) / T;
-    const int64_t b = (int64_t)t * per, e = b + per < n ? b + per : n;
-    int32_t s = 0;
-    for (int64_t i = b; i < e; ++i) s += data[i];
-    part[t] = s;
-    __syncthreads();
-    for (int off = 1; off < T; off <<= 1) {
-        int32_t v = t >= off ? part[t - off] : 0;
-        __syncthreads();
-        part[t] += v;
-        __syncthreads();
-    }
-    int32_t run = t ? part[t - 1] : 0;
-    for (int64_t i = b; i < e; ++i) { const int32_t v = data[i]; data[i] = run; run += v; }
-}
-
-// the vote at which entry e's running count reaches Q
-__global__ void k_fp_find(int64_t n, const int32_t* __restrict__ ent, const int32_t* __restrict__ excl, int32_t e,
-                          const int32_t* __restrict__ t_count, int32_t Q, FPState* __restrict__ st) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n || ent[i] != e) return;
-    if (t_count[e] + excl[i] + 1 == Q) {
-        const int32_t old = atomicMin(&st->i_star, (int32_t)i);
-        (void)old;
-    }
-}
-__global__ void k_fp_pick(int64_t n, const int32_t* __restrict__ ent, FPState* __restrict__ st) {
-    if (threadIdx.x == 0 && blockIdx.x == 0 && st->i_star < INT_MAX) { st->decided = 1; st->decided_entry = ent[st->i_star]; }
-    (void)n;
-}
-
-// apply the votes with index <= limit (limit = n-1 if no decision in this call)
-__global__ void k_fp_apply(int64_t n, const int32_t* __restrict__ sender, const int32_t* __restrict__ ent,
-                           const FPState* __restrict__ stc, int use_istar, int32_t* __restrict__ seen,
-                           int32_t* __restrict__ t_count, FPState* __restrict__ st) {
-    // counts are aggregated warp -> block (a handful of distinct proposals per block) -> one global atomic per
-    // (block, proposal): a million votes for one proposal would otherwise serialise on a single L2 address
-    __shared__ int32_t s_key[16], s_val[16], s_recv;
-    if (threadIdx.x < 16) { s_key[threadIdx.x] = -1; s_val[threadIdx.x] = 0; }
-    if (threadIdx.x == 0) s_recv = 0;
-    __syncthreads();
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t limit = use_istar ? (int64_t)stc->i_star : n - 1;
-    int32_t e = -1;
-    bool counted = false;
-    if (i < n) {
-        e = ent[i];
-        if (e >= 0) {
-            const int32_t s = sender[i];
-            if (i <= limit) { seen[s] = -1; counted = true; }    // votesReceived.add(sender) :141
-            else seen[s] = INT_MAX;                              // arrived after the decision: ignored entirely (:138)
-        }
-    }
-    const unsigned m = __ballot_sync(0xffffffffu, counted);
-    if (counted) {
-        const unsigned same = __match_any_sync(m, e);
-        if ((int)(threadIdx.x & 31) == __ffs(same) - 1) {
-            const int c = __popc(same);
-            int slot = -1;
-            for (int q = 0; q < 16; ++q) {
-                const int32_t k = atomicCAS(&s_key[q], -1, e);
-                if (k == -1 || k == e) { slot = q; break; }
-            }
-            if (slot >= 0) atomicAdd(&s_val[slot], c);
-            else atomicAdd(&t_count[e], c);                      // more than 16 distinct proposals in one block
-        }
-    }
-    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&s_recv, __popc(m));
-    __syncthreads();
-    if (threadIdx.x < 16 && s_key[threadIdx.x] >= 0) atomicAdd(&t_count[s_key[threadIdx.x]], s_val[threadIdx.x]);   // :142-144
-    if (threadIdx.x == 0 && s_recv) atomicAdd(&st->votes_received, s_recv);
-}
-
-// A call that fails after k_fp_first / k_fp_insert (bad sender id, too many candidates) must leave no trace: the first-index marks
-// of this call's senders go back to "has not voted" (a mark left behind would make every later vote of that sender look like a
-// duplicate), and the per-call counts are zeroed by k_fp_zero_call.
-__global__ void k_fp_rollback(int64_t n, const int32_t* __restrict__ sender, int64_t sender_cap, int32_t* __restrict__ seen) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int32_t s = sender[i];
-    if (s < 0 || s >= sender_cap) return;
-    const int32_t v = seen[s];
-    if (v >= 0 && v != INT_MAX) seen[s] = INT_MAX;          // (-1 = voted in an EARLIER call: stays)
-}
-
-__global__ void k_fp_zero_call(uint32_t T, int32_t* __restrict__ t_call) {
-    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e < T) t_call[e] = 0;
-}
-
-// votes of the receivers that announced in the last batch (FastPaxos.propose :94-108)
-__global__ void k_fp_votes_from_cd(int64_t R, const uint32_t* __restrict__ rflags, const int32_t* __restrict__ ring0,
-                                   int64_t rbegin, int32_t* __restrict__ sender) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= R) return;
-    sender[r] = (rflags[r] & RF_ANN_NOW) ? ring0[rbegin + r] : -1;
 }
 
 // ---- sharded tally: radix histogram over the proposal fingerprints, restricted to a prefix -----------------------
@@ -394,19 +168,7 @@ __global__ void k_fp_minmax(uint32_t T, const int32_t* __restrict__ t_state, con
 }
 
 __global__ void k_fp_begin(FPState* st) {
-    st->n_valid_call = 0; st->n_cand = 0; st->i_star = INT_MAX; st->bad_sender = -1;
-}
-
-__global__ void k_fp_result(const FPState* __restrict__ st, const uint64_t* __restrict__ t_h1, const uint64_t* __restrict__ t_h2,
-                            const int32_t* __restrict__ t_len, const int32_t* __restrict__ t_count, FPResult* __restrict__ out) {
-    FPResult r;
-    r.decided = st->decided; r.received = st->votes_received; r.len = 0; r.count = 0; r.h1 = 0; r.h2 = 0;
-    r.decided_call = st->decided_call; r.pad = 0;
-    if (r.decided && st->decided_entry >= 0) {
-        const int32_t e = st->decided_entry;
-        r.h1 = t_h1[e]; r.h2 = t_h2[e]; r.len = t_len[e]; r.count = t_count[e];
-    }
-    *out = r;
+    st->n_cand = 0; st->i_star = INT_MAX; st->bad_sender = -1;
 }
 
 // ---- sharded tally, the single all-reduce: per 12-bit bucket of the fingerprint, SUMS of (count, h1 hi/lo, h2 hi/lo, len,
@@ -419,64 +181,20 @@ __device__ __forceinline__ uint64_t fp_check_word(uint64_t h1, uint64_t h2, uint
     return splitmix64(h1 ^ rotl64(h2, 17) ^ (len * 0x9E3779B97F4A7C15ULL));
 }
 
-__global__ void k_fp_hist_sum(uint32_t T, const int32_t* __restrict__ t_state, const uint64_t* __restrict__ t_h1,
-                              const uint64_t* __restrict__ t_h2, const int32_t* __restrict__ t_len,
-                              const int32_t* __restrict__ t_count, const FPState* __restrict__ st,
-                              unsigned long long* __restrict__ buf) {
-    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e == 0) buf[(size_t)SUM_BUCKETS * SUM_WORDS] = (unsigned long long)st->votes_received;
-    if (e >= T || t_state[e] != 2) return;
-    const unsigned long long c = (unsigned long long)t_count[e];
-    if (c == 0) return;
-    const uint64_t h1 = t_h1[e], h2 = t_h2[e], len = (uint64_t)(uint32_t)t_len[e], m = fp_check_word(h1, h2, len);
-    unsigned long long* b = buf + (size_t)(h1 >> 52) * SUM_WORDS;
-    atomicAdd(b + 0, c);
-    atomicAdd(b + 1, c * (h1 >> 32)); atomicAdd(b + 2, c * (h1 & 0xFFFFFFFFull));
-    atomicAdd(b + 3, c * (h2 >> 32)); atomicAdd(b + 4, c * (h2 & 0xFFFFFFFFull));
-    atomicAdd(b + 5, c * len);
-    atomicAdd(b + 6, c * (m >> 32)); atomicAdd(b + 7, c * (m & 0xFFFFFFFFull));
-}
-
 struct FPSumResult {
     FPResult r;
     int32_t ambiguous;       // a bucket reached the quorum but holds more than one proposal
     int32_t pad;
 };
 
-__global__ void k_fp_decide_sum_impl(const unsigned long long* __restrict__ buf, unsigned long long Q, FPSumResult* __restrict__ out) {
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= SUM_BUCKETS) return;
-    const unsigned long long* w = buf + (size_t)b * SUM_WORDS;
-    const unsigned long long c = w[0];
-    if (c < Q || c == 0) return;
-    bool ok = true;
-    for (int q = 1; q < SUM_WORDS; ++q) ok = ok && (w[q] % c == 0);
-    uint64_t h1 = 0, h2 = 0, len = 0;
-    if (ok) {
-        const uint64_t a1 = w[1] / c, a2 = w[2] / c, b1 = w[3] / c, b2 = w[4] / c;
-        len = w[5] / c;
-        ok = a1 <= 0xFFFFFFFFull && a2 <= 0xFFFFFFFFull && b1 <= 0xFFFFFFFFull && b2 <= 0xFFFFFFFFull && len <= 0x7FFFFFFFull;
-        h1 = (a1 << 32) | a2; h2 = (b1 << 32) | b2;
-        if (ok) {
-            const uint64_t m = fp_check_word(h1, h2, len);
-            ok = (w[6] / c == (m >> 32)) && (w[7] / c == (m & 0xFFFFFFFFull)) && ((h1 >> 52) == (uint64_t)b);
-        }
-    }
-    if (ok) {
-        out->r.decided = 1; out->r.h1 = h1; out->r.h2 = h2; out->r.len = (int32_t)len; out->r.count = (int32_t)c;
-    } else {
-        out->ambiguous = 1;
-    }
-}
-
-// one block: initialise the result, then look for the bucket that reached the quorum (k_fp_sum_begin + k_fp_decide_sum_impl fused)
+// one block: initialise the result, then look for the bucket that reached the quorum
 __global__ void __launch_bounds__(1024) k_fp_decide_sum(const unsigned long long* __restrict__ buf, unsigned long long Q,
                                                         FPSumResult* __restrict__ out, FPState* __restrict__ st) {
     __shared__ int32_t s_call;
     if (threadIdx.x == 0) {
         out->r.decided = 0; out->r.len = 0; out->r.count = 0; out->r.h1 = 0; out->r.h2 = 0;
         out->r.received = (int32_t)buf[(size_t)SUM_BUCKETS * SUM_WORDS];
-        out->r.decided_call = st->decided_call; out->r.pad = 0;
+        out->r.decided_call = st->decided_call; out->r.bad_sender = -1;
         out->ambiguous = 0; out->pad = 0;
         s_call = st->calls;
         st->calls = s_call + 1;
@@ -510,38 +228,41 @@ __global__ void __launch_bounds__(1024) k_fp_decide_sum(const unsigned long long
     }
 }
 
-__global__ void k_fp_sum_begin(const unsigned long long* __restrict__ buf, FPSumResult* __restrict__ out) {
-    out->r.decided = 0; out->r.len = 0; out->r.count = 0; out->r.h1 = 0; out->r.h2 = 0;
-    out->r.received = (int32_t)buf[(size_t)SUM_BUCKETS * SUM_WORDS];
-    out->ambiguous = 0; out->pad = 0;
-}
-
 // ==================================================================================================================
-// k_fp_tally_cd: the fast-round tally of a detector's own votes in ONE cooperative launch.
+// k_fp_tally<ARRAY>: the fast-round tally of one call in ONE cooperative launch, for votes from either source.
 //
-// Every receiver that announced in the last batch votes for its proposal (FastPaxos.propose :94-108), in receiver order
-// (= arrival order on one GPU).  Senders are unique by construction, so "first vote of a sender" is just "has not voted
-// in an earlier call".  Phases (grid barriers in between, every block owns a CONTIGUOUS range of receivers so that
-// arrival order is block order):
-//   A  find-or-insert the proposal of every vote (warp- and block-aggregated counts -> t_call); the add that takes a
+// ARRAY = false: every receiver that announced in the last batch votes for its proposal (FastPaxos.propose :94-108), in
+//   receiver order (= arrival order on one GPU).  Senders are unique by construction, so "first vote of a sender" is just
+//   "has not voted in an earlier call".
+// ARRAY = true: vote i is (sender[i], vcfg[i], h1v[i], h2v[i], lenv[i]) in arrival order, as the host handed them over.  A
+//   sender may vote several times; only its first vote of this configuration counts (:126, :134).
+// Phases (grid barriers in between, every block owns a CONTIGUOUS range of votes so that arrival order is block order):
+//   V  (ARRAY) a sender outside [0, sender_cap) refuses the whole call before anything is marked
+//   F  (ARRAY) the first vote of every sender in this call: atomicMin of its index into seen[] (-1, voted earlier, stays)
+//   A  find-or-insert the proposal of every first vote (warp- and block-aggregated counts -> t_call); the add that takes a
 //      proposal over the quorum nominates it as a candidate
 //   C  only if there is a candidate: the exact vote i* at which its running count reaches the quorum (per-block counts,
 //      prefix over blocks, in-block scan) — votes after i* are ignored, as the sequential reference would (:138)
-//   D  apply: votesReceived, counts, seen marks for the votes with index <= i*
+//   D  apply: votesReceived, counts, seen marks for the votes with index <= i*; the first votes after i* are unmarked
 //   tail (last block): decision + result record, per-call scratch re-armed
-// direct != 0 (sharded tally): no arrival order across ranks — counts go straight to t_count and phase S adds this rank's
-// table to the all-reduce buffer.
+// More than 8 proposals crossing the quorum in one call refuses it: C is skipped and D counts nothing, so the refused call
+// leaves no trace and does not decide.  Once decided, a call changes nothing and reports the stored result.
+// direct != 0 (sharded tally, detector votes only): no arrival order across ranks — counts go straight to t_count and
+// phase S adds this rank's table to the all-reduce buffer.
 // ==================================================================================================================
 constexpr int TALLY_THREADS = 256;
-constexpr int SUM_BUCKETS_ = 4096, SUM_WORDS_ = 8;
 
-struct TallyCdArgs {
-    int64_t R, rbegin;
+struct TallyArgs {
+    int64_t R;                  // votes
+    int64_t rbegin;             // detector votes: receiver i votes iff rflags[i] & RF_ANN_NOW, as sender ring0[rbegin + i]
     const uint32_t* rflags;
     const int32_t* ring0;
+    const int32_t* sender;      // array votes: vote i comes from sender[i] for configuration vcfg[i] (vcfg NULL: cfg)
+    const int64_t* vcfg;
+    int64_t cfg;
     const uint64_t* h1v;
-    const uint64_t* h2v;
-    const int32_t* lenv;
+    const uint64_t* h2v;        // array votes: NULL means 0
+    const int32_t* lenv;        // array votes: NULL means 0
     int64_t sender_cap;
     int32_t* seen;
     uint32_t T;
@@ -562,7 +283,7 @@ struct TallyCdArgs {
     FPResult* out;
 };
 
-__device__ __forceinline__ int32_t fp_find_or_insert(const TallyCdArgs& a, uint64_t h1, uint64_t h2, int32_t len) {
+__device__ __forceinline__ int32_t fp_find_or_insert(const TallyArgs& a, uint64_t h1, uint64_t h2, int32_t len) {
     uint32_t pos = fp_slot_hash(h1, h2, len) & (a.T - 1);
     for (;;) {
         int32_t state = *(volatile int32_t*)&a.t_state[pos];              // published entries need no atomic
@@ -582,14 +303,14 @@ __device__ __forceinline__ int32_t fp_find_or_insert(const TallyCdArgs& a, uint6
 }
 
 // add c votes of this call to entry e; nominate it if THIS add takes it over the quorum
-__device__ __forceinline__ void fp_add_call(const TallyCdArgs& a, int32_t e, int32_t c) {
+__device__ __forceinline__ void fp_add_call(const TallyArgs& a, int32_t e, int32_t c) {
     if (a.direct) { atomicAdd(&a.t_count[e], c); return; }
     const int32_t old = atomicAdd(&a.t_call[e], c);
     if (old == 0) a.call_list[atomicAdd(&a.st->n_call, 1)] = e;
     const int32_t before = a.t_count[e] + old;
     if (before < a.Q && before + c >= a.Q) {
         const int32_t at = atomicAdd(&a.st->n_cand, 1);
-        if (at < 8) a.st->cand[at] = e; else a.st->too_many = 1;
+        if (at < 8) a.st->cand[at] = e;                  // more than 8 refuse the call
     }
 }
 
@@ -618,14 +339,16 @@ __device__ __forceinline__ int32_t tally_block_scan(int32_t v, int32_t* warp_sum
     return (wid ? warp_sums[wid - 1] : 0) + inc - v;
 }
 
-__global__ void __launch_bounds__(TALLY_THREADS) k_fp_tally_cd(const TallyCdArgs a) {
+template <bool ARRAY>
+__global__ void __launch_bounds__(TALLY_THREADS) k_fp_tally(const TallyArgs a) {
     cg::grid_group grid = cg::this_grid();
     __shared__ int32_t s_key[16], s_val[16], s_recv, s_last;
     __shared__ int32_t warp_sums[TALLY_THREADS / 32];
     const int t = threadIdx.x, G = gridDim.x, bid = blockIdx.x;
     const int64_t per = ((a.R + G - 1) / G + TALLY_THREADS - 1) / TALLY_THREADS * TALLY_THREADS;
     const int64_t c0 = min(a.R, (int64_t)bid * per), c1 = min(a.R, c0 + per);
-    const bool was_decided = a.st->decided != 0;          // :138 — everything after the decision is ignored
+    const bool direct = !ARRAY && a.direct;
+    bool skip = a.st->decided != 0;                       // :138 — everything after the decision is ignored
 
     auto block_flush = [&](bool to_count) {               // block-level partial counts -> global
         __syncthreads();
@@ -648,17 +371,35 @@ __global__ void __launch_bounds__(TALLY_THREADS) k_fp_tally_cd(const TallyCdArgs
         else fp_add_call(a, e, c);
     };
 
+    if (ARRAY && !skip) {
+        // ---- V: a sender outside the table refuses the call; nothing is marked yet, so nothing has to be undone ---------------
+        for (int64_t i = c0 + t; i < c1; i += TALLY_THREADS) {
+            const int32_t s = a.sender[i];
+            if (s < 0 || s >= a.sender_cap) atomicMax(&a.st->bad_sender, (int32_t)i);
+        }
+        grid.sync();
+        skip = *(volatile int32_t*)&a.st->bad_sender >= 0;
+        if (!skip) {
+            // ---- F: the first vote of every sender in this call (votesReceived.contains(sender), :134) ----------------------------
+            for (int64_t i = c0 + t; i < c1; i += TALLY_THREADS)
+                if (!a.vcfg || a.vcfg[i] == a.cfg) atomicMin(&a.seen[a.sender[i]], (int32_t)i);   // :126; -1 (voted earlier) stays
+            grid.sync();
+        }
+    }
     if (t < 16) { s_key[t] = -1; s_val[t] = 0; }
     if (t == 0) s_recv = 0;
     __syncthreads();
-    if (!was_decided) {
+    if (!skip) {
         // ---- A: one table probe per distinct fingerprint per warp ------------------------------------------------------------
         for (int64_t base = c0; base < c1; base += TALLY_THREADS) {
             const int64_t i = base + t;
             bool valid = false;
             uint64_t h1 = 0, h2 = 0;
             int32_t len = 0, sender = -1;
-            if (i < c1 && (a.rflags[i] & RF_ANN_NOW)) {
+            if (ARRAY) {
+                valid = i < c1 && (!a.vcfg || a.vcfg[i] == a.cfg) && a.seen[a.sender[i]] == (int32_t)i;
+                if (valid) { h1 = a.h1v[i]; h2 = a.h2v ? a.h2v[i] : 0; len = a.lenv ? a.lenv[i] : 0; }
+            } else if (i < c1 && (a.rflags[i] & RF_ANN_NOW)) {
                 sender = a.ring0[a.rbegin + i];
                 if (sender >= 0 && sender < a.sender_cap && a.seen[sender] != -1) {
                     valid = true;
@@ -677,29 +418,26 @@ __global__ void __launch_bounds__(TALLY_THREADS) k_fp_tally_cd(const TallyCdArgs
                 const bool mine = lh1 == h1 && lh2 == h2 && llen == len;
                 if (!mine) e = fp_find_or_insert(a, h1, h2, len);           // folded-key collision inside the warp (astronomically rare)
                 const unsigned grp = __match_any_sync(same, e);             // the leader's group minus the collided lanes, per entry
-                if ((t & 31) == __ffs(grp) - 1) block_add(e, __popc(grp), a.direct != 0);
-                if (a.direct) a.seen[sender] = -1;
+                if ((t & 31) == __ffs(grp) - 1) block_add(e, __popc(grp), direct);
+                if (direct) a.seen[sender] = -1;
             }
             if (i < c1) a.ent[i] = e;
-            if ((t & 31) == 0 && active) atomicAdd(&s_recv, __popc(active));
+            if (direct && (t & 31) == 0 && active) atomicAdd(&s_recv, __popc(active));
         }
-        block_flush(a.direct != 0);
-        if (t == 0 && s_recv) {
-            if (a.direct) atomicAdd(&a.st->votes_received, s_recv);
-            else atomicAdd(&a.st->n_valid_call, s_recv);
-        }
+        block_flush(direct);
+        if (direct && t == 0 && s_recv) atomicAdd(&a.st->votes_received, s_recv);
     }
-    if (a.direct) {
+    if (direct) {
         // ---- S: this rank's table -> the all-reduce buffer (count-weighted sums per 12-bit bucket of the fingerprint) ------
         grid.sync();
         const int32_t ne = *(volatile int32_t*)&a.st->n_entries;
-        if (bid == 0 && t == 0) a.sumbuf[(size_t)SUM_BUCKETS_ * SUM_WORDS_] = (unsigned long long)*(volatile int32_t*)&a.st->votes_received;
+        if (bid == 0 && t == 0) a.sumbuf[(size_t)SUM_BUCKETS * SUM_WORDS] = (unsigned long long)*(volatile int32_t*)&a.st->votes_received;
         for (int32_t q = bid * TALLY_THREADS + t; q < ne; q += G * TALLY_THREADS) {
             const int32_t e = a.entries[q];
             const unsigned long long c = (unsigned long long)a.t_count[e];
             if (c == 0) continue;
             const uint64_t h1 = a.t_h1[e], h2 = a.t_h2[e], len = (uint64_t)(uint32_t)a.t_len[e], m = fp_check_word(h1, h2, len);
-            unsigned long long* b = a.sumbuf + (size_t)(h1 >> 52) * SUM_WORDS_;
+            unsigned long long* b = a.sumbuf + (size_t)(h1 >> 52) * SUM_WORDS;
             atomicAdd(b + 0, c);
             atomicAdd(b + 1, c * (h1 >> 32)); atomicAdd(b + 2, c * (h1 & 0xFFFFFFFFull));
             atomicAdd(b + 3, c * (h2 >> 32)); atomicAdd(b + 4, c * (h2 & 0xFFFFFFFFull));
@@ -709,8 +447,10 @@ __global__ void __launch_bounds__(TALLY_THREADS) k_fp_tally_cd(const TallyCdArgs
         return;
     }
     grid.sync();
-    const int32_t n_cand = was_decided ? 0 : min(8, *(volatile int32_t*)&a.st->n_cand);
-    int64_t limit = INT64_MAX;
+    const int32_t nominated = skip ? 0 : *(volatile int32_t*)&a.st->n_cand;
+    const bool too_many = nominated > 8;
+    const int32_t n_cand = too_many ? 0 : nominated;
+    int64_t limit = too_many ? -1 : INT64_MAX;
     if (n_cand > 0) {
         // ---- C: the vote at which a candidate's running count reaches the quorum ------------------------------------------------
         for (int c = 0; c < n_cand; ++c) {
@@ -743,7 +483,7 @@ __global__ void __launch_bounds__(TALLY_THREADS) k_fp_tally_cd(const TallyCdArgs
         grid.sync();
         limit = (int64_t)*(volatile int32_t*)&a.st->i_star;
     }
-    if (!was_decided) {
+    if (!skip) {
         // ---- D: votesReceived.add(sender) :141, count :142-144 for the votes up to the decision ------------------------------
         if (t == 0) s_recv = 0;
         __syncthreads();
@@ -751,7 +491,8 @@ __global__ void __launch_bounds__(TALLY_THREADS) k_fp_tally_cd(const TallyCdArgs
             const int64_t i = base + t;
             const int32_t e = i < c1 ? a.ent[i] : -1;
             const bool counted = e >= 0 && i <= limit;
-            if (counted) a.seen[a.ring0[a.rbegin + i]] = -1;
+            if (counted) a.seen[ARRAY ? a.sender[i] : a.ring0[a.rbegin + i]] = -1;
+            else if (ARRAY && e >= 0) a.seen[a.sender[i]] = INT_MAX;          // a first vote after the decision: ignored (:138)
             const unsigned m = __ballot_sync(0xffffffffu, counted);
             if (counted) {
                 const unsigned same = __match_any_sync(m, e);
@@ -772,18 +513,21 @@ __global__ void __launch_bounds__(TALLY_THREADS) k_fp_tally_cd(const TallyCdArgs
     const int32_t nc = st->n_call;
     for (int32_t q = t; q < nc; q += TALLY_THREADS) a.t_call[a.call_list[q]] = 0;
     if (t == 0) {
-        if (!was_decided && n_cand > 0 && st->i_star < INT_MAX) { st->decided = 1; st->decided_entry = a.ent[st->i_star]; st->decided_call = st->calls; }
+        if (n_cand > 0 && st->i_star < INT_MAX) {
+            st->decided = 1; st->decided_entry = a.ent[st->i_star];
+            if (!ARRAY) st->decided_call = st->calls;
+        }
         FPResult r;
         r.decided = st->decided; r.received = st->votes_received; r.len = 0; r.count = 0; r.h1 = 0; r.h2 = 0;
-        r.decided_call = st->decided_call; r.pad = 0;
-        st->calls = st->calls + 1;
+        r.decided_call = st->decided_call; r.bad_sender = st->bad_sender;
+        if (!ARRAY) st->calls = st->calls + 1;                // decided_call counts rapid_fp_tally_cd[_async] calls only
         if (r.decided && st->decided_entry >= 0) {
             const int32_t e = st->decided_entry;
             r.h1 = a.t_h1[e]; r.h2 = a.t_h2[e]; r.len = a.t_len[e]; r.count = *(volatile int32_t*)&a.t_count[e];
         }
-        if (st->too_many) r.decided = -1;                  // reported as RAPID_EUNSUPPORTED by the host
+        if (too_many) r.decided = -1;                        // reported as RAPID_EUNSUPPORTED by the host
         *a.out = r;
-        st->n_call = 0; st->n_cand = 0; st->n_valid_call = 0; st->i_star = INT_MAX; st->ticket = 0; st->too_many = 0;
+        st->n_call = 0; st->n_cand = 0; st->i_star = INT_MAX; st->bad_sender = -1; st->ticket = 0;
     }
 }
 
@@ -793,79 +537,43 @@ static int32_t fp_reset_call_state(FP* fp) {        // per-call fields only; no 
     return RAPID_OK;
 }
 
-// votes are device arrays here
-static int32_t tally_device(FP* fp, int64_t n, const int32_t* sender, const int64_t* vcfg, const uint64_t* h1,
-                            const uint64_t* h2, const int32_t* len, int allow_skip, bool exact_order, bool unique_senders = false) {
-    // exact_order == false (sharded tally): senders are this rank's own members, counts only -> no mid-call readback
-    cudaStream_t s = fp->stream;
-    const int TB = 256;
-    fp->last_launches = 0;
-    RAPID_CHECK(fp_reset_call_state(fp));
-    if (fp->decided_host || n == 0) return RAPID_OK;                 // :138 — everything after the decision is ignored
-    RAPID_CHECK(fp->ent.reserve((size_t)n));
-    const unsigned g = (unsigned)ceil_div<int64_t>(n, TB);
-    if (!unique_senders) {
-        k_fp_first<<<g, TB, 0, s>>>(n, sender, vcfg, fp->cfg, fp->sender_cap, allow_skip, fp->seen.p, fp->st.p);
-        fp->last_launches += 1;
+// the grid of k_fp_tally (co-resident blocks of the smaller instantiation, so that either runs on it) and its scratch for R votes
+static int32_t tally_reserve(FP* fp, int64_t R) {
+    if (fp->tally_grid == 0) {
+        int dev = 0, sms = TARGET_SMS, per_cd = 4, per_array = 4;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_cd, k_fp_tally<false>, TALLY_THREADS, 0);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_array, k_fp_tally<true>, TALLY_THREADS, 0);
+        fp->tally_grid = std::max(1, sms * std::max(std::min(per_cd, per_array), 1));
+        RAPID_CHECK(fp->blk_cnt.reserve((size_t)8 * fp->tally_grid));
     }
-    const bool direct = !exact_order && unique_senders;
-    k_fp_insert<<<g, TB, 0, s>>>(n, sender, vcfg, fp->cfg, fp->sender_cap, h1, h2, len, fp->seen.p, fp->T, fp->t_state.p,
-                                 fp->t_h1.p, fp->t_h2.p, fp->t_len.p, direct ? fp->t_count.p : fp->t_call.p, fp->ent.p, fp->st.p,
-                                 unique_senders ? 1 : 0, direct ? 1 : 0, fp->entries.p);
-    if (direct) { RAPID_KERNEL_CHECK(); fp->last_launches += 1; return RAPID_OK; }
-    const unsigned gt = (unsigned)ceil_div<uint32_t>(fp->T, TB);
-    k_fp_candidates<<<gt, TB, 0, s>>>(fp->T, fp->t_count.p, fp->t_call.p, (int32_t)fp->Q, fp->st.p);
-    RAPID_KERNEL_CHECK();
-    fp->last_launches += 2;
-    if (!exact_order) {
-        k_fp_apply<<<g, TB, 0, s>>>(n, sender, fp->ent.p, fp->st.p, 0, fp->seen.p, fp->t_count.p, fp->st.p);
-        k_fp_zero_call<<<gt, TB, 0, s>>>(fp->T, fp->t_call.p);
-        RAPID_KERNEL_CHECK();
-        fp->last_launches += 2;
-        return RAPID_OK;
-    }
-    RAPID_CUDA(cudaMemcpyAsync(fp->h_st.p, fp->st.p, sizeof(FPState), cudaMemcpyDeviceToHost, s));
-    RAPID_CUDA(cudaStreamSynchronize(s));
-    const FPState st = *fp->h_st.p;
-    auto rollback = [&]() {
-        k_fp_rollback<<<g, TB, 0, s>>>(n, sender, fp->sender_cap, fp->seen.p);
-        k_fp_zero_call<<<gt, TB, 0, s>>>(fp->T, fp->t_call.p);
-        cudaStreamSynchronize(s);
-    };
-    if (st.bad_sender >= 0) {
-        rollback();                                          // nothing of this call stays behind
-        set_error("vote %d: sender id outside [0, sender_capacity)", st.bad_sender);
-        return RAPID_EINVAL;
-    }
-    int use_istar = 0;
-    if (st.n_cand > 0 && exact_order) {
-        if (st.n_cand > 8) { rollback(); set_error("more than 8 proposals reached the quorum in one call"); return RAPID_EUNSUPPORTED; }
-        RAPID_CHECK(fp->scan.reserve((size_t)n));
-        for (int c = 0; c < st.n_cand; ++c) {
-            const int32_t e = st.cand[c];
-            k_fp_flag<<<g, TB, 0, s>>>(n, fp->ent.p, e, fp->scan.p);
-            RAPID_CHECK(exclusive_scan_i32(fp->scan.p, n, fp->scan_sums, nullptr, s, nullptr));
-            k_fp_find<<<g, TB, 0, s>>>(n, fp->ent.p, fp->scan.p, e, fp->t_count.p, (int32_t)fp->Q, fp->st.p);
-            fp->last_launches += 3;
-        }
-        k_fp_pick<<<1, 32, 0, s>>>(n, fp->ent.p, fp->st.p);
-        RAPID_KERNEL_CHECK();
-        fp->last_launches += 1;
-        use_istar = 1;
-    }
-    k_fp_apply<<<g, TB, 0, s>>>(n, sender, fp->ent.p, fp->st.p, use_istar, fp->seen.p, fp->t_count.p, fp->st.p);
-    k_fp_zero_call<<<gt, TB, 0, s>>>(fp->T, fp->t_call.p);
-    RAPID_KERNEL_CHECK();
-    fp->last_launches += 2;
+    return fp->ent.reserve((size_t)std::max<int64_t>(R, 1));
+}
+
+// launch k_fp_tally over ta.R votes (ta holds their source; tally_reserve(fp, ta.R) came first) on the tally's stream; the
+// result record goes to d_res_raw
+static int32_t tally_launch(FP* fp, TallyArgs& ta, bool array) {
+    ta.sender_cap = fp->sender_cap; ta.seen = fp->seen.p; ta.T = fp->T;
+    ta.t_state = fp->t_state.p; ta.t_h1 = fp->t_h1.p; ta.t_h2 = fp->t_h2.p; ta.t_len = fp->t_len.p;
+    ta.t_count = fp->t_count.p; ta.t_call = fp->t_call.p; ta.ent = fp->ent.p;
+    ta.entries = fp->entries.p; ta.call_list = fp->call_list.p; ta.blk_cnt = fp->blk_cnt.p;
+    ta.st = fp->st.p; ta.Q = (int32_t)fp->Q; ta.sumbuf = fp->sumbuf.p;
+    ta.out = (FPResult*)fp->d_res_raw.p;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(fp->tally_grid, ceil_div<int64_t>(ta.R, TALLY_THREADS)));
+    void* args[] = {(void*)&ta};
+    RAPID_CUDA(cudaLaunchCooperativeKernel(array ? (void*)k_fp_tally<true> : (void*)k_fp_tally<false>, dim3((unsigned)grid),
+                                           dim3(TALLY_THREADS), args, 0, fp->stream));
+    fp->last_launches = 1;
     return RAPID_OK;
 }
 
-static int32_t read_result(FP* fp, int32_t* decided, uint64_t* dh1, uint64_t* dh2, int32_t* dlen, int32_t* dcount, int32_t* received) {
-    k_fp_result<<<1, 1, 0, fp->stream>>>(fp->st.p, fp->t_h1.p, fp->t_h2.p, fp->t_len.p, fp->t_count.p, (FPResult*)fp->d_res_raw.p);
-    RAPID_KERNEL_CHECK();
-    RAPID_CUDA(cudaMemcpyAsync(fp->h_res_raw.p, (FPResult*)fp->d_res_raw.p, sizeof(FPResult), cudaMemcpyDeviceToHost, fp->stream));
-    RAPID_CUDA(cudaStreamSynchronize(fp->stream));
+// the host copy of k_fp_tally's result record -> the caller's outputs, or the refusal it reports
+static int32_t take_result(FP* fp, int32_t* decided, uint64_t* dh1, uint64_t* dh2, int32_t* dlen, int32_t* dcount, int32_t* received,
+                           int32_t* decided_in_call) {
     const FPResult r = *(const FPResult*)fp->h_res_raw.p;
+    if (r.bad_sender >= 0) { set_error("vote %d: sender id outside [0, sender_capacity)", r.bad_sender); return RAPID_EINVAL; }
+    if (r.decided < 0) { set_error("more than 8 proposals reached the quorum in one call"); return RAPID_EUNSUPPORTED; }
     fp->decided_host = r.decided != 0;
     if (decided) *decided = r.decided;
     if (received) *received = r.received;
@@ -873,6 +581,7 @@ static int32_t read_result(FP* fp, int32_t* decided, uint64_t* dh1, uint64_t* dh
     if (dh2) *dh2 = r.h2;
     if (dlen) *dlen = r.len;
     if (dcount) *dcount = r.count;
+    if (decided_in_call) *decided_in_call = r.decided_call;
     return RAPID_OK;
 }
 
@@ -967,23 +676,28 @@ int32_t rapid_fp_tally(rapid_fp* fp, int64_t n_votes, const int32_t* sender, con
     if (!fp || n_votes < 0 || (n_votes && (!sender || !proposal_hash))) { set_error("bad arguments"); return RAPID_EINVAL; }
     DeviceGuard g(fp->device);
     cudaStream_t s = fp->stream;
-    const size_t m = (size_t)std::max<int64_t>(n_votes, 1);
+    const int64_t n = fp->decided_host ? 0 : n_votes;      // :138 — everything after the decision is ignored
+    const size_t m = (size_t)std::max<int64_t>(n, 1);
     RAPID_CHECK(fp->v_sender.reserve(m));
     RAPID_CHECK(fp->v_h1.reserve(m));
+    RAPID_CHECK(tally_reserve(fp, n));
     RAPID_CUDA(cudaEventRecord(fp->ev0, s));
-    if (n_votes) {
-        RAPID_CUDA(cudaMemcpyAsync(fp->v_sender.p, sender, (size_t)n_votes * 4, cudaMemcpyHostToDevice, s));
-        RAPID_CUDA(cudaMemcpyAsync(fp->v_h1.p, proposal_hash, (size_t)n_votes * 8, cudaMemcpyHostToDevice, s));
-        if (vote_cfg) { RAPID_CHECK(fp->v_cfg.reserve(m)); RAPID_CUDA(cudaMemcpyAsync(fp->v_cfg.p, vote_cfg, (size_t)n_votes * 8, cudaMemcpyHostToDevice, s)); }
-        if (proposal_hash2) { RAPID_CHECK(fp->v_h2.reserve(m)); RAPID_CUDA(cudaMemcpyAsync(fp->v_h2.p, proposal_hash2, (size_t)n_votes * 8, cudaMemcpyHostToDevice, s)); }
-        if (proposal_len) { RAPID_CHECK(fp->v_len.reserve(m)); RAPID_CUDA(cudaMemcpyAsync(fp->v_len.p, proposal_len, (size_t)n_votes * 4, cudaMemcpyHostToDevice, s)); }
+    if (n) {
+        RAPID_CUDA(cudaMemcpyAsync(fp->v_sender.p, sender, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+        RAPID_CUDA(cudaMemcpyAsync(fp->v_h1.p, proposal_hash, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+        if (vote_cfg) { RAPID_CHECK(fp->v_cfg.reserve(m)); RAPID_CUDA(cudaMemcpyAsync(fp->v_cfg.p, vote_cfg, (size_t)n * 8, cudaMemcpyHostToDevice, s)); }
+        if (proposal_hash2) { RAPID_CHECK(fp->v_h2.reserve(m)); RAPID_CUDA(cudaMemcpyAsync(fp->v_h2.p, proposal_hash2, (size_t)n * 8, cudaMemcpyHostToDevice, s)); }
+        if (proposal_len) { RAPID_CHECK(fp->v_len.reserve(m)); RAPID_CUDA(cudaMemcpyAsync(fp->v_len.p, proposal_len, (size_t)n * 4, cudaMemcpyHostToDevice, s)); }
     }
-    RAPID_CHECK(tally_device(fp, n_votes, fp->v_sender.p, vote_cfg ? fp->v_cfg.p : nullptr, fp->v_h1.p,
-                             proposal_hash2 ? fp->v_h2.p : nullptr, proposal_len ? fp->v_len.p : nullptr, 0, true));
+    TallyArgs ta = {};
+    ta.R = n; ta.sender = fp->v_sender.p; ta.vcfg = vote_cfg ? fp->v_cfg.p : nullptr; ta.cfg = fp->cfg;
+    ta.h1v = fp->v_h1.p; ta.h2v = proposal_hash2 ? fp->v_h2.p : nullptr; ta.lenv = proposal_len ? fp->v_len.p : nullptr;
+    RAPID_CHECK(tally_launch(fp, ta, true));
     RAPID_CUDA(cudaEventRecord(fp->ev1, s));
-    RAPID_CHECK(read_result(fp, decided, decided_hash, decided_hash2, decided_len, decided_count, votes_received));
+    RAPID_CUDA(cudaMemcpyAsync(fp->h_res_raw.p, fp->d_res_raw.p, sizeof(FPResult), cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
     cudaEventElapsedTime(&fp->last_ms, fp->ev0, fp->ev1);
-    return RAPID_OK;
+    return take_result(fp, decided, decided_hash, decided_hash2, decided_len, decided_count, votes_received, nullptr);
 }
 
 // enqueue the tally of the detector's votes (and, sharded, the all-reduce + decision kernel) on the tally's stream
@@ -993,16 +707,7 @@ static int32_t tally_cd_enqueue(rapid_fp* fp, const rapid_cd* cd, rapid_comm* co
     if (cd->raw) { set_error("RAW detectors do not announce proposals"); return RAPID_EINVAL; }
     if (comm && comm->device != fp->device) { set_error("comm and fp live on different devices"); return RAPID_EINVAL; }
     cudaStream_t s = fp->stream;
-    const int64_t R = cd->R;
-    RAPID_CHECK(fp->ent.reserve((size_t)R));
-    if (fp->tally_grid == 0) {
-        int dev = 0, sms = TARGET_SMS, per = 4;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_fp_tally_cd, TALLY_THREADS, 0);
-        fp->tally_grid = std::max(1, sms * std::max(per, 1));
-        RAPID_CHECK(fp->blk_cnt.reserve((size_t)8 * fp->tally_grid));
-    }
+    RAPID_CHECK(tally_reserve(fp, cd->R));
     // The detector's outputs are produced on ITS stream (possibly by an asynchronous batch still in flight): order this
     // tally after them on the device instead of waiting on the host.
     RAPID_CUDA(cudaStreamWaitEvent(s, cd->ev_done, 0));
@@ -1013,19 +718,11 @@ static int32_t tally_cd_enqueue(rapid_fp* fp, const rapid_cd* cd, rapid_comm* co
         RAPID_CHECK(fp->sumbuf.reserve(words));
         RAPID_CUDA(cudaMemsetAsync(fp->sumbuf.p, 0, words * sizeof(unsigned long long), s));
     }
-    TallyCdArgs ta;
-    ta.R = R; ta.rbegin = cd->rbegin; ta.rflags = cd->rflags.p; ta.ring0 = cd->view->ring.p;
+    TallyArgs ta = {};
+    ta.R = cd->R; ta.rbegin = cd->rbegin; ta.rflags = cd->rflags.p; ta.ring0 = cd->view->ring.p;
     ta.h1v = cd->out_h1.p; ta.h2v = cd->out_h2.p; ta.lenv = cd->out_len.p;
-    ta.sender_cap = fp->sender_cap; ta.seen = fp->seen.p; ta.T = fp->T;
-    ta.t_state = fp->t_state.p; ta.t_h1 = fp->t_h1.p; ta.t_h2 = fp->t_h2.p; ta.t_len = fp->t_len.p;
-    ta.t_count = fp->t_count.p; ta.t_call = fp->t_call.p; ta.ent = fp->ent.p;
-    ta.entries = fp->entries.p; ta.call_list = fp->call_list.p; ta.blk_cnt = fp->blk_cnt.p;
-    ta.st = fp->st.p; ta.Q = (int32_t)fp->Q; ta.direct = direct ? 1 : 0; ta.sumbuf = fp->sumbuf.p;
-    ta.out = (FPResult*)fp->d_res_raw.p;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(fp->tally_grid, ceil_div<int64_t>(R, TALLY_THREADS)));
-    void* args[] = {(void*)&ta};
-    RAPID_CUDA(cudaLaunchCooperativeKernel((void*)k_fp_tally_cd, dim3((unsigned)grid), dim3(TALLY_THREADS), args, 0, s));
-    fp->last_launches = 1;
+    ta.direct = direct ? 1 : 0;
+    RAPID_CHECK(tally_launch(fp, ta, false));
     fp->pending_comm = comm;
     fp->pending_cd = cd;
     if (direct && getenv("RAPID_B200_FORCE_REFINE") == nullptr) {
@@ -1053,19 +750,8 @@ static int32_t tally_cd_collect(rapid_fp* fp, int32_t* decided, uint64_t* decide
     cudaGetLastError();
     if (fp->pending_cd) RAPID_CHECK(cd_wait(fp->pending_cd, true));      // outcome of the (asynchronous) batches these votes came from
     rapid_comm* comm = fp->pending_comm;
-    if (comm == nullptr) {
-        const FPResult r = *(const FPResult*)fp->h_res_raw.p;
-        if (r.decided < 0) { set_error("more than 8 proposals reached the quorum in one call"); return RAPID_EUNSUPPORTED; }
-        fp->decided_host = r.decided != 0;
-        if (decided) *decided = r.decided;
-        if (votes_received) *votes_received = r.received;
-        if (decided_hash) *decided_hash = r.h1;
-        if (decided_hash2) *decided_hash2 = r.h2;
-        if (decided_len) *decided_len = r.len;
-        if (decided_count) *decided_count = r.count;
-        if (decided_in_call) *decided_in_call = r.decided_call;
-        return RAPID_OK;
-    }
+    if (comm == nullptr)
+        return take_result(fp, decided, decided_hash, decided_hash2, decided_len, decided_count, votes_received, decided_in_call);
     if (getenv("RAPID_B200_FORCE_REFINE") == nullptr) {
         const FPSumResult res = *(const FPSumResult*)fp->h_res_raw.p;
         if (!res.ambiguous) {

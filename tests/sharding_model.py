@@ -42,7 +42,7 @@ def decide(global_hist, global_words_of, quorum):
     return True, int(w[0]), int(w[2]), int(w[4]), int(global_hist[b])
 
 
-# ---- the single-all-reduce protocol (csrc/fast_paxos.cu: k_fp_hist_sum / k_fp_decide_sum_impl) ---------------------
+# ---- the single-all-reduce protocol (csrc/fast_paxos.cu: phase S of k_fp_tally / k_fp_decide_sum) ------------------
 SUM_BUCKETS, SUM_WORDS = 4096, 8
 _M64 = (1 << 64) - 1
 

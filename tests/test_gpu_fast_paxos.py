@@ -1,7 +1,10 @@
 """FastPaxos fast-round tally on the GPU vs the reference's FastPaxosWithoutFallbackTests tables
-(rapid/src/test/java/com/vrg/rapid/FastPaxosWithoutFallbackTests.java:85-90, :129-148) and vs the oracle."""
+(rapid/src/test/java/com/vrg/rapid/FastPaxosWithoutFallbackTests.java:85-90, :129-148), vs the oracle, and vs
+plainref.FastRound on host-array streams that span many blocks of the tally kernel."""
 import numpy as np
 import pytest
+
+import plainref
 
 pytestmark = pytest.mark.gpu
 
@@ -92,15 +95,17 @@ def test_bad_sender_rejected(rb):
 
 
 def test_a_refused_call_leaves_no_trace(rb):
-    """a call that is refused (a sender id outside the table) must not poison the tally: the senders it named can still vote"""
-    N = 40
-    fp = rb.FastPaxos(7, N, sender_capacity=N)
-    good = np.arange(10, dtype=np.int32)
-    with pytest.raises(rb.RapidError):
-        fp.handleFastRoundProposals(np.concatenate([good, [N + 5]]).astype(np.int32), np.full(11, 99, np.uint64))
-    q = rb.quorum(N)
-    t = fp.handleFastRoundProposals(np.arange(q, dtype=np.int32), np.full(q, 99, np.uint64))
-    assert t.decided and t.count == q and t.votes_received == q          # senders 0..9 were NOT burnt by the refused call
+    """a call that is refused (a sender id outside the table) must not poison the tally: the senders it named can still vote;
+    with 50,000 good votes the bad sender sits in a later block than the good ones"""
+    for N, n_good in [(40, 10), (100_000, 50_000)]:
+        fp = rb.FastPaxos(7, N, sender_capacity=N)
+        good = np.arange(n_good, dtype=np.int32)
+        with pytest.raises(rb.RapidError) as e:
+            fp.handleFastRoundProposals(np.concatenate([good, [N + 5]]).astype(np.int32), np.full(n_good + 1, 99, np.uint64))
+        assert e.value.code == rb._native.EINVAL and "vote %d:" % n_good in str(e.value), N
+        q = rb.quorum(N)
+        t = fp.handleFastRoundProposals(np.arange(q, dtype=np.int32), np.full(q, 99, np.uint64))
+        assert t.decided and t.count == q and t.votes_received == q, N   # the good senders were NOT burnt by the refused call
 
 
 def test_tally_from_cluster(orc, rb):
@@ -138,6 +143,8 @@ def test_empty_calls_and_reset(rb):
     assert not r.decided and r.votes_received == 6
     r = fp.handleFastRoundProposals([6], [h[0]], [h[1]], [2], vote_cfg=[CFG + 1])
     assert r.decided and r.votes_received == 7 and (r.hash, r.hash2, r.length) == (h[0], h[1], 2)
+    r = fp.handleFastRoundProposals([99], [h[0]], [h[1]], [2], vote_cfg=[CFG + 1])                # after the decision: not checked
+    assert r.decided and r.votes_received == 7 and r.count == 7 and (r.hash, r.hash2, r.length) == (h[0], h[1], 2)
 
 
 def test_many_distinct_proposals_never_decide(rb):
@@ -147,3 +154,101 @@ def test_many_distinct_proposals_never_decide(rb):
     hs = np.array([rb.proposal_fingerprint([i, i + 1]) for i in range(n)], dtype=np.uint64)
     r = fp.handleFastRoundProposals(np.arange(n), hs[:, 0], hs[:, 1], np.full(n, 2))
     assert not r.decided and r.votes_received == n
+
+
+# ---------------------------------------------------------------- host-array streams over many blocks vs plainref.FastRound -------
+BLOCK = 256                 # k_fp_tally gives every block a multiple of 256 votes
+SPAN = 1536                 # ... and 1,536 of 10^6 votes on an H100 SXM (132 SMs x 5 co-resident blocks)
+
+
+def _vote_stream(rb, rng, nv, cap, weights, p_stale=0.05):
+    """nv votes by senders drawn with repeats from [0, cap), proposal k with weight weights[k], a fraction p_stale of them for
+    the next configuration"""
+    props = [tuple(rb.proposal_fingerprint(list(range(100 * k, 100 * k + k + 1)))) + (k + 1,) for k in range(len(weights))]
+    pid = rng.choice(len(weights), size=nv, p=weights)
+    table = np.array(props, np.uint64)
+    return dict(senders=rng.integers(0, cap, size=nv).astype(np.int32), pid=pid, props=props, h1=table[pid, 0], h2=table[pid, 1],
+                ln=table[pid, 2].astype(np.int32), vcfg=np.where(rng.random(nv) < p_stale, CFG + 1, CFG).astype(np.int64))
+
+
+def _tally(fp, v, sl=slice(None)):
+    return fp.handleFastRoundProposals(v["senders"][sl], v["h1"][sl], v["h2"][sl], v["ln"][sl], vote_cfg=v["vcfg"][sl])
+
+
+def _ref_call(ref, v, sl=slice(None)):
+    """the reference has no configuration ids: the stale votes are dropped before it sees them; returns the kept indices"""
+    keep = np.nonzero(v["vcfg"][sl] == CFG)[0]
+    ref.call(v["senders"][sl][keep], [v["props"][p] for p in v["pid"][sl][keep].tolist()])
+    return keep
+
+
+def _same(t, ref, what):
+    assert t.decided == ref.decided, what
+    assert t.votes_received == ref.votes_received, what
+    if ref.decided:
+        assert (t.hash, t.hash2, t.length) == ref.decision and t.count == ref.count, what
+
+
+def _first_votes(v, sl=slice(None)):
+    """index (within sl) of every sender's first vote of this configuration"""
+    ok = np.nonzero(v["vcfg"][sl] == CFG)[0]
+    s, first = np.unique(v["senders"][sl][ok], return_index=True)
+    return s, ok[first]
+
+
+@pytest.mark.parametrize("nv", [100_000, 1_000_000])
+def test_multi_block_stream_one_call(rb, nv):
+    """one call of nv votes by senders that vote again in later blocks, two proposals 80 : 20, stale votes mixed in: the quorum
+    is reached mid-array inside a later block, and the first votes of new senders after it are not counted"""
+    N = 2 * nv // 5
+    cap = 2 * N
+    v = _vote_stream(rb, np.random.default_rng(nv), nv, cap, [0.8, 0.2])
+    ref = plainref.FastRound(N)
+    keep = _ref_call(ref, v)
+    assert ref.decided
+    i_star = int(keep[ref.decided_at[1]])
+    assert i_star >= 4 * SPAN and i_star % BLOCK not in (0, BLOCK - 1)          # inside a later block, not at its edge
+    s, first = _first_votes(v)
+    assert (first > i_star).sum() > 1000                                         # new senders after the decision
+    ok = np.nonzero(v["vcfg"] == CFG)[0]
+    late = ok - first[np.searchsorted(s, v["senders"][ok])] > 2 * SPAN
+    assert (ok[late] < i_star).sum() > 1000                                       # repeats blocks after the first vote
+    fp = rb.FastPaxos(CFG, N, sender_capacity=cap)
+    t = _tally(fp, v)
+    _same(t, ref, "decision")
+    assert t.votes_received == (first <= i_star).sum() < len(s)
+    _same(_tally(fp, v, slice(0, 1000)), ref, "after the decision")
+
+
+def test_multi_block_stream_three_calls(rb):
+    """the same stream in three calls: the first two stay below the quorum (repeats of their senders in later calls are
+    ignored), the third reaches it mid-array inside a later block"""
+    nv = 1_000_000
+    N = 2 * nv // 5
+    cap = 2 * N
+    v = _vote_stream(rb, np.random.default_rng(3), nv, cap, [0.8, 0.2])
+    cuts = [0, nv // 5 + 77, 2 * nv // 5 + 131, nv]
+    fp = rb.FastPaxos(CFG, N, sender_capacity=cap)
+    ref = plainref.FastRound(N)
+    for c in range(3):
+        sl = slice(cuts[c], cuts[c + 1])
+        keep = _ref_call(ref, v, sl)
+        assert ref.decided == (c == 2), c
+        _same(_tally(fp, v, sl), ref, c)
+    i_star = int(keep[ref.decided_at[1]])
+    assert ref.decided_at[0] == 2 and i_star >= 4 * SPAN and i_star % BLOCK not in (0, BLOCK - 1)
+
+
+def test_more_than_8_proposals_reaching_the_quorum_refuse_the_call(rb):
+    """N = 5 (quorum 4): 9 proposals with 4 senders each cross the quorum in one call, which is refused and leaves no trace:
+    the same senders then decide one proposal with exactly the quorum"""
+    fp = rb.FastPaxos(CFG, 5, sender_capacity=40)
+    hs = [rb.proposal_fingerprint([k]) for k in range(9)]
+    senders = np.arange(36, dtype=np.int32)
+    with pytest.raises(rb.RapidError) as e:
+        fp.handleFastRoundProposals(senders, [hs[k // 4][0] for k in range(36)], [hs[k // 4][1] for k in range(36)], [1] * 36)
+    assert e.value.code == rb._native.EUNSUPPORTED
+    again = [35, 2, 17, 8, 30]                      # one sender from each of five groups; the fourth vote decides
+    r = fp.handleFastRoundProposals(again, [hs[8][0]] * 5, [hs[8][1]] * 5, [1] * 5)
+    assert r.decided and (r.hash, r.hash2, r.length) == (hs[8][0], hs[8][1], 1)
+    assert r.count == 4 and r.votes_received == 4

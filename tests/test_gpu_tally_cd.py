@@ -1,4 +1,4 @@
-"""The fast-round tally of a detector's own votes (csrc/fast_paxos.cu: k_fp_tally_cd, the kernel that decides every bench.py step)
+"""The fast-round tally of a detector's own votes (csrc/fast_paxos.cu: k_fp_tally, the kernel that decides every bench.py step)
 against plainref.FastRound, field by field, on votes that conflict.
 
 The votes come from the detector itself.  A handful of nodes crash and every receiver hears of them; the alerts about a few
@@ -22,7 +22,7 @@ import plainref
 from rapid_b200 import workloads as W
 
 K, H, L = 10, 9, 4
-BLOCK = 256                 # k_fp_tally_cd gives every block a multiple of 256 receivers
+BLOCK = 256                 # k_fp_tally gives every block a multiple of 256 receivers
 
 
 # ---------------------------------------------------------------- the reference itself, against the oracle (CPU) ------------------
