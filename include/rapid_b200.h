@@ -362,7 +362,9 @@ int32_t rapid_pxa_create(rapid_pxa** out, int64_t cfg_id, int64_t n_acceptors, i
 int32_t rapid_pxa_destroy(rapid_pxa* a);
 int32_t rapid_pxa_reset(rapid_pxa* a, int64_t cfg_id);      /* rnd = vrnd = (0, 0), vval = [] (:82-85) for every acceptor */
 /* registerFastRoundVote :244-257 for the listed acceptors (local indexes): skipped where rnd.round > 1, else
- * rnd = vrnd = (1, 1), vval = the vote. */
+ * rnd = vrnd = (1, 1), vval = the vote.  An acceptor listed more than once ends with its LAST listed vote, whole, as calls
+ * made one by one in list order would leave it.  An index outside [0, n_acceptors) gives RAPID_EINVAL and changes no
+ * acceptor.  n <= 0x7ffffff0. */
 int32_t rapid_pxa_register_fast_round_votes(rapid_pxa* a, int64_t n, const int64_t* acceptor, const uint64_t* hash,
                                             const uint64_t* hash2, const int32_t* len);
 /* Same, straight from a detector's device-resident outputs: every receiver that announced a proposal in the last batch

@@ -195,7 +195,7 @@ class PaxosAcceptors:
         N.check(N.lib().rapid_pxa_reset(self._h, self.cfg))
 
     def registerFastRoundVotes(self, acceptor, value_hash, value_len, value_hash2=None):
-        """:244-257 for the listed acceptors"""
+        """:244-257 for the listed acceptors, as one-by-one calls in list order: an acceptor listed twice keeps its last vote"""
         a = N.as_i64(acceptor)
         h1, ln = _u64(value_hash), N.as_i32(value_len)
         h2 = None if value_hash2 is None else _u64(value_hash2)

@@ -300,15 +300,27 @@ __global__ void k_pxa_init(int64_t R, int64_t* rnd, int64_t* vrnd, uint64_t* h1,
     if (r >= R) return;
     rnd[r] = pack_rank(0, 0); vrnd[r] = pack_rank(0, 0); h1[r] = 0; h2[r] = 0; len[r] = 0;     // Paxos.java:82-85
 }
-// registerFastRoundVote (:244-257).  acceptor == NULL: acceptor r takes vote r where flag[r] has RF_ANN_NOW.
-__global__ void k_pxa_register(int64_t n, const int64_t* __restrict__ acceptor, const uint32_t* __restrict__ rflags, int64_t R,
-                               const uint64_t* __restrict__ vh1, const uint64_t* __restrict__ vh2, const int32_t* __restrict__ vlen,
-                               int64_t* __restrict__ rnd, int64_t* __restrict__ vrnd, uint64_t* __restrict__ h1,
-                               uint64_t* __restrict__ h2, int32_t* __restrict__ len, int32_t* __restrict__ bad) {
+// A list of votes may name an acceptor more than once: win[r] (-1 before the call) becomes the last list index naming r.
+__global__ void k_pxa_claim(int64_t n, const int64_t* __restrict__ acceptor, int64_t R, int32_t* __restrict__ win,
+                            int32_t* __restrict__ bad) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int64_t r = acceptor[i];
+    if (r < 0 || r >= R) { atomicExch(bad, 1); return; }
+    atomicMax(&win[r], (int32_t)i);
+}
+// registerFastRoundVote (:244-257).  acceptor == NULL: acceptor r takes vote r where flag[r] has RF_ANN_NOW.  With a list,
+// only the entry k_pxa_claim left in win[r] writes acceptor r, so r ends with its last listed vote whole, as calls made one by
+// one in list order would leave it; a list naming an acceptor out of range (*bad) writes nothing.
+__global__ void k_pxa_register(int64_t n, const int64_t* __restrict__ acceptor, const int32_t* __restrict__ win,
+                               const uint32_t* __restrict__ rflags, const uint64_t* __restrict__ vh1,
+                               const uint64_t* __restrict__ vh2, const int32_t* __restrict__ vlen, int64_t* __restrict__ rnd,
+                               int64_t* __restrict__ vrnd, uint64_t* __restrict__ h1, uint64_t* __restrict__ h2,
+                               int32_t* __restrict__ len, const int32_t* __restrict__ bad) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     int64_t r = i;
-    if (acceptor) { r = acceptor[i]; if (r < 0 || r >= R) { atomicExch(bad, 1); return; } }
+    if (acceptor) { if (*bad) return; r = acceptor[i]; if (win[r] != (int32_t)i) return; }
     else if (!(rflags[i] & RF_ANN_NOW)) return;
     if (rank_round(rnd[r]) > 1) return;                                              // :246-248
     rnd[r] = pack_rank(1, 1); vrnd[r] = pack_rank(1, 1);                             // :254-255
@@ -429,7 +441,7 @@ struct PXA {
     DevBuf<uint64_t> o_h1, o_h2;
     DevBuf<int32_t> scan_sums;
     PinnedBuf<int32_t> h_total;
-    DevBuf<int32_t> bad;
+    DevBuf<int32_t> bad, win;              // win: last list entry per acceptor of a vote registration
     DevBuf<int64_t> s_acc;
     DevBuf<uint64_t> s_h1, s_h2;
     DevBuf<int32_t> s_len;
@@ -1023,14 +1035,17 @@ int32_t rapid_pxa_destroy(rapid_pxa* a) {
 int32_t rapid_pxa_register_fast_round_votes(rapid_pxa* a, int64_t n, const int64_t* acceptor, const uint64_t* hash, const uint64_t* hash2,
                                             const int32_t* len) {
     if (!a) { set_error("NULL handle"); return RAPID_EINVAL; }
-    if (n < 0 || (n && (!acceptor || !hash || !len))) { set_error("bad arguments"); return RAPID_EINVAL; }
+    if (n < 0 || n > 0x7ffffff0LL || (n && (!acceptor || !hash || !len))) { set_error("bad arguments"); return RAPID_EINVAL; }
     if (n == 0) return RAPID_OK;
     DeviceGuard g(a->device);
     cudaStream_t s = a->stream;
     RAPID_CHECK(upload(a->s_acc, acceptor, n, s)); RAPID_CHECK(upload(a->s_h1, hash, n, s)); RAPID_CHECK(upload(a->s_len, len, n, s));
     if (hash2) RAPID_CHECK(upload(a->s_h2, hash2, n, s));
-    k_pxa_register<<<grid_for(n), TB, 0, s>>>(n, a->s_acc.p, nullptr, a->R, a->s_h1.p, hash2 ? a->s_h2.p : nullptr, a->s_len.p, a->rnd.p,
-                                              a->vrnd.p, a->h1.p, a->h2.p, a->len.p, a->bad.p);
+    RAPID_CHECK(a->win.reserve((size_t)a->R));
+    RAPID_CUDA(cudaMemsetAsync(a->win.p, 0xff, (size_t)a->R * sizeof(int32_t), s));
+    k_pxa_claim<<<grid_for(n), TB, 0, s>>>(n, a->s_acc.p, a->R, a->win.p, a->bad.p);
+    k_pxa_register<<<grid_for(n), TB, 0, s>>>(n, a->s_acc.p, a->win.p, nullptr, a->s_h1.p, hash2 ? a->s_h2.p : nullptr, a->s_len.p,
+                                              a->rnd.p, a->vrnd.p, a->h1.p, a->h2.p, a->len.p, a->bad.p);
     RAPID_KERNEL_CHECK();
     RAPID_CUDA(cudaMemcpyAsync(a->h_total.p, a->bad.p, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     RAPID_CUDA(cudaStreamSynchronize(s));
@@ -1048,7 +1063,7 @@ int32_t rapid_pxa_register_fast_round_votes_cd(rapid_pxa* a, const rapid_cd* cd)
     if (cd->R != a->R) { set_error("detector has %lld receivers, handle has %lld acceptors", (long long)cd->R, (long long)a->R); return RAPID_EINVAL; }
     DeviceGuard g(a->device);
     RAPID_CUDA(cudaStreamSynchronize(cd->stream));            // the detector's outputs are produced on its own stream
-    k_pxa_register<<<grid_for(a->R), TB, 0, a->stream>>>(a->R, nullptr, cd->rflags.p, a->R, cd->out_h1.p, cd->out_h2.p, cd->out_len.p,
+    k_pxa_register<<<grid_for(a->R), TB, 0, a->stream>>>(a->R, nullptr, nullptr, cd->rflags.p, cd->out_h1.p, cd->out_h2.p, cd->out_len.p,
                                                          a->rnd.p, a->vrnd.p, a->h1.p, a->h2.p, a->len.p, a->bad.p);
     RAPID_KERNEL_CHECK();
     RAPID_CUDA(cudaStreamSynchronize(a->stream));

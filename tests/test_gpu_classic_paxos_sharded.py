@@ -337,20 +337,35 @@ def test_conflicting_fast_round_on_sharded_clusters(orc, rb, comm):
 
 
 def test_one_million_acceptors_in_eight_shards(rb, comm):
-    """test_one_million_acceptors_classic_round's expectations with the acceptors in 8 uneven shards listed out of order"""
+    """test_one_million_acceptors_classic_round's expectations with the acceptors in 8 uneven shards listed out of order,
+    holding the Zipf-spread votes of test_gpu_classic_paxos_scale.py: every answer checked against tests/plainref.py, the
+    Phase1b answers delivered in acceptor order and in a permuted order"""
+    import plainref as P
+    from test_gpu_classic_paxos_scale import zipf_votes
     n = 1_000_000
     edges = [0, 1, 90_000, 250_000, 250_001, 500_000, 640_000, 999_999, n]
     shards = [rb.PaxosAcceptors(9, b - a, acceptor_begin=a) for a, b in zip(edges, edges[1:])]
+    voters, h1, h2, ln = zipf_votes(n, 8)
+    ref = P.Acceptors(9, n)
+    ref.registerFastRoundVotes(voters, h1, ln, h2)
     for (a, b), s in zip(zip(edges, edges[1:]), shards):
-        ids = np.arange(a, b, dtype=np.int64)
-        s.registerFastRoundVotes(ids - a, np.where(ids % 10 < 7, np.uint64(111), np.uint64(222)).astype(np.uint64),
-                                 np.full(b - a, 3, np.int32))
+        sel = (voters >= a) & (voters < b)
+        s.registerFastRoundVotes(voters[sel] - a, h1[sel], ln[sel], h2[sel])
     listed = [shards[i] for i in (5, 0, 7, 2, 6, 1, 4, 3)]
-    px = rb.Paxos(9, n, message_capacity=n)
-    px.startPhase1a(2, 2)
-    assert sum(s.handlePhase1aMessage((2, 2)) for s in listed) == n
-    got = px.handlePhase1bFromAcceptorShards(listed, comm=comm)
-    assert got.proposed and got.trigger_index == n // 2 and got.cval == (111, 0, 3) and got.n_messages == n
-    assert sum(s.handlePhase2aMessage((2, 2), got.cval) for s in listed) == n
+    assert sum(s.handlePhase1aMessage((2, 2)) for s in listed) == ref.phase1a((2, 2)) == n
+    cval = None
+    for perm in (0, 31337):
+        px, coord = rb.Paxos(9, n, message_capacity=n), P.Coordinator(n, 9)
+        assert px.startPhase1a(2, 2) and coord.startPhase1a(2, 2)
+        got = px.handlePhase1bFromAcceptorShards(listed, comm=comm, perm_seed=perm)
+        assert (got.proposed, got.trigger_index, got.cval, got.n_messages) == ref.deliver1b(coord, perm)
+        assert got.proposed and got.trigger_index == n // 2 and got.n_messages == n
+        cval = cval or got.cval
+    assert sum(s.handlePhase2aMessage((2, 2), cval) for s in listed) == ref.phase2a((2, 2), cval) == n
     dec = rb.Paxos(9, n, message_capacity=n).handlePhase2bFromAcceptorShards(listed, comm=comm, perm_seed=4242)
-    assert dec.decided and dec.decided_index == n // 2 and dec.decision == (111, 0, 3)
+    assert (dec.decided, dec.decided_index, dec.decision) == ref.deliver2b(P.Learner(n, 9), 4242)
+    assert dec.decided and dec.decided_index == n // 2 and dec.decision == cval
+    rng = np.random.default_rng(2)
+    for r in sorted(set(rng.choice(n, size=1000, replace=False).tolist()) | {0, n - 1, 90_000, 250_000}):
+        s = max(i for i, e in enumerate(edges[:-1]) if e <= r)
+        assert shards[s].read(r - edges[s]) == ref.read(r), r
