@@ -453,6 +453,54 @@ int32_t rapid_wire_decode_votes(rapid_wire* w, const uint8_t* bytes, const int64
                                 int32_t* proposal_len);
 int32_t rapid_wire_last_device_ms(const rapid_wire* w, float* total_ms);
 
+/* Consensus messages (rapid.proto:124-169).  A kind is the message's RapidRequest oneof case (rapid.proto:21-35). */
+#define RAPID_WIRE_FAST_ROUND_PHASE2B 5   /* FastRoundPhase2bMessage {sender 1, configurationId 2, endpoints 3}          */
+#define RAPID_WIRE_PHASE1A            6   /* Phase1aMessage {sender 1, configurationId 2, rank 3}                        */
+#define RAPID_WIRE_PHASE1B            7   /* Phase1bMessage {sender 1, configurationId 2, rnd 3, vrnd 4, vval 5}         */
+#define RAPID_WIRE_PHASE2A            8   /* Phase2aMessage {sender 1, configurationId 2, rnd 3, vval 5}                 */
+#define RAPID_WIRE_PHASE2B            9   /* Phase2bMessage {sender 1, configurationId 2, rnd 3, endpoints 4}            */
+/* n serialized messages of one kind, message i = bytes[off[i] .. off[i+1]) (off non-decreasing, within [0, 0x7ffffff0]).
+ * With RAPID_WIRE_REQUEST each is a RapidRequest whose content must be the `kind` case: repeated occurrences of it merge,
+ * another case occurring later replaces it, and a request whose content is not (or no longer) that case is malformed.
+ * Per message, on the device: the sender id (-1 for an endpoint outside the dictionary, or an absent sender); the
+ * configurationId; the rank — `rank` for Phase1a, `rnd` for Phase1b / 2a / 2b, (0, 0) for the fast round; `vrnd` for Phase1b,
+ * else (0, 0); and the list as rapid_proposal_fingerprint of its ids plus its length.  Parsing follows the protobuf runtime:
+ * proto3 defaults for absent fields (an absent Rank is (0, 0)), a repeated singular Rank or Endpoint is merged field by field,
+ * an int32 is the low 32 bits of its varint, a field with an unexpected wire type and any unknown field is skipped (group
+ * encodings, which rapid.proto never uses, are refused as malformed).  Malformed or truncated bytes give RAPID_EINVAL
+ * ("malformed Phase1bMessage at index i", ...).
+ * An endpoint outside the dictionary enters the fingerprint through its ring-0 key, exactly as in rapid_wire_decode_votes
+ * (which is this decoder for kind 5): one list has one fingerprint whichever kind carries it, equal to the detector's
+ * proposal fingerprint when every endpoint is known, so a value compares equal from fast-round vote to acceptor vval to
+ * Phase1b, Phase2a and Phase2b.  Identity is ORDER-INSENSITIVE, as for votes: every well-formed value is a ring-0-sorted list
+ * (MembershipService.java:346-348).  Outputs (may be NULL): messages whose sender is not in the dictionary, and list entries
+ * that are not.  The decoded messages stay on the device for rapid_px_phase1b_wire / rapid_px_phase2b_wire /
+ * rapid_fp_tally_wire.  Every decode on the handle (alerts included) replaces the last one; after a refused decode the
+ * handle holds no consensus decode. */
+int32_t rapid_wire_decode_consensus(rapid_wire* w, int32_t kind, const uint8_t* bytes, const int64_t* off, int64_t n,
+                                    uint32_t flags, int64_t* n_unknown_senders, int64_t* n_unknown_endpoints);
+/* Host copies of the per-message fields of the last consensus decode (arrays of n; each may be NULL). */
+int32_t rapid_wire_read_consensus(const rapid_wire* w, int32_t* sender, int64_t* cfg, int32_t* rnd_round, int32_t* rnd_node,
+                                  int32_t* vrnd_round, int32_t* vrnd_node, uint64_t* h1, uint64_t* h2, int32_t* len);
+/* The list of message `index` of the last consensus decode as ids in wire order (-1 for an endpoint outside the dictionary):
+ * writes min(cap, len) ids, *out_len = len.  Turns a trigger_index / decided_index back into a List<Endpoint>. */
+int32_t rapid_wire_consensus_value(const rapid_wire* w, int64_t index, int32_t* out_ids, int32_t cap, int32_t* out_len);
+/* The decoded messages of `w` handed to the tallies without leaving the device: rapid_px_phase1b / rapid_px_phase2b /
+ * rapid_fp_tally over them in message order, same device code, same outputs; trigger / decided indexes are message indexes
+ * of the decode.  RAPID_EINVAL, with the px / fp unchanged, if the last decode on w is not a successful decode of the
+ * matching kind (Phase1b, Phase2b, FastRoundPhase2b), if w lives on another device, or (Phase2b and the fast round) if a
+ * message OF THE CURRENT CONFIGURATION comes from an endpoint outside the dictionary.  Messages of another configuration are
+ * dropped first, whatever their sender (Paxos.java:224, FastPaxos.java:126), so a delayed message from a node that has
+ * since left is simply ignored.  The reference would count an unknown current-configuration sender as one more distinct
+ * sender; members are the only senders in well-formed traffic, and collapsing unknown senders into one id would undercount
+ * distinct senders, so the call is refused instead.  Phase1b never looks at its sender (handlePhase1bMessage appends). */
+int32_t rapid_px_phase1b_wire(rapid_px* px, const rapid_wire* w, int32_t* proposed, int64_t* trigger_index, uint64_t* cval_hash,
+                              uint64_t* cval_hash2, int32_t* cval_len, int64_t* n_messages);
+int32_t rapid_px_phase2b_wire(rapid_px* px, const rapid_wire* w, int32_t* decided, int64_t* decided_index, uint64_t* decided_hash,
+                              uint64_t* decided_hash2, int32_t* decided_len);
+int32_t rapid_fp_tally_wire(rapid_fp* fp, const rapid_wire* w, int32_t* decided, uint64_t* decided_hash, uint64_t* decided_hash2,
+                            int32_t* decided_len, int32_t* decided_count, int32_t* votes_received);
+
 /* ------------------------------------------------------------------------------------------------
  * Alert generation  (SURVEY.md §8 f4): PingPongFailureDetector.java:38-121 — one detector per entry of
  * getSubjectsOf(node), i.e. K per member (MembershipService.java:697-707) — and the AlertMessage a notifier

@@ -109,6 +109,20 @@ public final class Native {
     public static native int wireApplyToDetector(long wire, long cd, long cfgId, long nCells);
     /** same, enqueue only (rapid_cd_apply_batch_dev_async): the status comes back from cdSync / fpTallyCd */
     public static native int wireApplyToDetectorAsync(long wire, long cd, long cfgId, long nCells);
+    /** consensus messages of one kind (5 FastRoundPhase2b, 6 Phase1a, 7 Phase1b, 8 Phase2a, 9 Phase2b; each message's bytes
+     *  are bytes[off[i] .. off[i+1]), the RapidRequest when asRequest) decoded on the device; out2 = {unknown senders,
+     *  unknown list entries} */
+    public static native int wireDecodeConsensus(long wire, int kind, ByteBuffer bytes, long[] off, boolean asRequest, long[] out2);
+    /** per message of the last consensus decode (arrays of n, each may be null) */
+    public static native int wireReadConsensus(long wire, int[] sender, long[] cfg, int[] rndRound, int[] rndNode, int[] vrndRound,
+                                               int[] vrndNode, long[] hash, long[] hash2, int[] len);
+    /** the list of message `index` as ids in wire order (-1 = not in the view); returns its length or <0; fills min(len, outIds.length) */
+    public static native int wireConsensusValue(long wire, long index, int[] outIds);
+    /** handlePhase1bMessage / handlePhase2bMessage / handleFastRoundProposal over the last decode, without leaving the device;
+     *  outputs as pxPhase1b (out6), pxPhase2b (out5), fpTally (out6) */
+    public static native int pxPhase1bWire(long px, long wire, long[] out6);
+    public static native int pxPhase2bWire(long px, long wire, long[] out5);
+    public static native int fpTallyWire(long fp, long wire, long[] out6);
 
     // ---- alert generation: the K PingPongFailureDetectors of every virtual node ----
     public static native long fdetCreate(long view, int failureThreshold, int bootstrapThreshold);

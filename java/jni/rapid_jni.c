@@ -517,6 +517,79 @@ JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireApplyToDetectorAsync(JN
 }
 JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_cdSync(JNIEnv* env, jclass c, jlong cd) { return rapid_cd_sync(H(rapid_cd, cd)); }
 
+/* consensus messages of one kind, as the host split a drained inbox by RapidRequest content case */
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireDecodeConsensus(JNIEnv* env, jclass c, jlong w, jint kind, jobject bytes, jlongArray off,
+                                                                         jboolean asRequest, jlongArray out2) {
+    const jsize n = (*env)->GetArrayLength(env, off) - 1;
+    jlong* o = (*env)->GetLongArrayElements(env, off, NULL);
+    int64_t us = 0, ue = 0;
+    const int32_t rc = rapid_wire_decode_consensus(H(rapid_wire, w), kind, (const uint8_t*)BUF(env, bytes), (const int64_t*)o, n < 0 ? 0 : n,
+                                                   asRequest ? RAPID_WIRE_REQUEST : 0, &us, &ue);
+    (*env)->ReleaseLongArrayElements(env, off, o, JNI_ABORT);
+    const jlong v[2] = {(jlong)us, (jlong)ue};
+    (*env)->SetLongArrayRegion(env, out2, 0, 2, v);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireReadConsensus(JNIEnv* env, jclass c, jlong w, jintArray sender, jlongArray cfg,
+                                                                       jintArray rndRound, jintArray rndNode, jintArray vrndRound,
+                                                                       jintArray vrndNode, jlongArray hash, jlongArray hash2, jintArray len) {
+    jint* s = sender ? (*env)->GetIntArrayElements(env, sender, NULL) : NULL;
+    jlong* cf = cfg ? (*env)->GetLongArrayElements(env, cfg, NULL) : NULL;
+    jint* a0 = rndRound ? (*env)->GetIntArrayElements(env, rndRound, NULL) : NULL;
+    jint* a1 = rndNode ? (*env)->GetIntArrayElements(env, rndNode, NULL) : NULL;
+    jint* b0 = vrndRound ? (*env)->GetIntArrayElements(env, vrndRound, NULL) : NULL;
+    jint* b1 = vrndNode ? (*env)->GetIntArrayElements(env, vrndNode, NULL) : NULL;
+    jlong* h1 = hash ? (*env)->GetLongArrayElements(env, hash, NULL) : NULL;
+    jlong* h2 = hash2 ? (*env)->GetLongArrayElements(env, hash2, NULL) : NULL;
+    jint* ln = len ? (*env)->GetIntArrayElements(env, len, NULL) : NULL;
+    const int32_t rc = rapid_wire_read_consensus(H(rapid_wire, w), (int32_t*)s, (int64_t*)cf, (int32_t*)a0, (int32_t*)a1, (int32_t*)b0,
+                                                 (int32_t*)b1, (uint64_t*)h1, (uint64_t*)h2, (int32_t*)ln);
+    if (s) (*env)->ReleaseIntArrayElements(env, sender, s, 0);
+    if (cf) (*env)->ReleaseLongArrayElements(env, cfg, cf, 0);
+    if (a0) (*env)->ReleaseIntArrayElements(env, rndRound, a0, 0);
+    if (a1) (*env)->ReleaseIntArrayElements(env, rndNode, a1, 0);
+    if (b0) (*env)->ReleaseIntArrayElements(env, vrndRound, b0, 0);
+    if (b1) (*env)->ReleaseIntArrayElements(env, vrndNode, b1, 0);
+    if (h1) (*env)->ReleaseLongArrayElements(env, hash, h1, 0);
+    if (h2) (*env)->ReleaseLongArrayElements(env, hash2, h2, 0);
+    if (ln) (*env)->ReleaseIntArrayElements(env, len, ln, 0);
+    return rc;
+}
+/* the cval / decision list of a trigger_index / decided_index, without a protobuf runtime */
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireConsensusValue(JNIEnv* env, jclass c, jlong w, jlong index, jintArray outIds) {
+    const jsize cap = outIds ? (*env)->GetArrayLength(env, outIds) : 0;
+    jint* o = outIds ? (*env)->GetIntArrayElements(env, outIds, NULL) : NULL;
+    int32_t len = 0;
+    const int32_t rc = rapid_wire_consensus_value(H(rapid_wire, w), index, (int32_t*)o, cap, &len);
+    if (o) (*env)->ReleaseIntArrayElements(env, outIds, o, 0);
+    return rc == RAPID_OK ? len : rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_pxPhase1bWire(JNIEnv* env, jclass c, jlong px, jlong w, jlongArray out6) {
+    int32_t proposed = 0, clen = 0;
+    int64_t trigger = -1, total = 0;
+    uint64_t ca = 0, cb = 0;
+    const int32_t rc = rapid_px_phase1b_wire(H(rapid_px, px), H(rapid_wire, w), &proposed, &trigger, &ca, &cb, &clen, &total);
+    const jlong v[6] = {proposed, (jlong)trigger, (jlong)ca, (jlong)cb, clen, (jlong)total};
+    (*env)->SetLongArrayRegion(env, out6, 0, 6, v);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_pxPhase2bWire(JNIEnv* env, jclass c, jlong px, jlong w, jlongArray out5) {
+    int32_t decided = 0, dlen = 0;
+    int64_t at = -1;
+    uint64_t da = 0, db = 0;
+    const int32_t rc = rapid_px_phase2b_wire(H(rapid_px, px), H(rapid_wire, w), &decided, &at, &da, &db, &dlen);
+    const jlong v[5] = {decided, (jlong)at, (jlong)da, (jlong)db, dlen};
+    (*env)->SetLongArrayRegion(env, out5, 0, 5, v);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_fpTallyWire(JNIEnv* env, jclass c, jlong fp, jlong w, jlongArray out6) {
+    int32_t decided = 0, dlen = 0, dcount = 0, recv = 0;
+    uint64_t a = 0, b = 0;
+    const int32_t rc = rapid_fp_tally_wire(H(rapid_fp, fp), H(rapid_wire, w), &decided, &a, &b, &dlen, &dcount, &recv);
+    put_result(env, out6, decided, a, b, dlen, dcount, recv);
+    return rc;
+}
+
 /* ---------------------------------------------------------------- alert generation (PingPongFailureDetector.java) */
 JNIEXPORT jlong JNICALL Java_com_vrg_rapid_gpu_Native_fdetCreate(JNIEnv* env, jclass c, jlong view, jint thr, jint bootThr) {
     rapid_fdet* fd = NULL;

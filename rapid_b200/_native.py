@@ -17,6 +17,7 @@ EINVAL, ENOT_IN_RING, EALREADY_IN_RING, EUUID_SEEN, EHASH_COLLISION, ECUDA, ENCC
 CD_SERVICE, CD_RAW, CD_SWEEP, CD_BUCKETED, CD_LOG = 0, 1, 2, 4, 8
 DELIVERY_BLOCKED, DELIVERY_BITMAP, DELIVERY_PERMUTED = 1, 2, 4
 WIRE_REQUEST = 1
+WIRE_FAST_ROUND_PHASE2B, WIRE_PHASE1A, WIRE_PHASE1B, WIRE_PHASE2A, WIRE_PHASE2B = 5, 6, 7, 8, 9   # RapidRequest cases
 EDGE_UP, EDGE_DOWN = 0, 1
 MAX_K = 14
 
@@ -126,6 +127,12 @@ SIGNATURES = {
     "rapid_wire_read_messages": [_vp, _p, _p, _p, _p, _p, _p, _p, _p],
     "rapid_wire_decode_votes": [_vp, _p, _p, _i64, _u32, _p, _p, _p, _p, _p],
     "rapid_wire_last_device_ms": [_vp, _p],
+    "rapid_wire_decode_consensus": [_vp, _i32, _p, _p, _i64, _u32, _p, _p],
+    "rapid_wire_read_consensus": [_vp, _p, _p, _p, _p, _p, _p, _p, _p, _p],
+    "rapid_wire_consensus_value": [_vp, _i64, _p, _i32, _p],
+    "rapid_px_phase1b_wire": [_vp, _vp, _p, _p, _p, _p, _p, _p],
+    "rapid_px_phase2b_wire": [_vp, _vp, _p, _p, _p, _p, _p],
+    "rapid_fp_tally_wire": [_vp, _vp, _p, _p, _p, _p, _p, _p],
     "rapid_fdet_create": [_pp, _vp, _i32, _i32],
     "rapid_fdet_destroy": [_vp],
     "rapid_fdet_reset": [_vp],

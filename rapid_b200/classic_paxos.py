@@ -117,6 +117,13 @@ class Paxos:
         N.check(N.lib().rapid_px_phase1b_from_acceptors(self._h, acceptors._h, int(perm_seed), *[C.byref(x) for x in o]))
         return self._p1_result(o)
 
+    def handlePhase1bFromWire(self, decoder):
+        """:159-191 over the Phase1bMessages of decoder's last decode (WireDecoder.decodeConsensusMessages), on the device;
+        trigger_index is a message index of that decode (decoder.consensusValue(trigger_index) is cval as ids)"""
+        o = self._p1_outs()
+        N.check(N.lib().rapid_px_phase1b_wire(self._h, decoder._h, *[C.byref(x) for x in o]))
+        return self._p1_result(o)
+
     @staticmethod
     def _p2_outs():
         return C.c_int32(0), C.c_int64(-1), C.c_uint64(0), C.c_uint64(0), C.c_int32(0)
@@ -142,6 +149,13 @@ class Paxos:
     def handlePhase2bFromAcceptors(self, acceptors, perm_seed=0):
         o = self._p2_outs()
         N.check(N.lib().rapid_px_phase2b_from_acceptors(self._h, acceptors._h, int(perm_seed), *[C.byref(x) for x in o]))
+        return self._p2_result(o)
+
+    def handlePhase2bFromWire(self, decoder):
+        """:223-236 over the Phase2bMessages of decoder's last decode, on the device.  Raises RapidError(EINVAL), nothing
+        changed, if a message of the current configuration comes from an endpoint outside the dictionary"""
+        o = self._p2_outs()
+        N.check(N.lib().rapid_px_phase2b_wire(self._h, decoder._h, *[C.byref(x) for x in o]))
         return self._p2_result(o)
 
     @staticmethod

@@ -18,6 +18,7 @@
 #include "nccl_api.cuh"
 #include "radix.cuh"
 #include "scan.cuh"
+#include "wire_internal.cuh"
 
 namespace rapid {
 
@@ -35,6 +36,7 @@ struct PxScal {
     int32_t decide_idx, overflow, inserted;      // phase2b
     uint64_t h1, h2;                             // value of `chosen` / of the deciding message
     int32_t len, src;                            // src: batch index of the trigger message
+    int32_t unknown_sender;                      // phase2b from the wire: first current-configuration message of an unknown sender
 };
 
 // One open-addressing entry = one 32-byte sector: a probe, its key compare and its value update touch a single line.
@@ -270,6 +272,13 @@ __global__ void k_px2b_rounds(int64_t n, const int64_t* __restrict__ rnd, int64_
     }
     key[i] = k;
 }
+// decoded Phase2b messages: the first one of the current configuration whose sender is outside the dictionary (-1)
+__global__ void k_px2b_unknown(int64_t n, const int64_t* __restrict__ mcfg, int64_t cfg, const int32_t* __restrict__ sender,
+                               PxScal* __restrict__ sc) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && mcfg[i] == cfg && sender[i] < 0) atomicMin(&sc->unknown_sender, (int32_t)i);
+}
+__global__ void k_px2b_unknown_begin(PxScal* sc) { sc->unknown_sender = INT_MAX; }
 // the pairs of this call are "seen" from now on
 __global__ void k_px2b_seal(int64_t n, const int32_t* __restrict__ slot, PxEntry* __restrict__ ent) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -979,6 +988,63 @@ int32_t rapid_px_phase2b(rapid_px* px, int64_t n, const int64_t* msg_cfg, const 
     }
     const int32_t rc = px_phase2b_device(px, n, dcfg, px->s_rnd.p, 0, px->s_sender.p, px->s_h1.p, hash2 ? px->s_h2.p : nullptr, px->s_len.p,
                                          0, 0, 0, decided, decided_index, decided_hash, decided_hash2, decided_len);
+    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
+    return rc;
+}
+
+// the decoded messages of a wire handle (wire_internal.cuh): ranks packed on the device, nothing uploaded
+static int32_t px_wire_msgs(rapid_px* px, const rapid_wire* w, int32_t kind, WireMsgs* m) {
+    if (!px) { set_error("NULL handle"); return RAPID_EINVAL; }
+    RAPID_CHECK(wire_consensus_dev(w, kind, m));
+    if (m->device != px->device) { set_error("px and wire live on different devices"); return RAPID_EINVAL; }
+    return RAPID_OK;
+}
+
+int32_t rapid_px_phase1b_wire(rapid_px* px, const rapid_wire* w, int32_t* proposed, int64_t* trigger_index, uint64_t* cval_hash,
+                              uint64_t* cval_hash2, int32_t* cval_len, int64_t* n_messages) {
+    WireMsgs m;
+    RAPID_CHECK(px_wire_msgs(px, w, RAPID_WIRE_PHASE1B, &m));
+    DeviceGuard g(px->device);
+    cudaStream_t s = px->stream;
+    const int64_t n = m.n;
+    RAPID_CUDA(cudaEventRecord(px->ev0, s));
+    if (n > 0) {
+        RAPID_CHECK(px->s_rnd.reserve((size_t)n)); RAPID_CHECK(px->s_vr.reserve((size_t)n));
+        k_px_pack<<<grid_for(n), TB, 0, s>>>(n, m.rnd_round, m.rnd_node, px->s_rnd.p);
+        k_px_pack<<<grid_for(n), TB, 0, s>>>(n, m.vrnd_round, m.vrnd_node, px->s_vr.p);
+        RAPID_KERNEL_CHECK();
+    }
+    const int32_t rc = px_phase1b_device(px, n, m.cfg, px->s_rnd.p, 0, px->s_vr.p, m.h1, m.h2, m.len, proposed, trigger_index, cval_hash,
+                                         cval_hash2, cval_len, n_messages);
+    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
+    return rc;
+}
+
+int32_t rapid_px_phase2b_wire(rapid_px* px, const rapid_wire* w, int32_t* decided, int64_t* decided_index, uint64_t* decided_hash,
+                              uint64_t* decided_hash2, int32_t* decided_len) {
+    WireMsgs m;
+    RAPID_CHECK(px_wire_msgs(px, w, RAPID_WIRE_PHASE2B, &m));
+    DeviceGuard g(px->device);
+    cudaStream_t s = px->stream;
+    const int64_t n = m.n;
+    RAPID_CUDA(cudaEventRecord(px->ev0, s));
+    if (n > 0) {
+        // a message of another configuration is dropped whatever its sender (:224); one of this configuration from an endpoint
+        // outside the dictionary refuses the call before anything changes
+        k_px2b_unknown_begin<<<1, 1, 0, s>>>(px->sc.p);
+        k_px2b_unknown<<<grid_for(n), TB, 0, s>>>(n, m.cfg, px->cfg, m.sender, px->sc.p);
+        RAPID_KERNEL_CHECK();
+        RAPID_CHECK(px_read_scal(px));
+        if (px->h_sc.p->unknown_sender != INT_MAX) {
+            set_error("Phase2bMessage %d of the current configuration comes from an endpoint outside the dictionary", px->h_sc.p->unknown_sender);
+            return RAPID_EINVAL;
+        }
+        RAPID_CHECK(px->s_rnd.reserve((size_t)n));
+        k_px_pack<<<grid_for(n), TB, 0, s>>>(n, m.rnd_round, m.rnd_node, px->s_rnd.p);
+        RAPID_KERNEL_CHECK();
+    }
+    const int32_t rc = px_phase2b_device(px, n, m.cfg, px->s_rnd.p, 0, m.sender, m.h1, m.h2, m.len, 0, 0, 0, decided, decided_index,
+                                         decided_hash, decided_hash2, decided_len);
     if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
     return rc;
 }

@@ -18,6 +18,7 @@
 
 #include "cd_internal.cuh"
 #include "nccl_api.cuh"
+#include "wire_internal.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -236,8 +237,11 @@ __global__ void __launch_bounds__(1024) k_fp_decide_sum(const unsigned long long
 //   "has not voted in an earlier call".
 // ARRAY = true: vote i is (sender[i], vcfg[i], h1v[i], h2v[i], lenv[i]) in arrival order, as the host handed them over.  A
 //   sender may vote several times; only its first vote of this configuration counts (:126, :134).
+// WIRE = true (with ARRAY): the votes are decoded messages (rapid_fp_tally_wire), whose sender is -1 when the dictionary does
+//   not hold it.  A vote of another configuration is dropped first (:126), so only a vote of THIS configuration from a sender
+//   outside [0, sender_cap) refuses the call.
 // Phases (grid barriers in between, every block owns a CONTIGUOUS range of votes so that arrival order is block order):
-//   V  (ARRAY) a sender outside [0, sender_cap) refuses the whole call before anything is marked
+//   V  (ARRAY) a sender outside [0, sender_cap) refuses the whole call before anything is marked (WIRE: of this configuration)
 //   F  (ARRAY) the first vote of every sender in this call: atomicMin of its index into seen[] (-1, voted earlier, stays)
 //   A  find-or-insert the proposal of every first vote (warp- and block-aggregated counts -> t_call); the add that takes a
 //      proposal over the quorum nominates it as a candidate
@@ -339,7 +343,7 @@ __device__ __forceinline__ int32_t tally_block_scan(int32_t v, int32_t* warp_sum
     return (wid ? warp_sums[wid - 1] : 0) + inc - v;
 }
 
-template <bool ARRAY>
+template <bool ARRAY, bool WIRE = false>
 __global__ void __launch_bounds__(TALLY_THREADS) k_fp_tally(const TallyArgs a) {
     cg::grid_group grid = cg::this_grid();
     __shared__ int32_t s_key[16], s_val[16], s_recv, s_last;
@@ -375,7 +379,7 @@ __global__ void __launch_bounds__(TALLY_THREADS) k_fp_tally(const TallyArgs a) {
         // ---- V: a sender outside the table refuses the call; nothing is marked yet, so nothing has to be undone ---------------
         for (int64_t i = c0 + t; i < c1; i += TALLY_THREADS) {
             const int32_t s = a.sender[i];
-            if (s < 0 || s >= a.sender_cap) atomicMax(&a.st->bad_sender, (int32_t)i);
+            if ((s < 0 || s >= a.sender_cap) && (!WIRE || a.vcfg[i] == a.cfg)) atomicMax(&a.st->bad_sender, (int32_t)i);
         }
         grid.sync();
         skip = *(volatile int32_t*)&a.st->bad_sender >= 0;
@@ -537,15 +541,16 @@ static int32_t fp_reset_call_state(FP* fp) {        // per-call fields only; no 
     return RAPID_OK;
 }
 
-// the grid of k_fp_tally (co-resident blocks of the smaller instantiation, so that either runs on it) and its scratch for R votes
+// the grid of k_fp_tally (co-resident blocks of the smallest instantiation, so that any runs on it) and its scratch for R votes
 static int32_t tally_reserve(FP* fp, int64_t R) {
     if (fp->tally_grid == 0) {
-        int dev = 0, sms = TARGET_SMS, per_cd = 4, per_array = 4;
+        int dev = 0, sms = TARGET_SMS, per_cd = 4, per_array = 4, per_wire = 4;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_cd, k_fp_tally<false>, TALLY_THREADS, 0);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_array, k_fp_tally<true>, TALLY_THREADS, 0);
-        fp->tally_grid = std::max(1, sms * std::max(std::min(per_cd, per_array), 1));
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_wire, k_fp_tally<true, true>, TALLY_THREADS, 0);
+        fp->tally_grid = std::max(1, sms * std::max(std::min(std::min(per_cd, per_array), per_wire), 1));
         RAPID_CHECK(fp->blk_cnt.reserve((size_t)8 * fp->tally_grid));
     }
     return fp->ent.reserve((size_t)std::max<int64_t>(R, 1));
@@ -553,7 +558,7 @@ static int32_t tally_reserve(FP* fp, int64_t R) {
 
 // launch k_fp_tally over ta.R votes (ta holds their source; tally_reserve(fp, ta.R) came first) on the tally's stream; the
 // result record goes to d_res_raw
-static int32_t tally_launch(FP* fp, TallyArgs& ta, bool array) {
+static int32_t tally_launch(FP* fp, TallyArgs& ta, bool array, bool wire = false) {
     ta.sender_cap = fp->sender_cap; ta.seen = fp->seen.p; ta.T = fp->T;
     ta.t_state = fp->t_state.p; ta.t_h1 = fp->t_h1.p; ta.t_h2 = fp->t_h2.p; ta.t_len = fp->t_len.p;
     ta.t_count = fp->t_count.p; ta.t_call = fp->t_call.p; ta.ent = fp->ent.p;
@@ -562,7 +567,8 @@ static int32_t tally_launch(FP* fp, TallyArgs& ta, bool array) {
     ta.out = (FPResult*)fp->d_res_raw.p;
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(fp->tally_grid, ceil_div<int64_t>(ta.R, TALLY_THREADS)));
     void* args[] = {(void*)&ta};
-    RAPID_CUDA(cudaLaunchCooperativeKernel(array ? (void*)k_fp_tally<true> : (void*)k_fp_tally<false>, dim3((unsigned)grid),
+    void* k = wire ? (void*)k_fp_tally<true, true> : array ? (void*)k_fp_tally<true> : (void*)k_fp_tally<false>;
+    RAPID_CUDA(cudaLaunchCooperativeKernel(k, dim3((unsigned)grid),
                                            dim3(TALLY_THREADS), args, 0, fp->stream));
     fp->last_launches = 1;
     return RAPID_OK;
@@ -570,9 +576,14 @@ static int32_t tally_launch(FP* fp, TallyArgs& ta, bool array) {
 
 // the host copy of k_fp_tally's result record -> the caller's outputs, or the refusal it reports
 static int32_t take_result(FP* fp, int32_t* decided, uint64_t* dh1, uint64_t* dh2, int32_t* dlen, int32_t* dcount, int32_t* received,
-                           int32_t* decided_in_call) {
+                           int32_t* decided_in_call, const int32_t* wire_sender = nullptr) {
     const FPResult r = *(const FPResult*)fp->h_res_raw.p;
-    if (r.bad_sender >= 0) { set_error("vote %d: sender id outside [0, sender_capacity)", r.bad_sender); return RAPID_EINVAL; }
+    if (r.bad_sender >= 0) {
+        if (wire_sender && *wire_sender < 0)
+            set_error("vote %d of the current configuration comes from an endpoint outside the dictionary", r.bad_sender);
+        else set_error("vote %d: sender id outside [0, sender_capacity)", r.bad_sender);
+        return RAPID_EINVAL;
+    }
     if (r.decided < 0) { set_error("more than 8 proposals reached the quorum in one call"); return RAPID_EUNSUPPORTED; }
     fp->decided_host = r.decided != 0;
     if (decided) *decided = r.decided;
@@ -698,6 +709,30 @@ int32_t rapid_fp_tally(rapid_fp* fp, int64_t n_votes, const int32_t* sender, con
     RAPID_CUDA(cudaStreamSynchronize(s));
     cudaEventElapsedTime(&fp->last_ms, fp->ev0, fp->ev1);
     return take_result(fp, decided, decided_hash, decided_hash2, decided_len, decided_count, votes_received, nullptr);
+}
+
+int32_t rapid_fp_tally_wire(rapid_fp* fp, const rapid_wire* w, int32_t* decided, uint64_t* decided_hash, uint64_t* decided_hash2,
+                            int32_t* decided_len, int32_t* decided_count, int32_t* votes_received) {
+    if (!fp) { set_error("NULL handle"); return RAPID_EINVAL; }
+    WireMsgs m;
+    RAPID_CHECK(wire_consensus_dev(w, RAPID_WIRE_FAST_ROUND_PHASE2B, &m));
+    if (m.device != fp->device) { set_error("fp and wire live on different devices"); return RAPID_EINVAL; }
+    DeviceGuard g(fp->device);
+    cudaStream_t s = fp->stream;
+    const int64_t n = fp->decided_host ? 0 : m.n;          // :138 — everything after the decision is ignored
+    RAPID_CHECK(tally_reserve(fp, n));
+    RAPID_CUDA(cudaEventRecord(fp->ev0, s));
+    TallyArgs ta = {};
+    ta.R = n; ta.sender = m.sender; ta.vcfg = m.cfg; ta.cfg = fp->cfg; ta.h1v = m.h1; ta.h2v = m.h2; ta.lenv = m.len;
+    RAPID_CHECK(tally_launch(fp, ta, true, true));
+    RAPID_CUDA(cudaEventRecord(fp->ev1, s));
+    RAPID_CUDA(cudaMemcpyAsync(fp->h_res_raw.p, fp->d_res_raw.p, sizeof(FPResult), cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    cudaEventElapsedTime(&fp->last_ms, fp->ev0, fp->ev1);
+    int32_t bad = 0;                                        // the refused vote's sender: -1 (unknown endpoint) or past sender_capacity
+    const FPResult r = *(const FPResult*)fp->h_res_raw.p;
+    if (r.bad_sender >= 0) RAPID_CUDA(cudaMemcpy(&bad, m.sender + r.bad_sender, 4, cudaMemcpyDeviceToHost));
+    return take_result(fp, decided, decided_hash, decided_hash2, decided_len, decided_count, votes_received, nullptr, &bad);
 }
 
 // enqueue the tally of the detector's votes (and, sharded, the all-reduce + decision kernel) on the tally's stream

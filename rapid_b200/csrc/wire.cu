@@ -5,6 +5,8 @@
 // unknown fields — is parsed by one thread per AlertMessage.  Endpoints are resolved against an open-addressing
 // table over the view's endpoints keyed by the ring-0 key the view already holds (MembershipView.java:579-582),
 // with a byte compare on a hit.  Two passes over the messages: parse + count ring numbers, prefix sum, emit cells.
+// Consensus messages (FastRoundPhase2b, Phase1a/1b/2a/2b) go through one load-balanced decoder: a thread per message for the
+// top level, a scan over the list lengths, a thread per list ENTRY for the lookups, a warp per message for the fingerprint.
 #include <limits.h>
 
 #include <algorithm>
@@ -16,6 +18,7 @@
 
 #include "common.cuh"
 #include "scan.cuh"
+#include "wire_internal.cuh"
 
 namespace rapid {
 
@@ -92,11 +95,10 @@ __global__ void k_wire_table_build(int64_t tot, const int64_t* __restrict__ key0
     }
 }
 
-__device__ int32_t ep_lookup(const uint8_t* __restrict__ buf, const EpRef e, uint32_t T, const int32_t* __restrict__ table,
-                             const int64_t* __restrict__ key0, const uint8_t* __restrict__ hb, const int32_t* __restrict__ hoff,
-                             const int32_t* __restrict__ hport) {
-    if (!e.present) return -1;
-    const int64_t k = ring_key(buf + e.off, e.len, e.port, 0);
+// id of the endpoint e whose ring-0 key is k, -1 if the dictionary does not hold it
+__device__ int32_t ep_lookup_key(const uint8_t* __restrict__ buf, const EpRef e, int64_t k, uint32_t T, const int32_t* __restrict__ table,
+                                 const int64_t* __restrict__ key0, const uint8_t* __restrict__ hb, const int32_t* __restrict__ hoff,
+                                 const int32_t* __restrict__ hport) {
     uint32_t pos = ep_slot(k) & (T - 1);
     for (uint32_t probes = 0; probes < T; ++probes) {
         const int32_t id = table[pos];
@@ -112,6 +114,12 @@ __device__ int32_t ep_lookup(const uint8_t* __restrict__ buf, const EpRef e, uin
     }
     return -1;
 }
+__device__ int32_t ep_lookup(const uint8_t* __restrict__ buf, const EpRef e, uint32_t T, const int32_t* __restrict__ table,
+                             const int64_t* __restrict__ key0, const uint8_t* __restrict__ hb, const int32_t* __restrict__ hoff,
+                             const int32_t* __restrict__ hport) {
+    if (!e.present) return -1;
+    return ep_lookup_key(buf, e, ring_key(buf + e.off, e.len, e.port, 0), T, table, key0, hb, hoff, hport);
+}
 
 struct Dict {
     uint32_t T;
@@ -125,7 +133,9 @@ struct Dict {
 struct WireScal {
     int32_t bad_msg;        // lowest index of a malformed message, INT_MAX if none
     int32_t n_need;         // UP alerts whose edgeDst is not in the dictionary
-    int32_t n_cells, n_dropped, sender_id, bad_vote;
+    int32_t n_cells, n_dropped, sender_id;
+    int32_t n_items;        // consensus decode: endpoints in all the lists
+    int32_t n_unknown_senders, n_unknown_endpoints;
 };
 
 // ------------------------------------------------------------------ alert kernels
@@ -232,7 +242,10 @@ __global__ void k_wire_emit(int64_t M, const uint8_t* __restrict__ buf, const in
         } else rd_skip(rd, wt);
     }
 }
-__global__ void k_wire_begin(WireScal* sc) { sc->bad_msg = INT_MAX; sc->n_need = 0; sc->n_cells = 0; sc->n_dropped = 0; sc->sender_id = -1; sc->bad_vote = INT_MAX; }
+__global__ void k_wire_begin(WireScal* sc) {
+    sc->bad_msg = INT_MAX; sc->n_need = 0; sc->n_cells = 0; sc->n_dropped = 0; sc->sender_id = -1;
+    sc->n_items = 0; sc->n_unknown_senders = 0; sc->n_unknown_endpoints = 0;
+}
 __global__ void k_wire_sender(const uint8_t* __restrict__ buf, EpRef e, Dict d, WireScal* __restrict__ sc) {
     sc->sender_id = ep_lookup(buf, e, d.T, d.table, d.key0, d.hb, d.hoff, d.hport);
 }
@@ -245,70 +258,194 @@ __global__ void k_wire_msg_fields(int64_t M, const MsgRec* __restrict__ rec, int
     has[m] = (uint8_t)r.has_nid; moff[m] = r.meta_off; mlen[m] = r.meta_len;
 }
 
-// ------------------------------------------------------------------ vote kernel: one thread per FastRoundPhase2bMessage
-__global__ void k_wire_votes(int64_t n, const uint8_t* __restrict__ buf, const int64_t* __restrict__ off, int unwrap, Dict d,
-                             int32_t* __restrict__ sender, int64_t* __restrict__ cfg, uint64_t* __restrict__ h1, uint64_t* __restrict__ h2,
-                             int32_t* __restrict__ len, WireScal* __restrict__ sc) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint8_t* p = buf + off[i];
-    int64_t l = off[i + 1] - off[i];
-    bool ok = l >= 0;
-    if (ok && unwrap) {                                      // RapidRequest.fastRoundPhase2bMessage = 5
-        Rd r{p, p + l, true};
-        const uint8_t* q = nullptr; int64_t ql = -1;
-        while (r.ok && r.p < r.end) {
-            const uint64_t tag = rd_varint(r);
-            if (!r.ok) break;
-            if ((tag >> 3) == 5 && (tag & 7) == 2) rd_len(r, &q, &ql);
-            else if ((tag >> 3) == 0) r.ok = false;
-            else {
-                if ((tag >> 3) <= 10) { q = nullptr; ql = -1; }                  // another case of the oneof replaces it
-                rd_skip(r, (uint32_t)(tag & 7));
+// ------------------------------------------------------------------ consensus messages (rapid.proto:124-169)
+// Kinds are the RapidRequest oneof cases (rapid.proto:21-35).  Every kind is {sender = 1, configurationId = 2} plus up to two
+// Ranks and one repeated Endpoint list; the layout says which field numbers carry them (0: none).
+struct ConsLayout {
+    uint32_t rank_a;        // rank (Phase1a) or rnd
+    uint32_t rank_b;        // vrnd (Phase1b)
+    uint32_t list;          // endpoints / vval
+};
+RAPID_HD ConsLayout cons_layout(int32_t kind) {
+    switch (kind) {
+        case RAPID_WIRE_FAST_ROUND_PHASE2B: return ConsLayout{0, 0, 3};
+        case RAPID_WIRE_PHASE1A: return ConsLayout{3, 0, 0};
+        case RAPID_WIRE_PHASE1B: return ConsLayout{3, 4, 5};
+        case RAPID_WIRE_PHASE2A: return ConsLayout{3, 0, 5};
+        default: return ConsLayout{3, 0, 4};                 // RAPID_WIRE_PHASE2B: its list is field 4
+    }
+}
+
+// parse (merge) one Rank occurrence {round = 1, nodeIndex = 2}: int32 fields are the low 32 bits of the varint
+RAPID_HD void parse_rank(const uint8_t* p, int64_t n, int32_t* round, int32_t* node, bool* ok) {
+    Rd r{p, p + n, true};
+    while (r.ok && r.p < r.end) {
+        const uint64_t tag = rd_varint(r);
+        if (!r.ok) break;
+        const uint32_t f = (uint32_t)(tag >> 3), wt = (uint32_t)(tag & 7);
+        if (f == 0) r.ok = false;
+        else if (f == 1 && wt == 0) *round = (int32_t)rd_varint(r);
+        else if (f == 2 && wt == 0) *node = (int32_t)rd_varint(r);
+        else rd_skip(r, wt);
+    }
+    if (!r.ok) *ok = false;
+}
+
+struct ConsTop {                        // the top-level fields of one message
+    EpRef sender;
+    int64_t cfg;
+    int32_t ra_round, ra_node, rb_round, rb_node;
+    int32_t cnt;                        // list endpoints
+    bool ok;
+};
+
+// Walk one occurrence of the message's content.  EMIT = false: parse everything but the list entries, count those.
+// EMIT = true (the message is known to be well-formed): write the byte range and message index of every list entry.
+template <bool EMIT>
+__device__ void cons_part(const uint8_t* buf, const uint8_t* p, int64_t l, const ConsLayout L, ConsTop& t, int32_t msg,
+                          int32_t* o_off, int32_t* o_len, int32_t* o_msg) {
+    Rd r{p, p + l, true};
+    while (r.ok && r.p < r.end) {
+        const uint64_t tag = rd_varint(r);
+        if (!r.ok) break;
+        const uint32_t f = (uint32_t)(tag >> 3), wt = (uint32_t)(tag & 7);
+        const uint8_t* q; int64_t ql;
+        if (f == 0) r.ok = false;
+        else if (f == L.list && wt == 2) {
+            if (rd_len(r, &q, &ql)) {
+                if (EMIT) { o_off[t.cnt] = (int32_t)(q - buf); o_len[t.cnt] = (int32_t)ql; o_msg[t.cnt] = msg; }
+                ++t.cnt;
             }
         }
-        if (!r.ok || ql < 0) ok = false; else { p = q; l = ql; }
+        else if (EMIT) rd_skip(r, wt);
+        else if (f == 1 && wt == 2) { if (rd_len(r, &q, &ql)) parse_endpoint(buf, q, ql, &t.sender, &t.ok); }
+        else if (f == 2 && wt == 0) t.cfg = (int64_t)rd_varint(r);
+        else if (f == L.rank_a && wt == 2) { if (rd_len(r, &q, &ql)) parse_rank(q, ql, &t.ra_round, &t.ra_node, &t.ok); }
+        else if (f == L.rank_b && wt == 2) { if (rd_len(r, &q, &ql)) parse_rank(q, ql, &t.rb_round, &t.rb_node, &t.ok); }
+        else rd_skip(r, wt);                                // unknown field, or a known one with another wire type
     }
-    EpRef s{0, 0, 0, 0};
-    int64_t c = 0;
-    uint64_t a = 0, b = 0;
-    int32_t cnt = 0;
-    bool unknown = false;
-    if (ok) {
-        Rd r{p, p + l, true};
-        while (r.ok && r.p < r.end) {
-            const uint64_t tag = rd_varint(r);
-            if (!r.ok) break;
-            const uint32_t f = (uint32_t)(tag >> 3), wt = (uint32_t)(tag & 7);
+    if (!r.ok) t.ok = false;
+}
+
+// Walk the message content of bytes [p, p + l): the whole range, or (unwrap) the RapidRequest's `kind` case.  A oneof case of
+// message type that occurs several times is merged (the occurrences are walked in order into the same ConsTop); another case
+// occurring later replaces it.  false: malformed RapidRequest, or its content is not (or no longer) the `kind` case.
+template <bool EMIT>
+__device__ bool cons_walk(const uint8_t* buf, const uint8_t* p, int64_t l, bool unwrap, int32_t kind, const ConsLayout L, ConsTop& t,
+                          int32_t msg, int32_t* o_off, int32_t* o_len, int32_t* o_msg) {
+    if (!unwrap) { cons_part<EMIT>(buf, p, l, L, t, msg, o_off, o_len, o_msg); return true; }
+    Rd r{p, p + l, true};
+    const uint8_t* from = p;
+    bool have = false;
+    while (r.ok && r.p < r.end) {
+        const uint64_t tag = rd_varint(r);
+        if (!r.ok) break;
+        const uint32_t f = (uint32_t)(tag >> 3), wt = (uint32_t)(tag & 7);
+        if (f == 0) { r.ok = false; break; }
+        if (wt == 2 && f <= 10) {                           // a case of RapidRequest.content (all are messages)
             const uint8_t* q; int64_t ql;
-            if (f == 1 && wt == 2) { if (rd_len(r, &q, &ql)) parse_endpoint(buf, q, ql, &s, &ok); }
-            else if (f == 2 && wt == 0) c = (int64_t)rd_varint(r);
-            else if (f == 3 && wt == 2) {
-                if (rd_len(r, &q, &ql)) {
-                    EpRef e{0, 0, 0, 0};
-                    parse_endpoint(buf, q, ql, &e, &ok);
-                    const int32_t id = ep_lookup(buf, e, d.T, d.table, d.key0, d.hb, d.hoff, d.hport);
-                    if (id >= 0) { a += fp_mix1(id); b += fp_mix2(id); }
-                    else {
-                        // an endpoint outside the dictionary (a vote of another configuration, say — FastPaxos.java:126-132 drops
-                        // those by their configurationId, not by their content): it still gets an identity — its ring-0 key — so that
-                        // identical lists keep identical fingerprints and the tally's own filters decide what the vote is worth
-                        const uint64_t kk = (uint64_t)ring_key(buf + e.off, e.len, e.port, 0);
-                        a += splitmix64(kk ^ 0x554E4B4E4F574E31ULL); b += splitmix64((kk * 0xD6E8FEB86659FD93ULL) ^ 0x554E4B4E4F574E32ULL);
-                        unknown = true;
-                    }
-                    ++cnt;
-                }
-            }
-            else if (f == 0) r.ok = false;
-            else rd_skip(r, wt);
-        }
-        if (!r.ok) ok = false;
+            if (!rd_len(r, &q, &ql)) break;
+            if ((int32_t)f == kind) have = true;
+            else { have = false; from = r.p; }
+        } else rd_skip(r, wt);
     }
-    if (!ok) { atomicMin(&sc->bad_msg, (int32_t)i); sender[i] = -1; cfg[i] = 0; h1[i] = 0; h2[i] = 0; len[i] = 0; return; }
-    if (unknown) atomicMin(&sc->bad_vote, (int32_t)i);       // reported as a count-free diagnostic only (first such vote)
-    sender[i] = ep_lookup(buf, s, d.T, d.table, d.key0, d.hb, d.hoff, d.hport);
-    cfg[i] = c; h1[i] = a; h2[i] = b; len[i] = cnt;
+    if (!r.ok || !have) return false;
+    Rd r2{from, p + l, true};
+    while (r2.p < r2.end) {
+        const uint64_t tag = rd_varint(r2);
+        const uint32_t f = (uint32_t)(tag >> 3), wt = (uint32_t)(tag & 7);
+        const uint8_t* q; int64_t ql;
+        if (wt == 2 && (int32_t)f == kind) { rd_len(r2, &q, &ql); cons_part<EMIT>(buf, q, ql, L, t, msg, o_off, o_len, o_msg); }
+        else rd_skip(r2, wt);
+    }
+    return true;
+}
+
+// The one routine that turns a list endpoint into its terms of the order-insensitive list fingerprint: the id's mixes, as
+// rapid_proposal_fingerprint sums them, or for an endpoint outside the dictionary (a delayed message of another configuration
+// naming a node that has since left, say) mixes of its ring-0 key k.  So a list keeps one fingerprint whichever kind carries it,
+// identical stranger lists keep identical fingerprints, and the tallies' configuration filters decide what the message is worth.
+__device__ __forceinline__ void ep_fp_terms(int32_t id, int64_t k, uint64_t* a, uint64_t* b) {
+    if (id >= 0) { *a = fp_mix1(id); *b = fp_mix2(id); return; }
+    const uint64_t kk = (uint64_t)k;
+    *a = splitmix64(kk ^ 0x554E4B4E4F574E31ULL);
+    *b = splitmix64((kk * 0xD6E8FEB86659FD93ULL) ^ 0x554E4B4E4F574E32ULL);
+}
+
+// step 1, one thread per message: unwrap, top-level walk, sender lookup, list length
+__global__ void k_cons_top(int64_t n, const uint8_t* __restrict__ buf, const int64_t* __restrict__ off, int unwrap, int32_t kind, Dict d,
+                           int32_t* __restrict__ sender, int64_t* __restrict__ cfg, int32_t* __restrict__ ra_round,
+                           int32_t* __restrict__ ra_node, int32_t* __restrict__ rb_round, int32_t* __restrict__ rb_node,
+                           int32_t* __restrict__ cnt, WireScal* __restrict__ sc) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    bool unknown = false;
+    if (i < n) {
+        ConsTop t;
+        memset(&t, 0, sizeof(t));
+        t.ok = true;
+        const int64_t l = off[i + 1] - off[i];
+        const bool ok = cons_walk<false>(buf, buf + off[i], l, unwrap != 0, kind, cons_layout(kind), t, 0, nullptr, nullptr, nullptr) && t.ok;
+        if (!ok) {
+            atomicMin(&sc->bad_msg, (int32_t)i);
+            memset(&t, 0, sizeof(t));
+        }
+        const int32_t s = ok ? ep_lookup(buf, t.sender, d.T, d.table, d.key0, d.hb, d.hoff, d.hport) : -1;
+        unknown = ok && s < 0;
+        sender[i] = s; cfg[i] = t.cfg;
+        ra_round[i] = t.ra_round; ra_node[i] = t.ra_node; rb_round[i] = t.rb_round; rb_node[i] = t.rb_node;
+        cnt[i] = t.cnt;
+    }
+    const unsigned u = __ballot_sync(0xffffffffu, unknown);
+    if ((threadIdx.x & 31) == 0 && u) atomicAdd(&sc->n_unknown_senders, __popc(u));
+}
+
+// step 3, one thread per message: the byte range of every list entry, at its message's offset of the flat array
+__global__ void k_cons_items(int64_t n, const uint8_t* __restrict__ buf, const int64_t* __restrict__ off, int unwrap, int32_t kind,
+                             const int32_t* __restrict__ cnt, const int32_t* __restrict__ pos, int32_t* __restrict__ i_off,
+                             int32_t* __restrict__ i_len, int32_t* __restrict__ i_msg) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || cnt[i] == 0) return;
+    ConsTop t;
+    memset(&t, 0, sizeof(t));
+    const int32_t b = pos[i];
+    cons_walk<true>(buf, buf + off[i], off[i + 1] - off[i], unwrap != 0, kind, cons_layout(kind), t, (int32_t)i, i_off + b, i_len + b,
+                    i_msg + b);
+}
+
+// step 4, one thread per list entry: parse, look up, fingerprint terms
+__global__ void k_cons_resolve(int64_t m, const uint8_t* __restrict__ buf, const int32_t* __restrict__ i_off,
+                               const int32_t* __restrict__ i_len, const int32_t* __restrict__ i_msg, Dict d, int32_t* __restrict__ ids,
+                               uint64_t* __restrict__ m1, uint64_t* __restrict__ m2, WireScal* __restrict__ sc) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    bool unknown = false;
+    if (j < m) {
+        EpRef e{0, 0, 0, 0};
+        bool ok = true;
+        parse_endpoint(buf, buf + i_off[j], i_len[j], &e, &ok);
+        if (!ok) atomicMin(&sc->bad_msg, i_msg[j]);
+        const int64_t k = ring_key(buf + e.off, e.len, e.port, 0);
+        const int32_t id = ep_lookup_key(buf, e, k, d.T, d.table, d.key0, d.hb, d.hoff, d.hport);
+        uint64_t a, b;
+        ep_fp_terms(id, k, &a, &b);
+        ids[j] = id; m1[j] = a; m2[j] = b;
+        unknown = id < 0;
+    }
+    const unsigned u = __ballot_sync(0xffffffffu, unknown);
+    if ((threadIdx.x & 31) == 0 && u) atomicAdd(&sc->n_unknown_endpoints, __popc(u));
+}
+
+// step 5, one warp per message: segmented sum of the terms (lane-strided, then shuffles)
+__global__ void k_cons_reduce(int64_t n, const int32_t* __restrict__ pos, const int32_t* __restrict__ cnt, const uint64_t* __restrict__ m1,
+                              const uint64_t* __restrict__ m2, uint64_t* __restrict__ h1, uint64_t* __restrict__ h2) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (i >= n) return;                                     // uniform across the warp
+    const int32_t b = pos[i], c = cnt[i];
+    uint64_t a = 0, e = 0;
+    for (int32_t q = lane; q < c; q += 32) { a += m1[b + q]; e += m2[b + q]; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); e += __shfl_xor_sync(0xffffffffu, e, o); }
+    if (lane == 0) { h1[i] = a; h2[i] = e; }
 }
 
 // ------------------------------------------------------------------ handle
@@ -333,11 +470,18 @@ struct Wire {
     DevBuf<int32_t> o_src, o_dst;
     DevBuf<uint8_t> o_ring, o_status;
     DevBuf<int64_t> o_cfg;
-    // votes / message-field staging
-    DevBuf<int64_t> v_off, v_cfg, t_i64a, t_i64b, t_i64c;
-    DevBuf<int32_t> v_sender, v_len, t_i32a, t_i32b, t_i32c;
-    DevBuf<uint64_t> v_h1, v_h2;
+    // message-field staging
+    DevBuf<int64_t> t_i64a, t_i64b, t_i64c;
+    DevBuf<int32_t> t_i32a, t_i32b, t_i32c;
     DevBuf<uint8_t> t_u8a, t_u8b;
+    // the last consensus decode: per message (c_*), then per list entry in message order (i_*)
+    int32_t cons_kind = 0;            // its kind; 0 if the last decode was not a consensus decode or was refused
+    int64_t cons_n = 0;
+    DevBuf<int64_t> c_off, c_cfg;
+    DevBuf<int32_t> c_sender, c_ra_round, c_ra_node, c_rb_round, c_rb_node, c_len, c_pos;
+    DevBuf<uint64_t> c_h1, c_h2;
+    DevBuf<int32_t> i_off, i_len, i_msg, i_id;
+    DevBuf<uint64_t> i_m1, i_m2;
 };
 
 static const int TB = 128;
@@ -381,11 +525,100 @@ static bool host_find_field(const uint8_t* p, int64_t len, uint32_t field, const
     return r.ok;
 }
 
+static const char* cons_name(int32_t kind) {
+    switch (kind) {
+        case RAPID_WIRE_FAST_ROUND_PHASE2B: return "FastRoundPhase2bMessage";
+        case RAPID_WIRE_PHASE1A: return "Phase1aMessage";
+        case RAPID_WIRE_PHASE1B: return "Phase1bMessage";
+        case RAPID_WIRE_PHASE2A: return "Phase2aMessage";
+        default: return "Phase2bMessage";
+    }
+}
+
+// n serialized consensus messages of one kind -> the per-message fields and the flat list entries on the device.  Load-balanced:
+// one thread per message walks the top level and counts list entries, a scan places them, one thread per message writes their
+// byte ranges, one thread per ENTRY resolves it, one warp per message sums the fingerprint terms.  Whatever happens, the handle
+// holds no consensus decode unless this returns RAPID_OK.
+static int32_t wire_decode_consensus(Wire* w, int32_t kind, const uint8_t* bytes, const int64_t* off, int64_t n, uint32_t flags,
+                                     int64_t* n_unknown_senders, int64_t* n_unknown_endpoints) {
+    w->cons_kind = 0; w->cons_n = 0;
+    if (n < 0 || (n && (!bytes || !off)) || n > 0x7ffffff0LL || kind < RAPID_WIRE_FAST_ROUND_PHASE2B || kind > RAPID_WIRE_PHASE2B) {
+        set_error("bad arguments"); return RAPID_EINVAL;
+    }
+    if (n_unknown_senders) *n_unknown_senders = 0;
+    if (n_unknown_endpoints) *n_unknown_endpoints = 0;
+    if (n == 0) { w->cons_kind = kind; return RAPID_OK; }
+    for (int64_t i = 0; i < n; ++i)
+        if (off[i + 1] < off[i]) { set_error("off must be non-decreasing"); return RAPID_EINVAL; }
+    // byte offsets inside the buffer are int32 (EpRef); every list entry takes at least 2 bytes, so their count fits int32 too
+    if (off[0] < 0 || off[n] > 0x7ffffff0LL) { set_error("bad arguments: off must lie in [0, 0x7ffffff0]"); return RAPID_EINVAL; }
+    const int64_t len = off[n] - off[0];
+    DeviceGuard g(w->device);
+    cudaStream_t s = w->stream;
+    RAPID_CUDA(cudaEventRecord(w->ev0, s));
+    Dict d;
+    RAPID_CHECK(wire_dict(w, &d));
+    RAPID_CHECK(w->buf.reserve((size_t)std::max<int64_t>(off[n], 1)));
+    // keep the caller's offsets valid: copy [0, off[n]) (the prefix before off[0] is never read)
+    if (len) RAPID_CUDA(cudaMemcpyAsync(w->buf.p + off[0], bytes + off[0], (size_t)len, cudaMemcpyHostToDevice, s));
+    const size_t m = (size_t)n;
+    RAPID_CHECK(w->c_off.reserve(m + 1)); RAPID_CHECK(w->c_cfg.reserve(m)); RAPID_CHECK(w->c_sender.reserve(m));
+    RAPID_CHECK(w->c_ra_round.reserve(m)); RAPID_CHECK(w->c_ra_node.reserve(m)); RAPID_CHECK(w->c_rb_round.reserve(m));
+    RAPID_CHECK(w->c_rb_node.reserve(m)); RAPID_CHECK(w->c_len.reserve(m)); RAPID_CHECK(w->c_pos.reserve(m));
+    RAPID_CHECK(w->c_h1.reserve(m)); RAPID_CHECK(w->c_h2.reserve(m));
+    RAPID_CUDA(cudaMemcpyAsync(w->c_off.p, off, (m + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    const int unwrap = (flags & RAPID_WIRE_REQUEST) ? 1 : 0;
+    k_wire_begin<<<1, 1, 0, s>>>(w->sc.p);
+    k_cons_top<<<grid_for(n), TB, 0, s>>>(n, w->buf.p, w->c_off.p, unwrap, kind, d, w->c_sender.p, w->c_cfg.p, w->c_ra_round.p,
+                                          w->c_ra_node.p, w->c_rb_round.p, w->c_rb_node.p, w->c_len.p, w->sc.p);
+    RAPID_KERNEL_CHECK();
+    RAPID_CHECK(exclusive_scan_i32(w->c_pos.p, n, w->scan_sums, &w->sc.p->n_items, s, nullptr, w->c_len.p));
+    RAPID_CHECK(wire_read_scal(w));
+    const WireScal& sc = *w->h_sc.p;
+    if (sc.bad_msg == INT_MAX) {
+        const int64_t items = sc.n_items;
+        if (items > 0) {
+            const size_t k = (size_t)items;
+            RAPID_CHECK(w->i_off.reserve(k)); RAPID_CHECK(w->i_len.reserve(k)); RAPID_CHECK(w->i_msg.reserve(k));
+            RAPID_CHECK(w->i_id.reserve(k)); RAPID_CHECK(w->i_m1.reserve(k)); RAPID_CHECK(w->i_m2.reserve(k));
+            k_cons_items<<<grid_for(n), TB, 0, s>>>(n, w->buf.p, w->c_off.p, unwrap, kind, w->c_len.p, w->c_pos.p, w->i_off.p, w->i_len.p,
+                                                    w->i_msg.p);
+            k_cons_resolve<<<grid_for(items), TB, 0, s>>>(items, w->buf.p, w->i_off.p, w->i_len.p, w->i_msg.p, d, w->i_id.p, w->i_m1.p,
+                                                          w->i_m2.p, w->sc.p);
+            RAPID_KERNEL_CHECK();
+        }
+        k_cons_reduce<<<(unsigned)ceil_div<int64_t>(n * 32, TB), TB, 0, s>>>(n, w->c_pos.p, w->c_len.p, w->i_m1.p, w->i_m2.p, w->c_h1.p,
+                                                                             w->c_h2.p);
+        RAPID_KERNEL_CHECK();
+        RAPID_CUDA(cudaEventRecord(w->ev1, s));
+        RAPID_CHECK(wire_read_scal(w));
+        cudaEventElapsedTime(&w->last_ms, w->ev0, w->ev1);
+    }
+    if (sc.bad_msg != INT_MAX) { set_error("malformed %s at index %d", cons_name(kind), sc.bad_msg); return RAPID_EINVAL; }
+    if (n_unknown_senders) *n_unknown_senders = sc.n_unknown_senders;
+    if (n_unknown_endpoints) *n_unknown_endpoints = sc.n_unknown_endpoints;
+    w->cons_kind = kind; w->cons_n = n;
+    return RAPID_OK;
+}
+
 }  // namespace rapid
 
 using namespace rapid;
 
 struct rapid_wire : rapid::Wire {};
+
+int32_t rapid::wire_consensus_dev(const rapid_wire* w, int32_t kind, WireMsgs* out) {
+    if (!w) { set_error("NULL wire handle"); return RAPID_EINVAL; }
+    if (w->cons_kind != kind) {
+        set_error("the last decode on the wire handle is not a successful %s decode", cons_name(kind));
+        return RAPID_EINVAL;
+    }
+    out->device = w->device; out->n = w->cons_n;
+    out->sender = w->c_sender.p; out->cfg = w->c_cfg.p;
+    out->rnd_round = w->c_ra_round.p; out->rnd_node = w->c_ra_node.p; out->vrnd_round = w->c_rb_round.p; out->vrnd_node = w->c_rb_node.p;
+    out->h1 = w->c_h1.p; out->h2 = w->c_h2.p; out->len = w->c_len.p;
+    return RAPID_OK;
+}
 
 extern "C" {
 
@@ -424,6 +657,7 @@ int32_t rapid_wire_destroy(rapid_wire* w) {
 
 int32_t rapid_wire_decode_alerts(rapid_wire* w, const uint8_t* bytes, int64_t len, uint32_t flags, int64_t* n_messages, int64_t* n_cells,
                                  int64_t* n_dropped, int64_t* n_new_joiners, int32_t* sender_id) {
+    if (w) w->cons_kind = 0;                                 // any decode replaces the last consensus decode
     if (!w || len < 0 || (len && !bytes) || len > 0x7ffffff0LL) { set_error("bad arguments"); return RAPID_EINVAL; }
     DeviceGuard g(w->device);
     cudaStream_t s = w->stream;
@@ -579,38 +813,65 @@ int32_t rapid_wire_read_messages(const rapid_wire* cw, int32_t* dst, uint8_t* st
 
 int32_t rapid_wire_decode_votes(rapid_wire* w, const uint8_t* bytes, const int64_t* off, int64_t n, uint32_t flags, int32_t* sender,
                                 int64_t* vote_cfg, uint64_t* proposal_hash, uint64_t* proposal_hash2, int32_t* proposal_len) {
-    if (!w || n < 0 || (n && (!bytes || !off)) || n > 0x7ffffff0LL) { set_error("bad arguments"); return RAPID_EINVAL; }
+    if (!w) { set_error("bad arguments"); return RAPID_EINVAL; }
+    RAPID_CHECK(wire_decode_consensus(w, RAPID_WIRE_FAST_ROUND_PHASE2B, bytes, off, n, flags, nullptr, nullptr));
+    // (a vote naming an endpoint outside the dictionary is NOT an error: see ep_fp_terms)
     if (n == 0) return RAPID_OK;
-    for (int64_t i = 0; i < n; ++i)
-        if (off[i + 1] < off[i]) { set_error("off must be non-decreasing"); return RAPID_EINVAL; }
-    const int64_t len = off[n] - off[0];
     DeviceGuard g(w->device);
     cudaStream_t s = w->stream;
-    RAPID_CUDA(cudaEventRecord(w->ev0, s));
-    Dict d;
-    RAPID_CHECK(wire_dict(w, &d));
-    RAPID_CHECK(w->buf.reserve((size_t)std::max<int64_t>(off[n], 1)));
-    // keep the caller's offsets valid: copy [0, off[n]) (the prefix before off[0] is never read)
-    if (len) RAPID_CUDA(cudaMemcpyAsync(w->buf.p + off[0], bytes + off[0], (size_t)len, cudaMemcpyHostToDevice, s));
-    RAPID_CHECK(w->v_off.reserve((size_t)n + 1)); RAPID_CHECK(w->v_sender.reserve((size_t)n)); RAPID_CHECK(w->v_cfg.reserve((size_t)n));
-    RAPID_CHECK(w->v_h1.reserve((size_t)n)); RAPID_CHECK(w->v_h2.reserve((size_t)n)); RAPID_CHECK(w->v_len.reserve((size_t)n));
-    RAPID_CUDA(cudaMemcpyAsync(w->v_off.p, off, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
-    k_wire_begin<<<1, 1, 0, s>>>(w->sc.p);
-    k_wire_votes<<<grid_for(n), TB, 0, s>>>(n, w->buf.p, w->v_off.p, (flags & RAPID_WIRE_REQUEST) ? 1 : 0, d, w->v_sender.p, w->v_cfg.p,
-                                            w->v_h1.p, w->v_h2.p, w->v_len.p, w->sc.p);
-    RAPID_KERNEL_CHECK();
-    RAPID_CUDA(cudaEventRecord(w->ev1, s));
-    RAPID_CHECK(wire_read_scal(w));
-    cudaEventElapsedTime(&w->last_ms, w->ev0, w->ev1);
-    if (w->h_sc.p->bad_msg != INT_MAX) { set_error("malformed FastRoundPhase2bMessage at index %d", w->h_sc.p->bad_msg); return RAPID_EINVAL; }
-    // (a vote naming an endpoint outside the dictionary is NOT an error: see k_wire_votes)
     const size_t m = (size_t)n;
-    if (sender) RAPID_CUDA(cudaMemcpyAsync(sender, w->v_sender.p, m * 4, cudaMemcpyDeviceToHost, s));
-    if (vote_cfg) RAPID_CUDA(cudaMemcpyAsync(vote_cfg, w->v_cfg.p, m * 8, cudaMemcpyDeviceToHost, s));
-    if (proposal_hash) RAPID_CUDA(cudaMemcpyAsync(proposal_hash, w->v_h1.p, m * 8, cudaMemcpyDeviceToHost, s));
-    if (proposal_hash2) RAPID_CUDA(cudaMemcpyAsync(proposal_hash2, w->v_h2.p, m * 8, cudaMemcpyDeviceToHost, s));
-    if (proposal_len) RAPID_CUDA(cudaMemcpyAsync(proposal_len, w->v_len.p, m * 4, cudaMemcpyDeviceToHost, s));
+    if (sender) RAPID_CUDA(cudaMemcpyAsync(sender, w->c_sender.p, m * 4, cudaMemcpyDeviceToHost, s));
+    if (vote_cfg) RAPID_CUDA(cudaMemcpyAsync(vote_cfg, w->c_cfg.p, m * 8, cudaMemcpyDeviceToHost, s));
+    if (proposal_hash) RAPID_CUDA(cudaMemcpyAsync(proposal_hash, w->c_h1.p, m * 8, cudaMemcpyDeviceToHost, s));
+    if (proposal_hash2) RAPID_CUDA(cudaMemcpyAsync(proposal_hash2, w->c_h2.p, m * 8, cudaMemcpyDeviceToHost, s));
+    if (proposal_len) RAPID_CUDA(cudaMemcpyAsync(proposal_len, w->c_len.p, m * 4, cudaMemcpyDeviceToHost, s));
     RAPID_CUDA(cudaStreamSynchronize(s));
+    return RAPID_OK;
+}
+
+int32_t rapid_wire_decode_consensus(rapid_wire* w, int32_t kind, const uint8_t* bytes, const int64_t* off, int64_t n, uint32_t flags,
+                                    int64_t* n_unknown_senders, int64_t* n_unknown_endpoints) {
+    if (!w) { set_error("NULL handle"); return RAPID_EINVAL; }
+    return wire_decode_consensus(w, kind, bytes, off, n, flags, n_unknown_senders, n_unknown_endpoints);
+}
+
+int32_t rapid_wire_read_consensus(const rapid_wire* w, int32_t* sender, int64_t* cfg, int32_t* rnd_round, int32_t* rnd_node,
+                                  int32_t* vrnd_round, int32_t* vrnd_node, uint64_t* h1, uint64_t* h2, int32_t* len) {
+    if (!w) { set_error("NULL handle"); return RAPID_EINVAL; }
+    if (!w->cons_kind) { set_error("no consensus decode on this handle"); return RAPID_EINVAL; }
+    const size_t m = (size_t)w->cons_n;
+    if (m == 0) return RAPID_OK;
+    DeviceGuard g(w->device);
+    cudaStream_t s = w->stream;
+    if (sender) RAPID_CUDA(cudaMemcpyAsync(sender, w->c_sender.p, m * 4, cudaMemcpyDeviceToHost, s));
+    if (cfg) RAPID_CUDA(cudaMemcpyAsync(cfg, w->c_cfg.p, m * 8, cudaMemcpyDeviceToHost, s));
+    if (rnd_round) RAPID_CUDA(cudaMemcpyAsync(rnd_round, w->c_ra_round.p, m * 4, cudaMemcpyDeviceToHost, s));
+    if (rnd_node) RAPID_CUDA(cudaMemcpyAsync(rnd_node, w->c_ra_node.p, m * 4, cudaMemcpyDeviceToHost, s));
+    if (vrnd_round) RAPID_CUDA(cudaMemcpyAsync(vrnd_round, w->c_rb_round.p, m * 4, cudaMemcpyDeviceToHost, s));
+    if (vrnd_node) RAPID_CUDA(cudaMemcpyAsync(vrnd_node, w->c_rb_node.p, m * 4, cudaMemcpyDeviceToHost, s));
+    if (h1) RAPID_CUDA(cudaMemcpyAsync(h1, w->c_h1.p, m * 8, cudaMemcpyDeviceToHost, s));
+    if (h2) RAPID_CUDA(cudaMemcpyAsync(h2, w->c_h2.p, m * 8, cudaMemcpyDeviceToHost, s));
+    if (len) RAPID_CUDA(cudaMemcpyAsync(len, w->c_len.p, m * 4, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    return RAPID_OK;
+}
+
+int32_t rapid_wire_consensus_value(const rapid_wire* w, int64_t index, int32_t* out_ids, int32_t cap, int32_t* out_len) {
+    if (!w) { set_error("NULL handle"); return RAPID_EINVAL; }
+    if (!w->cons_kind) { set_error("no consensus decode on this handle"); return RAPID_EINVAL; }
+    if (index < 0 || index >= w->cons_n || cap < 0 || (cap > 0 && !out_ids)) { set_error("bad arguments"); return RAPID_EINVAL; }
+    DeviceGuard g(w->device);
+    cudaStream_t s = w->stream;
+    int32_t at = 0, len = 0;
+    RAPID_CUDA(cudaMemcpyAsync(&at, w->c_pos.p + index, 4, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaMemcpyAsync(&len, w->c_len.p + index, 4, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    const int32_t k = std::min(cap, len);
+    if (k > 0) {
+        RAPID_CUDA(cudaMemcpyAsync(out_ids, w->i_id.p + at, (size_t)k * 4, cudaMemcpyDeviceToHost, s));
+        RAPID_CUDA(cudaStreamSynchronize(s));
+    }
+    if (out_len) *out_len = len;
     return RAPID_OK;
 }
 

@@ -83,6 +83,14 @@ class FastPaxos:
                                        C.byref(a), C.byref(b), C.byref(l), C.byref(c), C.byref(r)))
         return TallyResult(bool(d.value), a.value, b.value, l.value, c.value, r.value)
 
+    def handleFastRoundProposalsFromWire(self, decoder):
+        """handleFastRoundProposals over the FastRoundPhase2bMessages of decoder's last decode, on the device.  Votes of another
+        configuration are dropped first; one of this configuration from an endpoint outside the dictionary raises
+        RapidError(EINVAL) with nothing changed"""
+        d, a, b, l, c, r = self._outs()
+        N.check(N.lib().rapid_fp_tally_wire(self._h, decoder._h, C.byref(d), C.byref(a), C.byref(b), C.byref(l), C.byref(c), C.byref(r)))
+        return TallyResult(bool(d.value), a.value, b.value, l.value, c.value, r.value)
+
     def tallyCluster(self, cluster, comm=None):
         """Every receiver of `cluster` that announced in the last batch votes for its proposal."""
         d, a, b, l, c, r = self._outs()

@@ -1,5 +1,5 @@
 """Wire-format ingest (SURVEY.md §8 f3): serialized rapid.proto messages -> alert cells / votes, decoded on the GPU by
-librapid_b200.so (csrc/wire.cu).  This is the step the reference's gRPC server does before
+librapid_b200.so (csrc/wire.cu), consensus messages included.  This is the step the reference's gRPC server does before
 MembershipService.handleMessage(RapidRequest) (MembershipService.java:174): no Python protobuf runtime is involved."""
 import ctypes as C
 
@@ -27,6 +27,7 @@ class WireDecoder:
         self._h = C.c_void_p()
         N.check(N.lib().rapid_wire_create(C.byref(self._h), view._h))
         self._last = None
+        self._n_cons = 0                     # messages of the last consensus decode
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -47,6 +48,7 @@ class WireDecoder:
         """bytes of a BatchedAlertMessage (or of the RapidRequest carrying it) -> DecodedAlerts; the cells stay on the device"""
         buf = np.frombuffer(bytes(data), dtype=np.uint8) if len(data) else np.zeros(1, np.uint8)
         m, c, d, j, s = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int32(-1)
+        self._n_cons = 0
         N.check(N.lib().rapid_wire_decode_alerts(self._h, N.ptr(buf), len(data), N.WIRE_REQUEST if is_request else 0, C.byref(m),
                                                  C.byref(c), C.byref(d), C.byref(j), C.byref(s)))
         self._last = DecodedAlerts(m.value, c.value, d.value, j.value, s.value)
@@ -77,19 +79,56 @@ class WireDecoder:
                                                                                    "has_node_id", "meta_off", "meta_len")]))
         return out
 
-    def decodeFastRoundPhase2bMessages(self, messages, is_request=False):
-        """list of serialized FastRoundPhase2bMessages -> (sender, cfg, hash, hash2, len) arrays"""
+    @staticmethod
+    def _pack(messages):
         n = len(messages)
         off = np.zeros(n + 1, np.int64)
         if n:
             off[1:] = np.cumsum([len(m) for m in messages])
         joined = b"".join(bytes(m) for m in messages)
-        buf = np.frombuffer(joined, dtype=np.uint8) if joined else np.zeros(1, np.uint8)
+        return n, off, np.frombuffer(joined, dtype=np.uint8) if joined else np.zeros(1, np.uint8)
+
+    def decodeFastRoundPhase2bMessages(self, messages, is_request=False):
+        """list of serialized FastRoundPhase2bMessages -> (sender, cfg, hash, hash2, len) arrays"""
+        n, off, buf = self._pack(messages)
+        self._n_cons = 0
         s, c = np.zeros(n, np.int32), np.zeros(n, np.int64)
         h1, h2, ln = np.zeros(n, np.uint64), np.zeros(n, np.uint64), np.zeros(n, np.int32)
         N.check(N.lib().rapid_wire_decode_votes(self._h, N.ptr(buf), N.ptr(off), n, N.WIRE_REQUEST if is_request else 0, N.ptr(s),
                                                 N.ptr(c), N.ptr(h1), N.ptr(h2), N.ptr(ln)))
+        self._n_cons = n
         return s, c, h1, h2, ln
+
+    def decodeConsensusMessages(self, kind, messages, is_request=False):
+        """serialized consensus messages of one kind (N.WIRE_FAST_ROUND_PHASE2B, N.WIRE_PHASE1A, N.WIRE_PHASE1B,
+        N.WIRE_PHASE2A, N.WIRE_PHASE2B) decoded on the device, where Paxos.handlePhase1bFromWire / handlePhase2bFromWire and
+        FastPaxos.handleFastRoundProposalsFromWire take them.  -> (messages whose sender is unknown, unknown list entries)"""
+        n, off, buf = self._pack(messages)
+        self._n_cons = 0
+        a, b = C.c_int64(0), C.c_int64(0)
+        N.check(N.lib().rapid_wire_decode_consensus(self._h, int(kind), N.ptr(buf), N.ptr(off), n, N.WIRE_REQUEST if is_request else 0,
+                                                    C.byref(a), C.byref(b)))
+        self._n_cons = n
+        return a.value, b.value
+
+    def consensusMessages(self):
+        """per message of the last consensus decode: dict of arrays sender, cfg, rnd_round, rnd_node, vrnd_round, vrnd_node,
+        hash, hash2, len"""
+        n = getattr(self, "_n_cons", 0)
+        out = {"sender": np.zeros(n, np.int32), "cfg": np.zeros(n, np.int64), "rnd_round": np.zeros(n, np.int32),
+               "rnd_node": np.zeros(n, np.int32), "vrnd_round": np.zeros(n, np.int32), "vrnd_node": np.zeros(n, np.int32),
+               "hash": np.zeros(n, np.uint64), "hash2": np.zeros(n, np.uint64), "len": np.zeros(n, np.int32)}
+        N.check(N.lib().rapid_wire_read_consensus(self._h, *[N.ptr(out[k]) for k in ("sender", "cfg", "rnd_round", "rnd_node", "vrnd_round",
+                                                                                   "vrnd_node", "hash", "hash2", "len")]))
+        return out
+
+    def consensusValue(self, index):
+        """the list of message `index` of the last consensus decode as ids in wire order (-1: endpoint not in the dictionary)"""
+        ln = C.c_int32(0)
+        N.check(N.lib().rapid_wire_consensus_value(self._h, int(index), None, 0, C.byref(ln)))
+        ids = np.zeros(max(ln.value, 1), np.int32)
+        N.check(N.lib().rapid_wire_consensus_value(self._h, int(index), N.ptr(ids), ln.value, C.byref(ln)))
+        return ids[:ln.value].tolist()
 
     def lastDeviceMs(self):
         out = C.c_float(0)
