@@ -406,6 +406,14 @@ int32_t rapid_px_phase2b_from_acceptor_shards(rapid_px* px, const rapid_pxa* con
                                               uint64_t* decided_hash2, int32_t* decided_len);
 /* State of one acceptor: ranks[4] = rnd.round, rnd.node_index, vrnd.round, vrnd.node_index; its vval triple. */
 int32_t rapid_pxa_read(const rapid_pxa* a, int64_t acceptor, int32_t* ranks, uint64_t* hash, uint64_t* hash2, int32_t* len);
+/* Crashed processes never answer: acceptors with silent[r] != 0 (host array of n_acceptors bytes) change no state and send
+ * nothing in rapid_pxa_phase1a / rapid_pxa_phase2a from now on.  silent == NULL clears the mask (every acceptor answers). */
+int32_t rapid_pxa_set_silent(rapid_pxa* a, const uint8_t* silent);
+/* *acceptor = the lowest local acceptor index whose vval is (hash, hash2, len), or -1 if none holds it.  A fast-round decision
+ * is always some registered vote and a classic cval always some acceptor's vval, so called BEFORE rapid_pxa_phase2a overwrites
+ * the vvals with the decided value this finds a proposer of it; with acceptors = detector receivers,
+ * rapid_cd_get_proposal(that receiver) gives the value as ids. */
+int32_t rapid_pxa_find_value(const rapid_pxa* a, uint64_t hash, uint64_t hash2, int32_t len, int64_t* acceptor);
 
 /* ------------------------------------------------------------------------------------------------
  * Wire-format ingest  (rapid.proto; SURVEY.md §8 f3) — the step BEFORE the path: serialized protobuf bytes, as
@@ -532,6 +540,17 @@ int32_t rapid_fdet_cells_dev(const rapid_fdet* fd, const int32_t** src, const in
  * window (MembershipService.java:613-637): batch b = the cells raised by one observer.  batch_off[0 .. *n_batches] feeds
  * rapid_cd_apply_batches_dev together with rapid_fdet_cells_dev; RAPID_ENOMEM (with *n_batches set) if cap is too small. */
 int32_t rapid_fdet_sender_batches(const rapid_fdet* fd, int64_t* batch_off, int64_t cap, int64_t* n_batches);
+/* Join phase 2 (MembershipService.java:232-281) in the interval of the last tick: for every listed registered joiner j (host
+ * array of view ids), each of its K expected observers o (predecessors of j on the rings) that is not RAPID_FD_CRASHED in that
+ * tick's node flags raises ONE AlertMessage{edgeSrc = o, edgeDst = j, UP, cfg_id, ring numbers = {k : observer k of j is o}}.
+ * They join the interval's alerts and cells, re-ordered so that every sender's alerts stay contiguous: by sender, the
+ * detectors' alerts first (tick order), then the join alerts in the order the joiners are listed.  rapid_fdet_sender_batches,
+ * rapid_fdet_cells_dev and rapid_fdet_read_* then describe the merged interval.  An id that is not a registered joiner gives
+ * RAPID_EINVAL and leaves the interval as the tick made it.  One call per tick: a second call before the next tick gives
+ * RAPID_EINVAL and changes nothing (list every joiner of the interval in one call).  *n_alerts / *n_cells: totals of the
+ * merged interval.  After rapid_fdet_tick_dev the caller's node_flags_dev must still hold that tick's flags. */
+int32_t rapid_fdet_join_alerts(rapid_fdet* fd, const int32_t* joiner_ids, int64_t n, int64_t cfg_id, int64_t* n_alerts,
+                               int64_t* n_cells);
 int32_t rapid_fdet_read_cells(const rapid_fdet* fd, int32_t* src, int32_t* dst, uint8_t* ring, uint8_t* status, int64_t* cfg);
 int32_t rapid_fdet_read_alerts(const rapid_fdet* fd, int32_t* observer, int32_t* subject, uint16_t* ring_mask);
 /* failureCount / notified of node's k-th detector */

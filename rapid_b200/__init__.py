@@ -12,7 +12,8 @@ from .fast_paxos import FastPaxos, NcclComm, quorum
 from .classic_paxos import Paxos, PaxosAcceptors
 from .wire import WireDecoder
 from .failure_detector import EdgeFailureDetectors
+from .simulation import ClusterSimulation
 
-__all__ = ["MembershipView", "MultiNodeCutDetector", "VirtualCluster", "FastPaxos", "NcclComm", "quorum", "Paxos", "PaxosAcceptors", "WireDecoder", "EdgeFailureDetectors",
+__all__ = ["MembershipView", "MultiNodeCutDetector", "VirtualCluster", "FastPaxos", "NcclComm", "quorum", "Paxos", "PaxosAcceptors", "WireDecoder", "EdgeFailureDetectors", "ClusterSimulation",
            "proposal_fingerprint", "UP", "DOWN", "RapidError", "NodeNotInRingException",
            "NodeAlreadyInRingException", "UUIDAlreadySeenException", "HashCollisionError"]

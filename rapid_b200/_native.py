@@ -140,6 +140,7 @@ SIGNATURES = {
     "rapid_fdet_tick_dev": [_vp, _p, _p, _i64, _p, _p],
     "rapid_fdet_cells_dev": [_vp, _p, _p, _p, _p, _p],
     "rapid_fdet_sender_batches": [_vp, _p, _i64, _p],
+    "rapid_fdet_join_alerts": [_vp, _p, _i64, _i64, _p, _p],
     "rapid_fdet_read_cells": [_vp, _p, _p, _p, _p, _p],
     "rapid_fdet_read_alerts": [_vp, _p, _p, _p],
     "rapid_fdet_state": [_vp, _i64, _i32, _p, _p],
@@ -160,6 +161,8 @@ SIGNATURES = {
     "rapid_px_phase1b_from_acceptor_shards": [_vp, _p, _i32, _vp, _u64, _p, _p, _p, _p, _p, _p],
     "rapid_px_phase2b_from_acceptor_shards": [_vp, _p, _i32, _vp, _u64, _p, _p, _p, _p, _p],
     "rapid_pxa_read": [_vp, _i64, _p, _p, _p, _p],
+    "rapid_pxa_set_silent": [_vp, _p],
+    "rapid_pxa_find_value": [_vp, _u64, _u64, _i32, _p],
 }
 
 

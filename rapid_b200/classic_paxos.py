@@ -233,6 +233,21 @@ class PaxosAcceptors:
                                           int(ln), C.byref(out)))
         return out.value
 
+    def setSilent(self, silent=None):
+        """acceptors with silent[r] != 0 (crashed processes) neither change nor answer in handlePhase1aMessage /
+        handlePhase2aMessage; None: every acceptor answers again"""
+        m = None if silent is None else N.as_u8(silent)
+        assert m is None or len(m) == self.R
+        N.check(N.lib().rapid_pxa_set_silent(self._h, N.ptr(m)))
+
+    def findValue(self, value):
+        """lowest acceptor index whose vval is value = (hash, hash2, len), -1 if none.  Finds a proposer of a decision when
+        called before handlePhase2aMessage overwrites the vvals"""
+        h1, h2, ln = value
+        out = C.c_int64(-1)
+        N.check(N.lib().rapid_pxa_find_value(self._h, int(h1), int(h2), int(ln), C.byref(out)))
+        return out.value
+
     def read(self, acceptor):
         """-> {'rnd': (r, i), 'vrnd': (r, i), 'vval': (hash, hash2, len)}"""
         rk = np.zeros(4, np.int32)

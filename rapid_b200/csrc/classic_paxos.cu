@@ -335,23 +335,37 @@ __global__ void k_pxa_register(int64_t n, const int64_t* __restrict__ acceptor, 
     rnd[r] = pack_rank(1, 1); vrnd[r] = pack_rank(1, 1);                             // :254-255
     h1[r] = vh1[i]; h2[r] = vh2 ? vh2[i] : 0; len[r] = vlen[i];                      // :256
 }
-// handlePhase1aMessage (:120-151) for one message; reply[r] = 1 where a Phase1bMessage goes back
-__global__ void k_pxa_phase1a(int64_t R, int64_t rank, int64_t* __restrict__ rnd, int32_t* __restrict__ reply) {
+// handlePhase1aMessage (:120-151) for one message; reply[r] = 1 where a Phase1bMessage goes back.  A silent acceptor (a
+// crashed process, rapid_pxa_set_silent) neither changes nor answers.
+__global__ void k_pxa_phase1a(int64_t R, int64_t rank, const uint8_t* __restrict__ silent, int64_t* __restrict__ rnd,
+                              int32_t* __restrict__ reply) {
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= R) return;
+    if (silent && silent[r]) { reply[r] = 0; return; }
     const bool up = rnd[r] < rank;                                                   // compareRanks(rnd, m.rank) < 0
     if (up) rnd[r] = rank;
     reply[r] = up ? 1 : 0;
 }
 // handlePhase2aMessage (:198-216) for one message; reply[r] = 1 where a Phase2bMessage is broadcast
-__global__ void k_pxa_phase2a(int64_t R, int64_t mr, uint64_t vh1, uint64_t vh2, int32_t vlen, int64_t* __restrict__ rnd,
-                              int64_t* __restrict__ vrnd, uint64_t* __restrict__ h1, uint64_t* __restrict__ h2,
+__global__ void k_pxa_phase2a(int64_t R, int64_t mr, uint64_t vh1, uint64_t vh2, int32_t vlen, const uint8_t* __restrict__ silent,
+                              int64_t* __restrict__ rnd, int64_t* __restrict__ vrnd, uint64_t* __restrict__ h1, uint64_t* __restrict__ h2,
                               int32_t* __restrict__ len, int32_t* __restrict__ reply) {
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= R) return;
+    if (silent && silent[r]) { reply[r] = 0; return; }
     const bool acc = rnd[r] <= mr && vrnd[r] != mr;                                  // :204
     if (acc) { rnd[r] = mr; vrnd[r] = mr; h1[r] = vh1; h2[r] = vh2; len[r] = vlen; }
     reply[r] = acc ? 1 : 0;
+}
+// lowest acceptor holding vval == (vh1, vh2, vlen): per warp a shuffle min, then one atomicMin per warp (*out = R before)
+__global__ void k_pxa_find(int64_t R, uint64_t vh1, uint64_t vh2, int32_t vlen, const uint64_t* __restrict__ h1,
+                           const uint64_t* __restrict__ h2, const int32_t* __restrict__ len, unsigned long long* __restrict__ out) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long best = (unsigned long long)R;
+    if (r < R && len[r] == vlen && h1[r] == vh1 && h2[r] == vh2) best = (unsigned long long)r;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
+    if ((threadIdx.x & 31) == 0 && best < (unsigned long long)R) atomicMin(out, best);
 }
 // compact the answering acceptors (arrival order = acceptor order, or by permutation key)
 __global__ void k_pxa_gather1b(int64_t R, const int32_t* __restrict__ reply, const int32_t* __restrict__ pos, int64_t begin,
@@ -454,6 +468,10 @@ struct PXA {
     DevBuf<int64_t> s_acc;
     DevBuf<uint64_t> s_h1, s_h2;
     DevBuf<int32_t> s_len;
+    DevBuf<uint8_t> silent;                // crashed acceptors (rapid_pxa_set_silent); has_silent == false: every acceptor answers
+    bool has_silent = false;
+    DevBuf<unsigned long long> found;
+    PinnedBuf<unsigned long long> h_found;
 };
 
 static const int TB = 256;
@@ -1157,7 +1175,7 @@ int32_t rapid_pxa_phase1a(rapid_pxa* a, int64_t msg_cfg, int32_t round, int32_t 
     DeviceGuard g(a->device);
     const int64_t rank = pack_rank(round, node_index);
     // answers carry the vrnd / vval each acceptor held when it answered, so they are gathered in the same pass
-    k_pxa_phase1a<<<grid_for(a->R), TB, 0, a->stream>>>(a->R, rank, a->rnd.p, a->reply.p);
+    k_pxa_phase1a<<<grid_for(a->R), TB, 0, a->stream>>>(a->R, rank, a->has_silent ? a->silent.p : nullptr, a->rnd.p, a->reply.p);
     RAPID_KERNEL_CHECK();
     RAPID_CHECK(pxa_compact(a, true));
     a->last_kind = 1; a->last_rank = rank;
@@ -1173,7 +1191,7 @@ int32_t rapid_pxa_phase2a(rapid_pxa* a, int64_t msg_cfg, int32_t round, int32_t 
     if (msg_cfg != a->cfg) return RAPID_OK;                                          // :199-201
     DeviceGuard g(a->device);
     const int64_t rank = pack_rank(round, node_index);
-    k_pxa_phase2a<<<grid_for(a->R), TB, 0, a->stream>>>(a->R, rank, hash, hash2, len, a->rnd.p, a->vrnd.p, a->h1.p, a->h2.p, a->len.p, a->reply.p);
+    k_pxa_phase2a<<<grid_for(a->R), TB, 0, a->stream>>>(a->R, rank, hash, hash2, len, a->has_silent ? a->silent.p : nullptr, a->rnd.p, a->vrnd.p, a->h1.p, a->h2.p, a->len.p, a->reply.p);
     RAPID_KERNEL_CHECK();
     RAPID_CHECK(pxa_compact(a, false));
     a->last_kind = 2; a->last_rank = rank; a->last_h1 = hash; a->last_h2 = hash2; a->last_len = len;
@@ -1243,6 +1261,32 @@ int32_t rapid_px_phase2b_from_acceptor_shards(rapid_px* px, const rapid_pxa* con
                                      decided_hash2, decided_len);
     if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
     return rc;
+}
+
+int32_t rapid_pxa_set_silent(rapid_pxa* a, const uint8_t* silent) {
+    if (!a) { set_error("NULL handle"); return RAPID_EINVAL; }
+    DeviceGuard g(a->device);
+    if (!silent) { a->has_silent = false; return RAPID_OK; }
+    RAPID_CHECK(upload(a->silent, silent, a->R, a->stream));
+    RAPID_CUDA(cudaStreamSynchronize(a->stream));                                    // the host array may go away after the call
+    a->has_silent = true;
+    return RAPID_OK;
+}
+
+int32_t rapid_pxa_find_value(const rapid_pxa* a, uint64_t hash, uint64_t hash2, int32_t len, int64_t* acceptor) {
+    if (!a || !acceptor) { set_error("bad arguments"); return RAPID_EINVAL; }
+    DeviceGuard g(a->device);
+    rapid_pxa* m = const_cast<rapid_pxa*>(a);                                        // scratch only; no acceptor state changes
+    cudaStream_t s = m->stream;
+    RAPID_CHECK(m->found.reserve(1)); RAPID_CHECK(m->h_found.reserve(1));
+    const unsigned long long none = (unsigned long long)a->R;
+    RAPID_CUDA(cudaMemcpyAsync(m->found.p, &none, sizeof(none), cudaMemcpyHostToDevice, s));
+    k_pxa_find<<<grid_for(a->R), TB, 0, s>>>(a->R, hash, hash2, len, a->h1.p, a->h2.p, a->len.p, m->found.p);
+    RAPID_KERNEL_CHECK();
+    RAPID_CUDA(cudaMemcpyAsync(m->h_found.p, m->found.p, sizeof(none), cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    *acceptor = *m->h_found.p < none ? (int64_t)*m->h_found.p : -1;
+    return RAPID_OK;
 }
 
 int32_t rapid_pxa_read(const rapid_pxa* a, int64_t acceptor, int32_t* ranks, uint64_t* hash, uint64_t* hash2, int32_t* len) {

@@ -251,6 +251,12 @@ class VirtualCluster:
         N.check(N.lib().rapid_cd_read_outputs(self._h, N.ptr(h1), N.ptr(h2), N.ptr(ln), N.ptr(ann)))
         return AlertBatchResult(h1, h2, ln, ann)
 
+    def readAnnounced(self):
+        """announcedProposal of every receiver (1 B each), without the proposal fingerprints readOutputs() copies too"""
+        ann = np.zeros(self.R, np.uint8)
+        N.check(N.lib().rapid_cd_read_outputs(self._h, None, None, None, N.ptr(ann)))
+        return ann
+
     def getProposal(self, receiver, cap=1 << 16):
         out = np.empty(cap, np.int32)
         cnt = C.c_int32(0)

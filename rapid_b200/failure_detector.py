@@ -43,6 +43,24 @@ class EdgeFailureDetectors:
         self.n_alerts, self.n_cells = a.value, c.value
         return a.value, c.value
 
+    def tickDevice(self, node_flags_dev, cfg_id, edge_fail_dev=None):
+        """tick() with the flags (and per-detector failures) already in device memory (raw pointers); the flags must stay
+        there until joinAlerts() of the same interval"""
+        a, c = C.c_int64(0), C.c_int64(0)
+        N.check(N.lib().rapid_fdet_tick_dev(self._h, node_flags_dev, edge_fail_dev or None, int(cfg_id), C.byref(a), C.byref(c)))
+        self.n_alerts, self.n_cells = a.value, c.value
+        return a.value, c.value
+
+    def joinAlerts(self, joiner_ids, cfg_id):
+        """join phase 2 (MembershipService.java:232-281) in the last tick's interval: every live expected observer of each listed
+        registered joiner raises one UP alert; merged per sender after the detectors' alerts, joiners in list order.
+        -> (number of AlertMessages, number of cells) of the merged interval"""
+        ids = N.as_i32(joiner_ids)
+        a, c = C.c_int64(0), C.c_int64(0)
+        N.check(N.lib().rapid_fdet_join_alerts(self._h, N.ptr(ids), len(ids), int(cfg_id), C.byref(a), C.byref(c)))
+        self.n_alerts, self.n_cells = a.value, c.value
+        return a.value, c.value
+
     def alerts(self):
         """[(observer, subject, [ring numbers])] of the last tick, in the order the notifiers fired"""
         n = self.n_alerts
@@ -51,6 +69,7 @@ class EdgeFailureDetectors:
         return [(int(o[i]), int(s[i]), [r for r in range(16) if (int(m[i]) >> r) & 1]) for i in range(n)]
 
     def cells(self):
+        """(src, dst, ring, status, cfg) of the interval's cells"""
         n = self.n_cells
         src, dst = np.zeros(n, np.int32), np.zeros(n, np.int32)
         ring, status, cfg = np.zeros(n, np.uint8), np.zeros(n, np.uint8), np.zeros(n, np.int64)

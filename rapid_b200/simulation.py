@@ -1,0 +1,313 @@
+"""A whole Rapid cluster simulated on the device, configuration after configuration: the loop MembershipService runs
+(alert generation -> per-sender alert batches -> cut detection -> fast round -> classic fallback -> decideViewChange,
+MembershipService.java:300-354, :385-444, FastPaxos.java:94-203), composed from the classes of this package.
+
+ClusterSimulation rules (tests/simref.py restates them independently; DESIGN.md §4.11):
+
+* Nodes are named by TAGS: the members given at creation are 0..n-1 in the given order, joiners get the next tags in the
+  order addJoiners() lists them.  Tags never change; the device ids of a configuration are dense (view.applyCut renumbers),
+  and the driver keeps the id -> tag map.  Scenario flags (failure_detector.CRASHED, INGRESS_BLOCKED, ...) are kept per tag,
+  so a view change carries them over; an admitted joiner starts with flags 0.
+* One interval, in this order:
+    1. one failure-detector interval of every member (EdgeFailureDetectors.tickDevice with the members' flags);
+    2. in the FIRST interval of a configuration only, every pending joiner asks again (joinAlerts, one join attempt per
+       configuration: its live expected observers each send one UP alert);
+    3. the interval's alerts, one batch per sender in ascending sender id, reach every receiver (receiver r = ring-0
+       position r) through VirtualCluster.handleBatchesDevice: crashed receivers get nothing, batch b reaches receiver r in
+       its own cell order seeded interval_seed(seed, cfg, interval) + b;
+    4. every receiver that announced registers its fast-round vote with its acceptor (FastPaxos.propose :94-98);
+    5. one FastPaxos tally of those votes; the tally accumulates over the configuration's intervals.
+  Steps 3-5 are skipped in an interval without alerts.
+* Fallback: if the fast round has not decided at the end of interval i0 + fallback_intervals (i0 = the configuration's
+  first interval with a proposal), the classic round runs in that interval: the coordinator is the proposer with the
+  smallest splitmix64(seed ^ tag) (a seeded stand-in for the expovariate jitter of FastPaxos.java:200-203); its
+  Phase1a has rank (2, coordinator tag); crashed acceptors are silent; Phase1b and Phase2b answers arrive in ascending
+  splitmix64(phase_seed ^ ring-0 position) order (phase_seed = classic_seeds(...)).  A classic round that does not decide
+  stalls the run.
+* View change (decideViewChange :385-444): a proposer of the decided value is found on the device
+  (PaxosAcceptors.findValue, before any Phase2a), its proposal is the cut; view.applyCut; joiners not admitted are
+  registered again with their NodeIds; the configuration id comes from the device's identifiersSeen; the detectors are
+  reset; the cut detector and the acceptors are created anew for the new membership size.
+* Delivery model (a limit): every receiver gets the senders' batches in the same (ascending sender) order; only the cell
+  order within a batch is per receiver.  The reference shuffles batch order per receiver (UnicastToAllBroadcaster.java:59-62).
+  Every node sees every vote, so one tally stands for every node's.
+"""
+import time
+
+import numpy as np
+
+from .classic_paxos import Paxos, PaxosAcceptors
+from .cut_detector import VirtualCluster
+from .failure_detector import CRASHED, EdgeFailureDetectors, FAILURE_THRESHOLD
+from .fast_paxos import FastPaxos
+from .membership_view import MembershipView
+from .workloads import splitmix64
+
+_M64 = 0xFFFFFFFFFFFFFFFF
+
+
+def _sm(x):
+    return int(splitmix64(np.uint64(x & _M64)))
+
+
+def interval_seed(seed, cfg, interval):
+    """cell-order seed of one interval: batch b of it is delivered with interval_seed + b"""
+    return _sm(_sm(seed ^ cfg) + interval)
+
+
+def classic_seeds(seed, cfg, interval):
+    """(Phase1b, Phase2b) arrival-order seeds of a classic round run in that interval (never 0: 0 means acceptor order)"""
+    s = interval_seed(seed, cfg, interval)
+    return _sm(s ^ 1) or 1, _sm(s ^ 2) or 1
+
+
+def coordinator(seed, proposer_tags):
+    """the proposer whose recovery timer fires first: smallest splitmix64(seed ^ tag), ties by tag"""
+    t = np.asarray(proposer_tags, np.uint64)
+    keys = splitmix64(t ^ np.uint64(seed & _M64))
+    return int(t[np.lexsort((t, keys))[0]])
+
+
+class ClusterSimulation:
+    """ClusterSimulation((host_bytes, host_off, ports), (id_high, id_low)): a cluster of the given members on one device.
+
+    setFlags / setEdgeFail / addJoiners describe the scenario; interval() runs one failure-detector interval of the whole
+    cluster; run() runs intervals until the membership has converged or the run stalls.  history holds one record per
+    configuration, intervals one per interval."""
+
+    def __init__(self, endpoints, node_ids, K=10, H=9, L=4, seed=0, failure_threshold=FAILURE_THRESHOLD, fallback_intervals=1,
+                 device=0):
+        import torch                                              # device buffers of the scenario's flags
+        self._torch = torch
+        self.K, self.H, self.L, self.seed, self.device = int(K), int(H), int(L), int(seed), device
+        self.fallback_intervals = int(fallback_intervals)
+        hb, off, ports = endpoints
+        self.view = MembershipView.from_packed(self.K, hb, off, ports, device=device)
+        self.view.setNodeIds(*node_ids)
+        n = len(ports)
+        self.tags = np.arange(n, dtype=np.int64)                  # device id -> tag
+        self.flags = np.zeros(n, np.uint8)                        # per tag
+        self.edge_fail = {}                                       # (tag, k) -> probes of that tag's k-th detector fail
+        self.joiners = {}                                         # tag -> (hostname, port, id_high, id_low)
+        self.pending = []                                         # joiner tags not yet admitted, in tag order
+        self.history, self.intervals = [], []
+        self.cfg = self.view.currentConfigurationId()
+        self.fd = EdgeFailureDetectors(self.view, failure_threshold)
+        self.fp = None
+        self._new_handles()
+
+    # ---- scenario ------------------------------------------------------------------------------------------------------------
+    def setFlags(self, node, flags):
+        """RAPID_FD_* bits of a node (tag); applies from the next interval"""
+        self.flags[int(node)] = np.uint8(flags)
+        self._dirty = True
+
+    def setEdgeFail(self, node, k, fail=True):
+        """probes of node's k-th detector (k-th entry of getSubjectsOf, current configuration) fail regardless of flags"""
+        if fail:
+            self.edge_fail[(int(node), int(k))] = True
+        else:
+            self.edge_fail.pop((int(node), int(k)), None)
+        self._dirty = True
+
+    def addJoiners(self, hostnames, ports, id_high, id_low):
+        """endpoints that ask to join from the next configuration's first interval on (the current one if it has not run an
+        interval yet); -> their tags"""
+        first = len(self.flags)
+        tags = list(range(first, first + len(ports)))
+        for i, t in enumerate(tags):
+            self.joiners[t] = (hostnames[i], int(ports[i]), int(id_high[i]), int(id_low[i]))
+        self.flags = np.concatenate([self.flags, np.zeros(len(tags), np.uint8)])
+        self._register(tags)
+        self.pending += tags
+        return tags
+
+    def members(self):
+        """tags of the current members, in device id order"""
+        return self.tags.tolist()
+
+    def converged(self):
+        return not self.flags[self.tags].any() and not self.pending
+
+    # ---- handles of one configuration ------------------------------------------------------------------------------------------
+    def _register(self, tags):
+        if not tags:
+            return
+        ids = self.view.registerJoiners([self.joiners[t][0] for t in tags], [self.joiners[t][1] for t in tags])
+        self.view.setJoinerIds(ids[0], [self.joiners[t][2] for t in tags], [self.joiners[t][3] for t in tags])
+        self.joiner_id.update(zip(tags, ids))
+
+    def _new_handles(self):
+        n = self.view.n
+        self.N = n
+        self.cl = VirtualCluster(self.view, self.H, self.L, kernel="bucketed")
+        self.acc = PaxosAcceptors(self.cfg, n, device=self.device)
+        if self.fp is None or n > self._fp_cap:
+            self.fp, self._fp_cap = FastPaxos(self.cfg, n, device=self.device), n
+        else:
+            self.fp.reset(self.cfg, n)
+        self.ring0 = np.asarray(self.view.getRing(0), np.int64)
+        self.joiner_id = {}
+        self.interval_in_cfg = 0
+        self.first_proposal = None
+        self.votes = 0
+        self.announced = 0
+        self._ann = None                                          # announcedProposal flags, read at most once per interval
+        self._dirty = True
+        self._cfg_t = {"detect_ms": 0.0, "classic_ms": 0.0, "view_change_ms": 0.0, "handles_ms": 0.0, "device_ms": 0.0}
+
+    def _upload_flags(self):
+        torch = self._torch
+        f = self.flags[self.tags]
+        self.d_flags = torch.from_numpy(np.ascontiguousarray(f)).to("cuda:%d" % self.device)
+        self.crashed_r = (f[self.ring0] & CRASHED) != 0                  # per receiver / acceptor
+        self.d_blocked = torch.from_numpy(self.crashed_r.astype(np.uint8)).to("cuda:%d" % self.device)
+        self.d_edge = None
+        if self.edge_fail:
+            pos = {int(t): i for i, t in enumerate(self.tags)}
+            e = np.zeros(self.N * self.K, np.uint8)
+            for (t, k) in self.edge_fail:
+                if t in pos:
+                    e[pos[t] * self.K + k] = 1
+            self.d_edge = torch.from_numpy(e).to("cuda:%d" % self.device)
+        self._dirty = False
+
+    # ---- one interval ----------------------------------------------------------------------------------------------------------
+    def interval(self):
+        """one failure-detector interval of the cluster -> its record (also appended to intervals); record["event"] is
+        quiet / alerts / proposals / decided-fast / decided-classic (the view has changed) / stalled"""
+        t0 = time.perf_counter()
+        self._ann = None
+        if self._dirty:
+            self._upload_flags()
+        i, cfg = self.interval_in_cfg, self.cfg
+        na, nc = self.fd.tickDevice(self.d_flags.data_ptr(), cfg, 0 if self.d_edge is None else self.d_edge.data_ptr())
+        dev_ms = self.fd.lastDeviceMs()
+        if i == 0 and self.pending:
+            na, nc = self.fd.joinAlerts([self.joiner_id[t] for t in self.pending], cfg)
+        rec = {"cfg": cfg, "interval": i, "alerts": na, "cells": nc, "announced": 0, "event": "quiet"}
+        decided = None
+        if nc:
+            rec["event"] = "alerts"
+            p = self.fd.cellsDevice()
+            self.cl.handleBatchesDevice(cfg, nc, p[1], p[2], p[3], self.fd.senderBatches(), cell_cfg_dev=p[4],
+                                        blocked_dev=self.d_blocked.data_ptr(), perm_seed=interval_seed(self.seed, cfg, i))
+            dev_ms += self.cl.lastDeviceMs()[0]
+            self.acc.registerFastRoundVotesFrom(self.cl)
+            t = self.fp.tallyCluster(self.cl)
+            dev_ms += self.fp.lastDeviceMs()
+            # votes are counted up to the decision (FastPaxos.java:138): in a deciding interval the announcers are counted instead,
+            # from the announcedProposal flags (1 B per receiver, read once per configuration)
+            rec["announced"] = int(self._announced_flags().sum()) - self.announced if t.decided else t.votes_received - self.votes
+            self.votes = t.votes_received
+            if rec["announced"]:
+                rec["event"] = "proposals"
+                self.announced += rec["announced"]
+                if self.first_proposal is None:
+                    self.first_proposal = i
+            if t.decided:
+                decided = ("fast", (t.hash, t.hash2, t.length))
+        self._cfg_t["detect_ms"] += (time.perf_counter() - t0) * 1e3
+        if decided is None and self.first_proposal is not None and i - self.first_proposal >= self.fallback_intervals:
+            t1 = time.perf_counter()
+            value, ms = self._classic_round(cfg, i)
+            self._cfg_t["classic_ms"] += (time.perf_counter() - t1) * 1e3
+            dev_ms += ms
+            if value is None:
+                rec["event"] = "stalled"
+            else:
+                decided = ("classic", value)
+        self._cfg_t["device_ms"] += dev_ms
+        rec["device_ms"] = dev_ms
+        self.interval_in_cfg += 1
+        if decided is not None:
+            rec["event"] = "decided-" + decided[0]
+            self._view_change(decided[0], decided[1], i)
+        self.intervals.append(rec)
+        return rec
+
+    def _classic_round(self, cfg, i):
+        """Paxos.java round 2 from the seeded coordinator over the acceptors -> (decided value or None, device ms)"""
+        ann = self._announced_flags() != 0
+        coord = coordinator(self.seed, self.tags[self.ring0[ann]])
+        s1, s2 = classic_seeds(self.seed, cfg, i)
+        px = Paxos(cfg, self.N, device=self.device)
+        try:
+            return self._rounds(px, coord, s1, s2)
+        finally:
+            px.close()
+
+    def _rounds(self, px, coord, s1, s2):
+        px.startPhase1a(2, coord)
+        self.acc.setSilent(self.crashed_r)
+        self.acc.handlePhase1aMessage((2, coord))
+        r1 = px.handlePhase1bFromAcceptors(self.acc, perm_seed=s1)
+        ms = px.lastDeviceMs()
+        if not r1.proposed:
+            return None, ms
+        self._proposer = self.acc.findValue(r1.cval)                # before Phase2a overwrites the vvals
+        self.acc.handlePhase2aMessage((2, coord), r1.cval)
+        r2 = px.handlePhase2bFromAcceptors(self.acc, perm_seed=s2)
+        ms += px.lastDeviceMs()
+        return (r2.decision if r2.decided else None), ms
+
+    def _announced_flags(self):
+        if self._ann is None:
+            self._ann = self.cl.readAnnounced()
+        return self._ann
+
+    def _view_change(self, path, value, i):
+        t0 = time.perf_counter()
+        r = self._proposer if path == "classic" else self.acc.findValue(value)
+        assert r >= 0, "a decided value is some acceptor's vote"
+        cut = self.cl.getProposal(r)
+        old_tags = np.concatenate([self.tags, np.zeros(self.view.numJoiners(), np.int64)])
+        for t, j in self.joiner_id.items():
+            old_tags[j] = t
+        cut_tags = sorted(int(old_tags[c]) for c in cut)
+        mapping = self.view.applyCut(cut)
+        new_tags = np.zeros(self.view.n, np.int64)
+        kept = mapping >= 0
+        new_tags[mapping[kept]] = old_tags[kept]
+        self.tags = new_tags
+        admitted = set(cut_tags) & set(self.joiners)
+        self.flags[list(admitted)] = 0
+        self.pending = [t for t in self.pending if t not in admitted]
+        before, size_before = self.cfg, self.N
+        self.cfg = self.view.currentConfigurationId()
+        self._cfg_t["view_change_ms"] += (time.perf_counter() - t0) * 1e3
+        t1 = time.perf_counter()
+        self.fd.reset()
+        self.cl.close()
+        self.acc.close()
+        times, announced, votes = self._cfg_t, self.announced, self.votes
+        self._new_handles()
+        self._register(self.pending)
+        times["handles_ms"] += (time.perf_counter() - t1) * 1e3
+        self.history.append({"cfg_before": before, "cfg_after": self.cfg, "size_before": size_before, "size": self.view.n,
+                             "cut": cut_tags, "path": path, "intervals": i + 1, "announced": announced,
+                             "votes": votes, "members": sorted(self.tags.tolist()), **times})
+
+    # ---- whole runs --------------------------------------------------------------------------------------------------------------
+    def run(self, max_intervals):
+        """intervals until no flagged node is a member and no joiner is pending (converged), a classic round fails, or
+        max_intervals pass without a view change (stalled) -> {"converged", "stalled", "intervals", "stuck"}; stuck = the
+        flagged members and pending joiners the run waits on"""
+        since, total = 0, 0
+        t0 = time.perf_counter()
+        while not self.converged():
+            if since >= max_intervals:
+                break
+            rec = self.interval()
+            total += 1
+            since = 0 if rec["event"].startswith("decided") else since + 1
+            if rec["event"] == "stalled":
+                break
+        done = self.converged()
+        stuck = sorted(set(int(t) for t in self.tags[self.flags[self.tags] != 0]) | set(self.pending))
+        return {"converged": done, "stalled": not done, "intervals": total, "stuck": stuck,
+                "wall_ms": (time.perf_counter() - t0) * 1e3}
+
+    def close(self):
+        for h in (self.cl, self.acc, self.fp, self.fd):
+            h.close()
