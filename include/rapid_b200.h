@@ -548,9 +548,26 @@ int32_t rapid_fdet_sender_batches(const rapid_fdet* fd, int64_t* batch_off, int6
  * rapid_fdet_cells_dev and rapid_fdet_read_* then describe the merged interval.  An id that is not a registered joiner gives
  * RAPID_EINVAL and leaves the interval as the tick made it.  One call per tick: a second call before the next tick gives
  * RAPID_EINVAL and changes nothing (list every joiner of the interval in one call).  *n_alerts / *n_cells: totals of the
- * merged interval.  After rapid_fdet_tick_dev the caller's node_flags_dev must still hold that tick's flags. */
+ * merged interval.  After rapid_fdet_tick_dev the caller's node_flags_dev must still hold that tick's flags.
+ * Same as rapid_fdet_merge_alerts(fd, joiner_ids, n, NULL, 0, cfg_id, n_alerts, n_cells). */
 int32_t rapid_fdet_join_alerts(rapid_fdet* fd, const int32_t* joiner_ids, int64_t n, int64_t cfg_id, int64_t* n_alerts,
                                int64_t* n_cells);
+/* Join and leave alerts merged into the interval of the last tick, in one call.
+ * Join candidates: as rapid_fdet_join_alerts (UP, one alert per distinct live expected observer).
+ * Leave candidates (MembershipService.leave :545-565 -> handleLeaveMessage :372-376 -> edgeFailureNotification :472-495): for
+ * every listed member l (host array of view ids) and every k in 0..K-1, o = observer k of l (getObserversOf, the obs row of l)
+ * raises one AlertMessage{edgeSrc = o, edgeDst = l, DOWN, cfg_id, ring numbers = {r : observer r of l is o}} unless o is
+ * RAPID_FD_CRASHED in the tick's node flags.  Repeats are kept, as the reference sends one LeaveMessage per entry of
+ * getObserversOf: an observer on m rings of l raises m identical alerts, so a leaver whose observers all live raises K alerts
+ * and sum_o m_o^2 cells.  The leaver's own flags are not read (it has shut down; callers mark it crashed in the same tick).
+ * Only RAPID_FD_CRASHED silences an observer.  In a view of fewer than 2 members a leave raises nothing (:240-242).
+ * Order per sender: the tick's alerts (tick order), then the join alerts (list order), then the leave alerts (list order, then
+ * k).  RAPID_EINVAL, with the interval exactly as the tick made it: an id that is not a registered joiner (joiner_ids) or not a
+ * member (leaver_ids), 2^30 or more candidates (tick alerts + K per listed id), a view changed since the tick, no tick yet, or
+ * a second merge into the same interval ("already added", whichever kinds the first call carried).  An accepted merge sets
+ * rapid_fdet_last_device_ms to its own device time (0 if it launched nothing). */
+int32_t rapid_fdet_merge_alerts(rapid_fdet* fd, const int32_t* joiner_ids, int64_t n_joiners, const int32_t* leaver_ids,
+                                int64_t n_leavers, int64_t cfg_id, int64_t* n_alerts, int64_t* n_cells);
 int32_t rapid_fdet_read_cells(const rapid_fdet* fd, int32_t* src, int32_t* dst, uint8_t* ring, uint8_t* status, int64_t* cfg);
 int32_t rapid_fdet_read_alerts(const rapid_fdet* fd, int32_t* observer, int32_t* subject, uint16_t* ring_mask);
 /* failureCount / notified of node's k-th detector */

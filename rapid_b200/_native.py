@@ -141,6 +141,7 @@ SIGNATURES = {
     "rapid_fdet_cells_dev": [_vp, _p, _p, _p, _p, _p],
     "rapid_fdet_sender_batches": [_vp, _p, _i64, _p],
     "rapid_fdet_join_alerts": [_vp, _p, _i64, _i64, _p, _p],
+    "rapid_fdet_merge_alerts": [_vp, _p, _i64, _p, _i64, _i64, _p, _p],
     "rapid_fdet_read_cells": [_vp, _p, _p, _p, _p, _p],
     "rapid_fdet_read_alerts": [_vp, _p, _p, _p],
     "rapid_fdet_state": [_vp, _i64, _i32, _p, _p],

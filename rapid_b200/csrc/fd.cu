@@ -89,14 +89,16 @@ __global__ void k_fd_emit(int32_t nf, uint32_t K, const uint32_t* __restrict__ f
 }
 __global__ void k_fd_begin(FdScal* sc) { sc->n_fired = 0; sc->n_cells = 0; }
 
-// ---- join alerts merged into the interval (rapid_fdet_join_alerts) ------------------------------------------------------------
-// Candidate m < nf is the tick's alert m; candidate nf + i * K + k is observer k of listed joiner i.  A joiner raises one alert
-// per distinct live observer (its first ring), so a candidate is kept iff it is an alert or such a first ring.  Sort key =
-// (sender << mb) | candidate, candidate < 2^mb: per sender, the tick's alerts first in their order, then the join alerts in list
-// order.  A dropped candidate gets all ones, above every kept key in the sorted bits.
-__global__ void k_fd_join_keys(int64_t M, int32_t nf, uint32_t K, int mb, const int32_t* __restrict__ a_obs, const int32_t* __restrict__ jids,
-                               const int32_t* __restrict__ obs_tab, const uint8_t* __restrict__ flags, uint64_t* __restrict__ key,
-                               FdScal* __restrict__ sc) {
+// ---- join and leave alerts merged into the interval (rapid_fdet_merge_alerts) ----------------------------------------------------
+// ids[0 .. nj) are the listed joiners, ids[nj .. nj + nl) the listed leavers; the rows of both are obs[id][K] (a joiner's expected
+// observers, a member's getObserversOf).  Candidate m < nf is the tick's alert m; candidate nf + i * K + k is observer k of ids[i],
+// so the candidates are laid out [tick | joins * K | leaves * K].  A joiner raises one alert per distinct live observer (its first
+// ring); a leaver one per live observer and ring, repeats kept (MembershipService.leave sends one LeaveMessage per entry of
+// getObserversOf).  Sort key = (sender << mb) | candidate, candidate < 2^mb: per sender, the tick's alerts first in their order,
+// then the join alerts, then the leave alerts, each in list order.  A dropped candidate gets all ones, above every kept key.
+__global__ void k_fd_merge_keys(int64_t M, int32_t nf, uint32_t K, int64_t nj, int mb, const int32_t* __restrict__ a_obs,
+                                const int32_t* __restrict__ ids, const int32_t* __restrict__ obs_tab, const uint8_t* __restrict__ flags,
+                                uint64_t* __restrict__ key, FdScal* __restrict__ sc) {
     const int64_t m = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (m >= M) return;
     int32_t o;
@@ -106,18 +108,19 @@ __global__ void k_fd_join_keys(int64_t M, int32_t nf, uint32_t K, int mb, const 
     } else {
         const int64_t s = m - nf, i = s / K;
         const uint32_t k = (uint32_t)(s - i * K);
-        const int32_t* row = obs_tab + (int64_t)jids[i] * K;
+        const int32_t* row = obs_tab + (int64_t)ids[i] * K;
         o = row[k];
-        for (uint32_t q = 0; q < k; ++q) keep &= row[q] != o;
+        if (i < nj)                                                              // a joiner's observer sends once, on its first ring
+            for (uint32_t q = 0; q < k; ++q) keep &= row[q] != o;
         keep &= !(flags[o] & RAPID_FD_CRASHED);                                  // a crashed observer sends nothing
     }
     key[m] = keep ? (((uint64_t)(uint32_t)o << mb) | (uint64_t)m) : ~0ull;
     if (keep) atomicAdd(&sc->n_fired, 1);
 }
-// ring numbers of every kept alert, in merged order
-__global__ void k_fd_join_count(int32_t nv, int32_t nf, uint32_t K, int mb, const uint64_t* __restrict__ skey, const uint16_t* __restrict__ a_mask,
-                                const int32_t* __restrict__ jids, const int32_t* __restrict__ obs_tab, uint16_t* __restrict__ mask,
-                                int32_t* __restrict__ cnt) {
+// ring numbers of every kept alert, in merged order: {r : obs[id][r] == sender} for a join or leave alert
+__global__ void k_fd_merge_count(int32_t nv, int32_t nf, uint32_t K, int mb, const uint64_t* __restrict__ skey, const uint16_t* __restrict__ a_mask,
+                                 const int32_t* __restrict__ ids, const int32_t* __restrict__ obs_tab, uint16_t* __restrict__ mask,
+                                 int32_t* __restrict__ cnt) {
     const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nv) return;
     const int64_t m = (int64_t)(skey[i] & ((1ull << mb) - 1));
@@ -126,7 +129,7 @@ __global__ void k_fd_join_count(int32_t nv, int32_t nf, uint32_t K, int mb, cons
         mk = a_mask[m];
     } else {
         const int64_t s = m - nf, j = s / K;
-        const int32_t* row = obs_tab + (int64_t)jids[j] * K;
+        const int32_t* row = obs_tab + (int64_t)ids[j] * K;
         const int32_t o = (int32_t)(skey[i] >> mb);
         mk = 0;
         for (uint32_t r = 0; r < K; ++r) mk |= (row[r] == o ? 1u : 0u) << r;
@@ -134,21 +137,22 @@ __global__ void k_fd_join_count(int32_t nv, int32_t nf, uint32_t K, int mb, cons
     mask[i] = (uint16_t)mk;
     cnt[i] = __popc(mk);
 }
-__global__ void k_fd_join_emit(int32_t nv, int32_t nf, uint32_t K, int mb, const uint64_t* __restrict__ skey, const int32_t* __restrict__ a_subj,
-                               const int32_t* __restrict__ jids, const uint16_t* __restrict__ mask, const int32_t* __restrict__ cnt,
-                               const int32_t* __restrict__ pos, int64_t tick_cfg, int64_t join_cfg, int32_t* __restrict__ o_obs,
-                               int32_t* __restrict__ o_subj, int32_t* __restrict__ c_src,
-                               int32_t* __restrict__ c_dst, uint8_t* __restrict__ c_ring, uint8_t* __restrict__ c_status,
-                               int64_t* __restrict__ c_cfg, FdScal* __restrict__ sc) {
+__global__ void k_fd_merge_emit(int32_t nv, int32_t nf, uint32_t K, int64_t nj, int mb, const uint64_t* __restrict__ skey,
+                                const int32_t* __restrict__ a_subj, const int32_t* __restrict__ ids, const uint16_t* __restrict__ mask,
+                                const int32_t* __restrict__ cnt, const int32_t* __restrict__ pos, int64_t tick_cfg, int64_t merge_cfg,
+                                int32_t* __restrict__ o_obs, int32_t* __restrict__ o_subj, int32_t* __restrict__ c_src,
+                                int32_t* __restrict__ c_dst, uint8_t* __restrict__ c_ring, uint8_t* __restrict__ c_status,
+                                int64_t* __restrict__ c_cfg, FdScal* __restrict__ sc) {
     const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nv) return;
     if (i == nv - 1) sc->n_cells = pos[i] + cnt[i];
     const int64_t m = (int64_t)(skey[i] & ((1ull << mb) - 1));
     const int32_t o = (int32_t)(skey[i] >> mb);
-    const bool join = m >= nf;
-    const int32_t s = join ? jids[(m - nf) / K] : a_subj[m];
-    const uint8_t st = join ? RAPID_EDGE_UP : RAPID_EDGE_DOWN;
-    const int64_t cc = join ? join_cfg : tick_cfg;
+    const bool tick = m < nf;
+    const int64_t j = tick ? 0 : (m - nf) / K;
+    const int32_t s = tick ? a_subj[m] : ids[j];
+    const uint8_t st = (!tick && j < nj) ? RAPID_EDGE_UP : RAPID_EDGE_DOWN;
+    const int64_t cc = tick ? tick_cfg : merge_cfg;
     const uint32_t mk = mask[i];
     int32_t c = pos[i];
     for (uint32_t r = 0; r < K; ++r) {
@@ -181,10 +185,10 @@ struct FD {
     DevBuf<uint16_t> a_mask;
     DevBuf<uint8_t> c_ring, c_status;
     DevBuf<int64_t> c_cfg;
-    // the last tick's node flags / configuration (join alerts skip crashed observers of that interval), and the merge's buffers
+    // the last tick's node flags / configuration (merged alerts skip crashed observers of that interval), and the merge's buffers
     const uint8_t* tick_flags = nullptr;
     int64_t tick_cfg = 0;
-    bool joined = false;                   // join alerts were merged into this interval already
+    bool merged = false;                   // join / leave alerts were merged into this interval already
     DevBuf<int32_t> j_ids, m_obs, m_subj, m_src, m_dst;
     DevBuf<uint64_t> j_key, j_skey;
     DevBuf<uint16_t> m_mask;
@@ -221,7 +225,7 @@ static int32_t fd_tick_device(FD* fd, const uint8_t* d_flags, const uint8_t* d_e
     cudaStream_t s = fd->stream;
     const int64_t D = fd->n * fd->K;
     fd->n_alerts = fd->n_cells = 0;
-    fd->tick_flags = d_flags; fd->tick_cfg = cfg; fd->joined = false;
+    fd->tick_flags = d_flags; fd->tick_cfg = cfg; fd->merged = false;
     if (fd->n >= 2 && D > 0) {                               // getSubjectsOf is empty in a one-node view (MembershipView.java:270-272)
         k_fd_begin<<<1, 1, 0, s>>>(fd->sc.p);
         k_fd_tick<<<grid_for(D), TB, 0, s>>>((uint32_t)D, (uint32_t)fd->K, fd->view->subj.p, d_flags, d_edge, fd->thr, fd->boot_thr, fd->st.p,
@@ -359,47 +363,57 @@ int32_t rapid_fdet_sender_batches(const rapid_fdet* h, int64_t* batch_off, int64
     return RAPID_OK;
 }
 
-int32_t rapid_fdet_join_alerts(rapid_fdet* h, const int32_t* joiner_ids, int64_t n, int64_t cfg_id, int64_t* n_alerts, int64_t* n_cells) {
+int32_t rapid_fdet_merge_alerts(rapid_fdet* h, const int32_t* joiner_ids, int64_t n_joiners, const int32_t* leaver_ids, int64_t n_leavers,
+                                int64_t cfg_id, int64_t* n_alerts, int64_t* n_cells) {
     rapid_fdet* fd = h;
-    if (!fd || n < 0 || (n && !joiner_ids)) { set_error("bad arguments"); return RAPID_EINVAL; }
+    if (!fd || n_joiners < 0 || (n_joiners && !joiner_ids) || n_leavers < 0 || (n_leavers && !leaver_ids)) { set_error("bad arguments"); return RAPID_EINVAL; }
     if (fd->view_epoch != fd->view->member_epoch || fd->n != fd->view->n) { set_error("the view changed: call rapid_fdet_reset"); return RAPID_EINVAL; }
     if (!fd->tick_flags) { set_error("no interval to add join alerts to (call rapid_fdet_tick first)"); return RAPID_EINVAL; }
-    // the merged list no longer tells the tick's alerts from join alerts: a second merge would turn earlier UP alerts into DOWN ones
-    if (fd->joined) { set_error("join alerts were already added to this interval (one call per tick)"); return RAPID_EINVAL; }
+    // the merged list no longer tells the tick's alerts from merged ones: a second merge would turn earlier UP alerts into DOWN ones
+    if (fd->merged) { set_error("join alerts were already added to this interval (one call per tick)"); return RAPID_EINVAL; }
     const View* v = fd->view;
-    for (int64_t i = 0; i < n; ++i)
+    for (int64_t i = 0; i < n_joiners; ++i)
         if (joiner_ids[i] < v->n || joiner_ids[i] >= v->n + v->nj) { set_error("id %d is not a registered joiner", joiner_ids[i]); return RAPID_EINVAL; }
-    const int64_t nf = fd->n_alerts, M = nf + n * fd->K;
-    if (M >= (1LL << 30)) { set_error("too many join alerts in one interval"); return RAPID_EINVAL; }
+    for (int64_t i = 0; i < n_leavers; ++i)
+        if (leaver_ids[i] < 0 || leaver_ids[i] >= v->n) { set_error("id %d is not a member", leaver_ids[i]); return RAPID_EINVAL; }
+    const int64_t nl = fd->n >= 2 ? n_leavers : 0;          // getObserversOf is empty in a one-node view (MembershipView.java:240-242)
+    const int64_t nf = fd->n_alerts, lim = 1LL << 30;
+    if (n_joiners >= lim || nl >= lim || nf + (n_joiners + nl) * fd->K >= lim) {
+        set_error("too many %s alerts in one interval", n_leavers ? "join and leave" : "join"); return RAPID_EINVAL;
+    }
+    const int64_t nj = n_joiners, ni = nj + nl, M = nf + ni * fd->K;
     DeviceGuard g(fd->device);
     cudaStream_t s = fd->stream;
     const uint32_t K = (uint32_t)fd->K;
-    if (n > 0) {
-        RAPID_CHECK(fd->j_ids.reserve((size_t)n)); RAPID_CHECK(fd->j_key.reserve((size_t)M)); RAPID_CHECK(fd->j_skey.reserve((size_t)M));
-        RAPID_CUDA(cudaMemcpyAsync(fd->j_ids.p, joiner_ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    fd->last_ms = 0.f;
+    if (ni > 0) {
+        RAPID_CUDA(cudaEventRecord(fd->ev0, s));
+        RAPID_CHECK(fd->j_ids.reserve((size_t)ni)); RAPID_CHECK(fd->j_key.reserve((size_t)M)); RAPID_CHECK(fd->j_skey.reserve((size_t)M));
+        if (nj) RAPID_CUDA(cudaMemcpyAsync(fd->j_ids.p, joiner_ids, (size_t)nj * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        if (nl) RAPID_CUDA(cudaMemcpyAsync(fd->j_ids.p + nj, leaver_ids, (size_t)nl * sizeof(int32_t), cudaMemcpyHostToDevice, s));
         k_fd_begin<<<1, 1, 0, s>>>(fd->sc.p);
         int mb = 1;                                                              // candidates are < 2^mb
         while ((1LL << mb) < M) ++mb;
-        k_fd_join_keys<<<grid_for(M), TB, 0, s>>>(M, (int32_t)nf, K, mb, fd->a_obs.p, fd->j_ids.p, v->obs.p, fd->tick_flags, fd->j_key.p, fd->sc.p);
+        k_fd_merge_keys<<<grid_for(M), TB, 0, s>>>(M, (int32_t)nf, K, nj, mb, fd->a_obs.p, fd->j_ids.p, v->obs.p, fd->tick_flags, fd->j_key.p, fd->sc.p);
         RAPID_KERNEL_CHECK();
         int ob = 1;                                                              // senders are member ids < 2^ob
         while ((1LL << ob) <= fd->n) ++ob;
         RAPID_CHECK(radix_sort_pairs<uint64_t>(fd->rs, fd->j_key.p, nullptr, fd->j_skey.p, nullptr, M, 0, mb + ob, s, true));
         RAPID_CHECK(fd_read_scal(fd));
-        const int32_t nv = fd->h_sc.p->n_fired;                                 // kept: the tick's alerts + the join alerts
+        const int32_t nv = fd->h_sc.p->n_fired;                                 // kept: the tick's alerts + the merged ones
         if (nv > nf) {
             const size_t F = (size_t)nv, C = F * K;
             RAPID_CHECK(fd->cnt.reserve(F)); RAPID_CHECK(fd->pos.reserve(F)); RAPID_CHECK(fd->m_mask.reserve(F));
             RAPID_CHECK(fd->m_obs.reserve(F)); RAPID_CHECK(fd->m_subj.reserve(F));
             RAPID_CHECK(fd->m_src.reserve(C)); RAPID_CHECK(fd->m_dst.reserve(C)); RAPID_CHECK(fd->m_ring.reserve(C));
             RAPID_CHECK(fd->m_status.reserve(C)); RAPID_CHECK(fd->m_cfg.reserve(C));
-            k_fd_join_count<<<grid_for(nv), TB, 0, s>>>(nv, (int32_t)nf, K, mb, fd->j_skey.p, fd->a_mask.p, fd->j_ids.p, v->obs.p, fd->m_mask.p, fd->cnt.p);
+            k_fd_merge_count<<<grid_for(nv), TB, 0, s>>>(nv, (int32_t)nf, K, mb, fd->j_skey.p, fd->a_mask.p, fd->j_ids.p, v->obs.p, fd->m_mask.p, fd->cnt.p);
             RAPID_KERNEL_CHECK();
             RAPID_CHECK(exclusive_scan_i32_to(fd->cnt.p, fd->pos.p, nv, fd->scan_sums, s));
             // the merged interval is written beside the tick's (it reads them), then takes their place
-            k_fd_join_emit<<<grid_for(nv), TB, 0, s>>>(nv, (int32_t)nf, K, mb, fd->j_skey.p, fd->a_subj.p, fd->j_ids.p, fd->m_mask.p, fd->cnt.p, fd->pos.p,
-                                                      fd->tick_cfg, cfg_id, fd->m_obs.p, fd->m_subj.p, fd->m_src.p, fd->m_dst.p,
-                                                      fd->m_ring.p, fd->m_status.p, fd->m_cfg.p, fd->sc.p);
+            k_fd_merge_emit<<<grid_for(nv), TB, 0, s>>>(nv, (int32_t)nf, K, nj, mb, fd->j_skey.p, fd->a_subj.p, fd->j_ids.p, fd->m_mask.p, fd->cnt.p,
+                                                       fd->pos.p, fd->tick_cfg, cfg_id, fd->m_obs.p, fd->m_subj.p, fd->m_src.p, fd->m_dst.p,
+                                                       fd->m_ring.p, fd->m_status.p, fd->m_cfg.p, fd->sc.p);
             RAPID_KERNEL_CHECK();
             RAPID_CHECK(fd_read_scal(fd));
             swap_buf(fd->a_obs, fd->m_obs); swap_buf(fd->a_subj, fd->m_subj); swap_buf(fd->a_mask, fd->m_mask);
@@ -407,11 +421,18 @@ int32_t rapid_fdet_join_alerts(rapid_fdet* h, const int32_t* joiner_ids, int64_t
             swap_buf(fd->c_status, fd->m_status); swap_buf(fd->c_cfg, fd->m_cfg);
             fd->n_alerts = nv; fd->n_cells = fd->h_sc.p->n_cells;
         }
+        RAPID_CUDA(cudaEventRecord(fd->ev1, s));
+        RAPID_CUDA(cudaEventSynchronize(fd->ev1));
+        RAPID_CUDA(cudaEventElapsedTime(&fd->last_ms, fd->ev0, fd->ev1));
     }
-    fd->joined = true;
+    fd->merged = true;
     if (n_alerts) *n_alerts = fd->n_alerts;
     if (n_cells) *n_cells = fd->n_cells;
     return RAPID_OK;
+}
+
+int32_t rapid_fdet_join_alerts(rapid_fdet* h, const int32_t* joiner_ids, int64_t n, int64_t cfg_id, int64_t* n_alerts, int64_t* n_cells) {
+    return rapid_fdet_merge_alerts(h, joiner_ids, n, nullptr, 0, cfg_id, n_alerts, n_cells);
 }
 
 int32_t rapid_fdet_read_cells(const rapid_fdet* h, int32_t* src, int32_t* dst, uint8_t* ring, uint8_t* status, int64_t* cfg) {

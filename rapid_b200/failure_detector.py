@@ -61,6 +61,18 @@ class EdgeFailureDetectors:
         self.n_alerts, self.n_cells = a.value, c.value
         return a.value, c.value
 
+    def mergeAlerts(self, joiner_ids, leaver_ids, cfg_id):
+        """joinAlerts() and graceful leaves (MembershipService.leave :545-565 -> handleLeaveMessage :372-376) in one merge into the
+        last tick's interval: every live observer k of each listed member raises one DOWN alert with the ring numbers of that edge,
+        repeats kept (K alerts for a leaver whose observers all live).  Per sender: the detectors' alerts, then the join alerts,
+        then the leave alerts, each in list order.  One merge per tick.  -> (number of AlertMessages, number of cells)"""
+        jids, lids = N.as_i32(joiner_ids), N.as_i32(leaver_ids)
+        a, c = C.c_int64(0), C.c_int64(0)
+        N.check(N.lib().rapid_fdet_merge_alerts(self._h, N.ptr(jids), len(jids), N.ptr(lids), len(lids), int(cfg_id), C.byref(a),
+                                                C.byref(c)))
+        self.n_alerts, self.n_cells = a.value, c.value
+        return a.value, c.value
+
     def alerts(self):
         """[(observer, subject, [ring numbers])] of the last tick, in the order the notifiers fired"""
         n = self.n_alerts

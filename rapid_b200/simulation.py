@@ -2,16 +2,21 @@
 (alert generation -> per-sender alert batches -> cut detection -> fast round -> classic fallback -> decideViewChange,
 MembershipService.java:300-354, :385-444, FastPaxos.java:94-203), composed from the classes of this package.
 
-ClusterSimulation rules (tests/simref.py restates them independently; DESIGN.md §4.11):
+ClusterSimulation rules (tests/simref.py restates them independently, tests/simref_leave.py the leave and rejoin rules; DESIGN.md
+§4.11):
 
 * Nodes are named by TAGS: the members given at creation are 0..n-1 in the given order, joiners get the next tags in the
   order addJoiners() lists them.  Tags never change; the device ids of a configuration are dense (view.applyCut renumbers),
   and the driver keeps the id -> tag map.  Scenario flags (failure_detector.CRASHED, INGRESS_BLOCKED, ...) are kept per tag,
   so a view change carries them over; an admitted joiner starts with flags 0.
 * One interval, in this order:
+    0. the members that asked to leave since the last interval (leave()) get the CRASHED flag: they have shut down, so they
+       answer no probe, run no detector, receive nothing, and their acceptors are silent;
     1. one failure-detector interval of every member (EdgeFailureDetectors.tickDevice with the members' flags);
-    2. in the FIRST interval of a configuration only, every pending joiner asks again (joinAlerts, one join attempt per
-       configuration: its live expected observers each send one UP alert);
+    2. one merge into that interval (mergeAlerts): in the FIRST interval of a configuration only, every pending joiner asks
+       again (one join attempt per configuration: its live expected observers each send one UP alert); and every leaver of
+       step 0 sends its LeaveMessages (MembershipService.leave :545-565): each live entry o of getObserversOf(leaver) raises
+       one DOWN alert with getRingNumbers(o, leaver), repeats kept (handleLeaveMessage :372-376);
     3. the interval's alerts, one batch per sender in ascending sender id, reach every receiver (receiver r = ring-0
        position r) through VirtualCluster.handleBatchesDevice: crashed receivers get nothing, batch b reaches receiver r in
        its own cell order seeded interval_seed(seed, cfg, interval) + b;
@@ -28,6 +33,13 @@ ClusterSimulation rules (tests/simref.py restates them independently; DESIGN.md 
   (PaxosAcceptors.findValue, before any Phase2a), its proposal is the cut; view.applyCut; joiners not admitted are
   registered again with their NodeIds; the configuration id comes from the device's identifiersSeen; the detectors are
   reset; the cut detector and the acceptors are created anew for the new membership size.
+* Leave (leave(tags)): every tag must be a current member that is not CRASHED and has not asked to leave already, else
+  ValueError and nothing changes.  A leave is one-shot, as in the reference: if the interval's decision does not include a
+  leaver, it stays a crashed member and the detectors cut it later.  Interval records count the leavers merged ("leavers").
+* Rejoin (rejoin(tag, id_high, id_low)): the endpoint of a departed tag asks to join again with a new NodeId, as the same tag
+  (tags name endpoints).  Refused with ValueError and no change if the tag is still a member (HOSTNAME_ALREADY_IN_RING), is
+  already pending, or if the NodeId was ever given to this simulation (UUID_ALREADY_IN_RING: creation, addJoiners, rejoin).
+  Otherwise the tag becomes a pending joiner under the join rules above, and its flags are cleared on admission.
 * Delivery model (a limit): every receiver gets the senders' batches in the same (ascending sender) order; only the cell
   order within a batch is per receiver.  The reference shuffles batch order per receiver (UnicastToAllBroadcaster.java:59-62).
   Every node sees every vote, so one tally stands for every node's.
@@ -71,7 +83,7 @@ def coordinator(seed, proposer_tags):
 class ClusterSimulation:
     """ClusterSimulation((host_bytes, host_off, ports), (id_high, id_low)): a cluster of the given members on one device.
 
-    setFlags / setEdgeFail / addJoiners describe the scenario; interval() runs one failure-detector interval of the whole
+    setFlags / setEdgeFail / addJoiners / leave / rejoin describe the scenario; interval() runs one failure-detector interval of the whole
     cluster; run() runs intervals until the membership has converged or the run stalls.  history holds one record per
     configuration, intervals one per interval."""
 
@@ -85,6 +97,11 @@ class ClusterSimulation:
         self.view = MembershipView.from_packed(self.K, hb, off, ports, device=device)
         self.view.setNodeIds(*node_ids)
         n = len(ports)
+        # creation endpoints per tag, so that a departed member can register its hostname and port again (rejoin)
+        self._hb, self._off, self._ports = (np.array(a, copy=True) for a in (hb, off, ports))
+        self._seen_hi, self._seen_lo, self._n_seen = np.zeros(0, np.int64), np.zeros(0, np.int64), 0
+        self._add_seen(node_ids[0], node_ids[1])                  # every NodeId this simulation was given, as arrays
+        self.leaving = []                                         # tags that leave in the next interval, in call order
         self.tags = np.arange(n, dtype=np.int64)                  # device id -> tag
         self.flags = np.zeros(n, np.uint8)                        # per tag
         self.edge_fail = {}                                       # (tag, k) -> probes of that tag's k-th detector fail
@@ -117,17 +134,67 @@ class ClusterSimulation:
         tags = list(range(first, first + len(ports)))
         for i, t in enumerate(tags):
             self.joiners[t] = (hostnames[i], int(ports[i]), int(id_high[i]), int(id_low[i]))
+        self._add_seen(id_high, id_low)
         self.flags = np.concatenate([self.flags, np.zeros(len(tags), np.uint8)])
         self._register(tags)
         self.pending += tags
         return tags
+
+    def leave(self, tags):
+        """Cluster.leaveGracefully of each tag: in the next interval the tags shut down (CRASHED) and their observers raise
+        the leave alerts in that interval's merge"""
+        tags = [int(t) for t in tags]
+        member = np.zeros(len(self.flags), bool)
+        member[self.tags] = True
+        asked = set(self.leaving)
+        for t in tags:
+            if not 0 <= t < len(self.flags) or not member[t]:
+                raise ValueError("tag %d is not a member" % t)
+            if self.flags[t] & CRASHED:
+                raise ValueError("tag %d has crashed" % t)
+            if t in asked:
+                raise ValueError("tag %d is leaving already" % t)
+            asked.add(t)
+        self.leaving += tags
+
+    def rejoin(self, tag, id_high, id_low):
+        """the endpoint of departed tag asks to join again with NodeId (id_high, id_low), from the next configuration's first
+        interval on (the current one if it has not run an interval yet)"""
+        t, hi, lo = int(tag), int(id_high), int(id_low)
+        if not 0 <= t < len(self.flags):
+            raise ValueError("tag %d names no endpoint of this simulation" % t)
+        if (self.tags == t).any():
+            raise ValueError("tag %d is a member (HOSTNAME_ALREADY_IN_RING)" % t)
+        if t in self.pending:
+            raise ValueError("tag %d is already asking to join" % t)
+        k = self._n_seen
+        if ((self._seen_hi[:k] == hi) & (self._seen_lo[:k] == lo)).any():
+            raise ValueError("NodeId of tag %d was seen before (UUID_ALREADY_IN_RING)" % t)
+        if t in self.joiners:
+            host, port = self.joiners[t][:2]
+        else:
+            host, port = self._hb[self._off[t]: self._off[t + 1]].tobytes(), int(self._ports[t])
+        self.joiners[t] = (host, port, hi, lo)
+        self._add_seen([hi], [lo])
+        self._register([t])
+        self.pending.append(t)
 
     def members(self):
         """tags of the current members, in device id order"""
         return self.tags.tolist()
 
     def converged(self):
-        return not self.flags[self.tags].any() and not self.pending
+        return not self.flags[self.tags].any() and not self.pending and not self.leaving
+
+    def _add_seen(self, id_high, id_low):
+        hi, lo = np.asarray(id_high, np.int64), np.asarray(id_low, np.int64)
+        k, m = self._n_seen, len(hi)
+        if k + m > len(self._seen_hi):                            # doubling: a rejoin appends one id
+            cap = max(2 * len(self._seen_hi), k + m, 16)
+            self._seen_hi = np.concatenate([self._seen_hi[:k], np.zeros(cap - k, np.int64)])
+            self._seen_lo = np.concatenate([self._seen_lo[:k], np.zeros(cap - k, np.int64)])
+        self._seen_hi[k: k + m], self._seen_lo[k: k + m] = hi, lo
+        self._n_seen = k + m
 
     # ---- handles of one configuration ------------------------------------------------------------------------------------------
     def _register(self, tags):
@@ -178,14 +245,20 @@ class ClusterSimulation:
         quiet / alerts / proposals / decided-fast / decided-classic (the view has changed) / stalled"""
         t0 = time.perf_counter()
         self._ann = None
+        leavers, self.leaving = self.leaving, []
+        if leavers:
+            self.flags[leavers] = CRASHED                         # shut down: silent from this interval on
+            self._dirty = True
         if self._dirty:
             self._upload_flags()
         i, cfg = self.interval_in_cfg, self.cfg
         na, nc = self.fd.tickDevice(self.d_flags.data_ptr(), cfg, 0 if self.d_edge is None else self.d_edge.data_ptr())
         dev_ms = self.fd.lastDeviceMs()
-        if i == 0 and self.pending:
-            na, nc = self.fd.joinAlerts([self.joiner_id[t] for t in self.pending], cfg)
-        rec = {"cfg": cfg, "interval": i, "alerts": na, "cells": nc, "announced": 0, "event": "quiet"}
+        joiners = [self.joiner_id[t] for t in self.pending] if i == 0 else []
+        if joiners or leavers:
+            na, nc = self.fd.mergeAlerts(joiners, self._member_ids(leavers), cfg)
+            dev_ms += self.fd.lastDeviceMs()
+        rec = {"cfg": cfg, "interval": i, "alerts": na, "cells": nc, "announced": 0, "event": "quiet", "leavers": len(leavers)}
         decided = None
         if nc:
             rec["event"] = "alerts"
@@ -225,6 +298,14 @@ class ClusterSimulation:
             self._view_change(decided[0], decided[1], i)
         self.intervals.append(rec)
         return rec
+
+    def _member_ids(self, tags):
+        """device ids of member tags"""
+        if not tags:
+            return []
+        inv = np.full(len(self.flags), -1, np.int64)
+        inv[self.tags] = np.arange(len(self.tags))
+        return inv[np.asarray(tags, np.int64)]
 
     def _classic_round(self, cfg, i):
         """Paxos.java round 2 from the seeded coordinator over the acceptors -> (decided value or None, device ms)"""
@@ -304,7 +385,7 @@ class ClusterSimulation:
             if rec["event"] == "stalled":
                 break
         done = self.converged()
-        stuck = sorted(set(int(t) for t in self.tags[self.flags[self.tags] != 0]) | set(self.pending))
+        stuck = sorted(set(int(t) for t in self.tags[self.flags[self.tags] != 0]) | set(self.pending) | set(self.leaving))
         return {"converged": done, "stalled": not done, "intervals": total, "stuck": stuck,
                 "wall_ms": (time.perf_counter() - t0) * 1e3}
 
