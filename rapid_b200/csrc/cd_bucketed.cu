@@ -3,9 +3,9 @@
 // Reference semantics: MultiNodeCutDetector.java:84-128 applied per cell in arrival order, then :137-164, driven
 // by MembershipService.java:300-354.  The Java walks the batch once per process and probes a hash map per cell.
 // Here the batch is regrouped BY SUBJECT once (counting sort by subject slot inside cd_prepare.cu), and every receiver's
-// 16-bit ring mask for a subject is read ONCE, updated in a register and written ONCE:
+// state word for a subject (12 bits at K <= 10, see RowRef) is read ONCE, updated in a register and written ONCE:
 //
-//   traffic = 4 bytes x (#subjects in the batch) x (#receivers)          (SURVEY.md §8d "4·S·R")
+//   traffic = 3 bytes x (#subjects in the batch) x (#receivers)          (SURVEY.md §8d "4·S·R" with 16-bit words)
 //
 // instead of 4 bytes x #cells x #receivers for a per-cell sweep.  What makes that legal is that the sequential
 // rule "emit when updatesInProgress returns to 0" only depends on, per subject, the two moments at which its
@@ -23,7 +23,7 @@
 //
 // A batch is a fixed chain of launches with no host round trip between them (cd_prepare.cu's k_prepare, then the kernels below); the
 // host learns the outcome from a snapshot of the device counters at its next synchronisation point:
-//   k_apply_uniform<PERM, SEQ>  SWAR, 8 receivers per thread, 128-bit loads/stores, write-only fresh-subject path, per-block memo +
+//   k_apply_uniform<PERM, SEQ, HB>  SWAR, 8 receivers per thread, lo + hi plane group loads/stores, write-only fresh-subject path, per-block memo +
 //                          L2 prefetch on the read-modify-write path.  PERM = every receiver gets every cell but in its OWN order
 //                          (RAPID_DELIVERY_PERMUTED): the new state and all the crossing COUNTS do not depend on the order, so the
 //                          kernel is the uniform one minus the moments; the (rare) receivers whose classification needs their own
@@ -106,7 +106,7 @@ struct ChunkAcc {                     // what the FRESH subjects of a chunk cont
 };
 
 // Partials::cnt.z holds touched_pre in its low 30 bits and the PF_* flags above them: a chunk holds fewer than 2^30 subjects
-// (the slot count is bounded far below that by the mask rows, 4 * Rpad bytes per slot)
+// (the slot count is bounded far below that by the state rows, at least 3 * Rpad bytes per slot)
 constexpr int PF_SHIFT = 30;
 constexpr uint32_t TP_MASK = (1u << PF_SHIFT) - 1u;
 
@@ -317,8 +317,7 @@ __device__ __forceinline__ uint32_t observer_L_batch(uint32_t uo, const SubjDesc
 }
 
 struct ApplyArgs {
-    uint16_t* masks;
-    const uint8_t* cur;
+    RowRef rows;                  // the double-buffered state rows (rows.cur: which of a slot's two rows is current)
     size_t Rpad;
     int K, H, L;
     int64_t R, rbegin;
@@ -346,7 +345,8 @@ struct ApplyArgs {
 __device__ __forceinline__ void note_unresolved(const ApplyArgs& a, int tile, int32_t slot) { worklist_note(a.wl, tile, slot); }
 
 // ---- uniform delivery: every active receiver gets every valid cell in array order -------------------------------------
-// One thread owns 8 consecutive receivers (one 128-bit load + one 128-bit store per subject).  The common case is
+// One thread owns 8 consecutive receivers: per subject one group load and one group store (RowRef: 64-bit lo plane + 32-bit hi
+// plane at HB = 4, so a warp writes one whole 256-byte and one whole 128-byte line).  The common case is
 // that all of a thread's ACTIVE receivers hold the same state for the subject (they saw the same history): the
 // visit is computed once, merged into the new word with a SWAR mask, and accumulated in registers ("com").  Only
 // when active neighbours disagree (partitions) do we fall back to a per-receiver visit whose accumulators live in
@@ -467,9 +467,9 @@ __device__ __forceinline__ uint32_t receiver_down_batch(const ApplyArgs& a, uint
     return sd == INT_MAX ? T32_NONE : (uint32_t)sd;
 }
 // pre-call row of a slot: before the flip it is the current one; after the flip the other one — for the slots the call touched
-__device__ __forceinline__ const uint16_t* precall_row(const ApplyArgs& a, int32_t slot, bool post_flip) {
+__device__ __forceinline__ const uint8_t* precall_row(const ApplyArgs& a, int32_t slot, bool post_flip) {
     const int flipped = post_flip && a.touch[slot] == a.serial ? 1 : 0;
-    return a.masks + ((size_t)slot * 2 + (a.cur[slot] ^ flipped)) * a.Rpad;
+    return a.rows.lo(slot, a.rows.cur[slot] ^ flipped);
 }
 // generic (one receiver, scalar loads): u[k] for every ring of `slot` whose observer is a subject itself; returns the ring mask
 __device__ __noinline__ uint32_t edge_times(const ApplyArgs& a, int32_t slot, int64_t r, bool post_flip, uint32_t bDown, uint32_t* u) {
@@ -482,7 +482,7 @@ __device__ __noinline__ uint32_t edge_times(const ApplyArgs& a, int32_t slot, in
         if (so < 0) continue;
         const bool ot = a.touch[so] == a.serial;
         const int bo = ot ? a.batch_index[so] : 0;
-        const uint32_t uo = so >= S_before ? 0u : (precall_row(a, so, post_flip)[r] & RM);
+        const uint32_t uo = so >= S_before ? 0u : (a.rows.get(precall_row(a, so, post_flip), r) & RM);
         const uint32_t bLo = observer_L_batch(uo, ot ? &a.desc[bo] : nullptr, ot ? &a.pwalk[bo] : nullptr, a.L);
         u[k] = (bLo == T32_NONE || bDown == T32_NONE) ? T32_NONE : max(bLo, bDown);
         umask |= 1u << k;
@@ -499,28 +499,29 @@ __device__ __forceinline__ uint32_t seq_state(const ApplyArgs& a, const SubjDesc
     return prefix_core(nullptr, old, d, a.pwalk[b_index], u, umask, a.L, a.H, (uint32_t)a.bc->seq_last);
 }
 
-template <bool PERM, bool SEQ>
+template <bool PERM, bool SEQ, int HB>
 __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_uniform(const ApplyArgs a) {
     __shared__ SubjDesc sd[STAGE];
     __shared__ SubjWalk sw[PERM ? 1 : STAGE];
     __shared__ SubjWalk spw[SEQ ? STAGE : 1];
-    __shared__ const uint16_t* s_src[STAGE];
-    __shared__ uint16_t* s_dst[STAGE];
-    __shared__ uint32_t s_nw[STAGE];          // (rings reported by the call) replicated in both half-words
+    __shared__ const uint8_t* s_src[STAGE];   // lo planes of the current / the other row
+    __shared__ uint8_t* s_dst[STAGE];
+    __shared__ uint32_t s_nw[STAGE];          // rings reported by the call
+    __shared__ uint2 s_nrep[STAGE];           // ... replicated over the lanes (group8_rep)
     __shared__ int s_unres[STAGE];
     __shared__ ChunkAcc s_facc;               // fresh-subject accumulators of this block's chunk (same for every receiver)
     __shared__ int s_heavy;                   // staged subjects that are NOT plain fresh ones (carried, or with dictionary observers)
     // SEQ: the dictionary observers ("edges") of the staged subjects — their pre-call rows (nullptr: fresh, state 0) and batch index
     __shared__ uint8_t s_ne[SEQ ? STAGE : 1];
     __shared__ uint8_t s_ek[SEQ ? STAGE : 1][MAXK];
-    __shared__ const uint16_t* s_erow[SEQ ? STAGE : 1][MAXK];
+    __shared__ const uint8_t* s_erow[SEQ ? STAGE : 1][MAXK];
     __shared__ int32_t s_eob[SEQ ? STAGE : 1][MAXK];
     // Memo of the carried subjects (RAPID_MEMO): receivers of a tile have almost always seen the same history, so warp 0 computes
     // the visit ONCE per (block, subject) for the state the tile's first active receiver holds; a thread whose active receivers
     // all hold exactly that state only merges the precomputed new word, and takes the stage's summed contribution at the end of the
     // stage.  (The visit itself — the walk over the first-occurrence rings — was what kept the read-modify-write path issue-bound.)
     __shared__ uint32_t s_mst[STAGE];         // the sample state (0xFFFFFFFF: no memo for this subject)
-    __shared__ uint32_t s_mnw[STAGE];         // the new word for that state, replicated in both half-words
+    __shared__ uint2 s_mrep[STAGE];           // the new word for that state, replicated over the lanes
     __shared__ uint8_t s_mun[STAGE];          // the subject stays in the unstable band for that state
     __shared__ StageAcc s_macc[STAGE];        // what one such (subject, receiver) visit contributes
     __shared__ StageAcc s_msum;               // ... summed over the stage's memo subjects
@@ -551,10 +552,8 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
             if (SEQ && (rf & RF_SEEN_DOWN)) seen |= 1u << j;
         }
     }
-    // SWAR masks: 0xFFFF per active half-word
-    uint32_t am[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) am[q] = (((act >> (2 * q)) & 1u) ? 0x0000FFFFu : 0u) | (((act >> (2 * q + 1)) & 1u) ? 0xFFFF0000u : 0u);
+    const Group8<HB> am = group8_mask<HB>(act);     // SWAR masks: all-ones lanes of the active receivers
+    const RowRef& rows = a.rows;
     if (t == 0) s_facc = chunk_zero();
     if (MEMO) {                                     // the tile's first active receiver
         const int mine = act ? t * 8 + __ffs(act) - 1 : INT_MAX;
@@ -584,11 +583,12 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
             if (t < n) {
                 const SubjDesc d = a.desc[base + t];
                 sd[t] = d;
-                const uint8_t c = a.cur[d.slot];
+                const uint8_t c = rows.cur[d.slot];
                 const bool fresh = d.slot >= S_before;
-                s_src[t] = fresh ? nullptr : a.masks + ((size_t)d.slot * 2 + c) * a.Rpad;
-                s_dst[t] = a.masks + ((size_t)d.slot * 2 + (c ^ 1)) * a.Rpad;
-                s_nw[t] = (uint32_t)(d.bmask | d.pmask) * 0x10001u;
+                s_src[t] = fresh ? nullptr : rows.lo(d.slot, c);
+                s_dst[t] = rows.lo(d.slot, c ^ 1);
+                s_nw[t] = (uint32_t)(d.bmask | d.pmask);
+                s_nrep[t] = group8_rep<HB>(d.bmask | d.pmask);
                 int un = 0;
                 const bool edges = SEQ && a.wl.has_so[d.slot];   // implicit reports inside the prefix: per-receiver state matters
                 if (SEQ) {
@@ -598,7 +598,7 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
                             const int32_t so = a.wl.so_tab[(size_t)d.slot * SO_STRIDE + k];
                             if (so < 0) continue;
                             s_ek[t][ne] = (uint8_t)k;
-                            s_erow[t][ne] = so >= S_before ? nullptr : a.masks + ((size_t)so * 2 + a.cur[so]) * a.Rpad;
+                            s_erow[t][ne] = so >= S_before ? nullptr : rows.cur_lo(so);
                             s_eob[t][ne] = a.touch[so] == a.serial ? a.batch_index[so] : -1;
                             ++ne;
                         }
@@ -614,11 +614,11 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
                     if (SEQ) spw[t] = a.pwalk[base + t];
                     if (fresh) s_src[t] = nullptr;
                     if (MEMO && !fresh && !edges && block_active) {
-                        const uint32_t sst = s_src[t][sample_at];
+                        const uint32_t sst = rows.get(s_src[t], (int64_t)sample_at);
                         uint32_t at_last = sst;
                         const bool mun = visit_acc<PERM, SEQ>(m, sst & RM, d, &sw[PERM ? 0 : t], &spw[SEQ ? t : 0], RM, L, H, nullptr, 0u, seq_last, &at_last);
                         s_mst[t] = sst;
-                        s_mnw[t] = (SEQ ? (at_last | (sst & ~RM)) : sst) * 0x10001u | s_nw[t];
+                        s_mrep[t] = group8_rep<HB>((SEQ ? (at_last | (sst & ~RM)) : sst) | s_nw[t]);
                         s_mun[t] = mun ? 1 : 0;
                         memo = true;
                     }
@@ -649,59 +649,60 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
         __syncthreads();
         uint32_t hit = 0;                                  // staged subjects for which this thread took the memo
 #if RAPID_PF > 0
-        // The read-modify-write path has ONE 128-bit load in flight per thread (the loop body branches on the loaded word), i.e.
-        // 10 KB per SM at 5 blocks x 128 threads — well below what the HBM latency-bandwidth product needs.  The rows of the
-        // next RAPID_PF staged subjects are therefore pulled into L2 ahead of their loads.
+        // The read-modify-write path has ONE group load (both planes) in flight per thread (the loop body branches on the loaded
+        // words), far below what the HBM latency-bandwidth product needs.  The rows of the next RAPID_PF staged subjects are
+        // therefore pulled into L2 ahead of their loads.
         const bool pf_on = !SEQ && s_heavy != 0;          // (the sequence kernels keep their measured code: no memo, no prefetch)
         if (pf_on) {
 #pragma unroll
             for (int j = 0; j < RAPID_PF; ++j)
-                if (j < n && s_src[j]) asm volatile(RAPID_PF_ASM ::"l"(s_src[j] + r0));
+                if (j < n && s_src[j]) {
+                    asm volatile(RAPID_PF_ASM ::"l"(s_src[j] + r0));
+                    asm volatile(RAPID_PF_ASM ::"l"(group8_hi<HB>(rows, s_src[j], r0)));
+                }
         }
 #endif
 #if RAPID_SPLIT_LOOP
         // fresh subjects of the stage first: write-only, in a loop of their own
 #pragma unroll 4
         for (int i = 0; i < n; ++i) {
-            const uint32_t nwb = s_nw[i];
-            if (s_src[i] == nullptr && (!SEQ || s_ne[i] == 0))
-                *reinterpret_cast<uint4*>(s_dst[i] + r0) = make_uint4(nwb & am[0], nwb & am[1], nwb & am[2], nwb & am[3]);
+            if (s_src[i] == nullptr && (!SEQ || s_ne[i] == 0)) group8_store<HB>(rows, s_dst[i], r0, group8_fill<HB>(s_nrep[i], am));
         }
         const int n_heavy = s_heavy ? n : 0;               // (uniform) nothing but plain fresh subjects in this stage: skip the visit loop
         for (int i = 0; i < n_heavy; ++i) {
-            const uint16_t* src = s_src[i];
-            uint16_t* dst = s_dst[i];
-            const uint32_t nwb = s_nw[i];
+            const uint8_t* src = s_src[i];
+            uint8_t* dst = s_dst[i];
             const int ne = SEQ ? (int)s_ne[i] : 0;
             if (src == nullptr && ne == 0) continue;       // (done above)
 #else
 #pragma unroll 4
         for (int i = 0; i < n; ++i) {
-            const uint16_t* src = s_src[i];
-            uint16_t* dst = s_dst[i];
-            const uint32_t nwb = s_nw[i];
+            const uint8_t* src = s_src[i];
+            uint8_t* dst = s_dst[i];
             const int ne = SEQ ? (int)s_ne[i] : 0;
 #if RAPID_PF > 0
             if (pf_on && i + RAPID_PF < n) {
-                const uint16_t* nx = s_src[i + RAPID_PF];
-                if (nx) asm volatile(RAPID_PF_ASM ::"l"(nx + r0));
+                const uint8_t* nx = s_src[i + RAPID_PF];
+                if (nx) {
+                    asm volatile(RAPID_PF_ASM ::"l"(nx + r0));
+                    asm volatile(RAPID_PF_ASM ::"l"(group8_hi<HB>(rows, nx, r0)));
+                }
             }
 #endif
-            if (src == nullptr && ne == 0) {               // fresh subject: write-only
-                *reinterpret_cast<uint4*>(dst + r0) = make_uint4(nwb & am[0], nwb & am[1], nwb & am[2], nwb & am[3]);
+            if (src == nullptr && ne == 0) {               // fresh subject: write-only, full width (zeros for inactive receivers)
+                group8_store<HB>(rows, dst, r0, group8_fill<HB>(s_nrep[i], am));
                 continue;
             }
 #endif
-            uint4 w = src ? *reinterpret_cast<const uint4*>(src + r0) : make_uint4(0u, 0u, 0u, 0u);
+            Group8<HB> w;
+            if (src) w = group8_load<HB>(rows, src, r0);
+            else { w.lo = 0; w.hi = 0; }
             bool unres = false;
             if (act) {
                 const SubjDesc& d = sd[i];
-                // all active half-words equal  <=>  AND over them == OR over them
-                const uint32_t andw = (w.x | ~am[0]) & (w.y | ~am[1]) & (w.z | ~am[2]) & (w.w | ~am[3]);
-                const uint32_t orw = (w.x & am[0]) | (w.y & am[1]) | (w.z & am[2]) | (w.w & am[3]);
-                const uint32_t andv = andw & (andw >> 16) & 0xFFFFu, st = (orw | (orw >> 16)) & 0xFFFFu;
+                uint32_t st;
+                bool same = group8_same<HB>(w, am, &st);     // all active receivers hold the same word
                 carried = true;
-                bool same = andv == st;
                 const bool mhit = MEMO && same && st == s_mst[i];   // (subjects with edges have no memo)
                 // SEQ, subject with dictionary observers: their state (and seenLinkDownEvents) must be the same across the thread's
                 // active receivers too, or every receiver is visited on its own
@@ -713,13 +714,7 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
                     const uint32_t bDown = sact ? 0u : (a.bc->seq_down == INT_MAX ? T32_NONE : (uint32_t)a.bc->seq_down);
                     for (int e = 0; e < ne && same; ++e) {
                         uint32_t so_st = 0;
-                        if (s_erow[i][e]) {
-                            const uint4 wo = *reinterpret_cast<const uint4*>(s_erow[i][e] + r0);
-                            const uint32_t aw = (wo.x | ~am[0]) & (wo.y | ~am[1]) & (wo.z | ~am[2]) & (wo.w | ~am[3]);
-                            const uint32_t ow = (wo.x & am[0]) | (wo.y & am[1]) | (wo.z & am[2]) | (wo.w & am[3]);
-                            so_st = (ow | (ow >> 16)) & 0xFFFFu;
-                            same = (aw & (aw >> 16) & 0xFFFFu) == so_st;
-                        }
+                        if (s_erow[i][e]) same = group8_same<HB>(group8_load<HB>(rows, s_erow[i][e], r0), am, &so_st);
                         const int ob = s_eob[i][e], k = s_ek[i][e];
                         const uint32_t bLo = observer_L_batch(so_st & RM, ob >= 0 ? &a.desc[ob] : nullptr, ob >= 0 ? &a.pwalk[ob] : nullptr, L);
                         u[k] = (bLo == T32_NONE || bDown == T32_NONE) ? T32_NONE : max(bLo, bDown);
@@ -729,19 +724,11 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
                 if (mhit) {                                // the tile's common state: everything is precomputed
                     hit |= 1u << i;
                     unres = s_mun[i] != 0;
-                    const uint32_t nw = s_mnw[i];
-                    w.x = (w.x & ~am[0]) | (nw & am[0]);
-                    w.y = (w.y & ~am[1]) | (nw & am[1]);
-                    w.z = (w.z & ~am[2]) | (nw & am[2]);
-                    w.w = (w.w & ~am[3]) | (nw & am[3]);
+                    group8_merge<HB>(w, s_mrep[i], am);
                 } else if (same) {
                     uint32_t at_last = st;
                     unres = visit_acc<PERM, SEQ>(com, st & RM, d, &sw[PERM ? 0 : i], &spw[SEQ ? i : 0], RM, L, H, u, umask, seq_last, &at_last);
-                    const uint32_t nw = (SEQ ? (at_last | (st & ~RM)) : st) * 0x10001u | nwb;
-                    w.x = (w.x & ~am[0]) | (nw & am[0]);
-                    w.y = (w.y & ~am[1]) | (nw & am[1]);
-                    w.z = (w.z & ~am[2]) | (nw & am[2]);
-                    w.w = (w.w & ~am[3]) | (nw & am[3]);
+                    group8_merge<HB>(w, group8_rep<HB>((SEQ ? (at_last | (st & ~RM)) : st) | s_nw[i]), am);
                 } else {
                     if (!had_exc) {
                         had_exc = true;
@@ -749,22 +736,22 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
 #pragma unroll
                         for (int j = 0; j < 8; ++j) part_store<SEQ>(a.part, pbase + j, zero);
                     }
-                    uint32_t words[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
+                    const uint32_t nwb = s_nw[i];
+                    // (the sequence kernels keep this rare per-receiver path rolled: unrolled, it spills their hot loop)
+#pragma unroll (SEQ ? 1 : 8)
                     for (int j = 0; j < 8; ++j) {
                         if (!((act >> j) & 1u)) continue;
-                        const uint32_t sj = (words[j >> 1] >> ((j & 1) * 16)) & 0xFFFFu;
+                        const uint32_t sj = group8_word<HB>(w, j);
                         Acc ex;
                         uint32_t at_last = sj;
                         if (SEQ && ne) umask = edge_times(a, d.slot, r0 + j, false, receiver_down_batch(a, ((seen >> j) & 1u) ? RF_SEEN_DOWN : 0u, false), u);
                         unres |= visit_acc<PERM, SEQ>(ex, sj & RM, d, &sw[PERM ? 0 : i], &spw[SEQ ? i : 0], RM, L, H, u, umask, seq_last, &at_last);
                         part_merge<SEQ>(a.part, pbase + j, ex);
-                        words[j >> 1] |= ((SEQ ? (at_last & RM) : 0u) | (nwb & 0xFFFFu)) << ((j & 1) * 16);
+                        group8_or_word<HB>(w, j, (SEQ ? (at_last & RM) : 0u) | nwb);
                     }
-                    w = make_uint4(words[0], words[1], words[2], words[3]);
                 }
             }
-            *reinterpret_cast<uint4*>(dst + r0) = w;       // the non-current row becomes the new state
+            group8_store<HB>(rows, dst, r0, w);            // the non-current row becomes the new state
             if (__any_sync(0xffffffffu, unres) && (t & 31) == 0 && s_unres[i] == 0) s_unres[i] = 1;
         }
         if (MEMO && hit) {                           // the memo subjects this thread met: usually all of the stage's
@@ -892,8 +879,8 @@ __device__ __forceinline__ GVisit visit_generic(uint32_t ur, const SubjDesc& d, 
 
 __global__ void __launch_bounds__(GEN_THREADS, 4) k_apply_generic(const ApplyArgs a) {
     __shared__ SubjDesc sd[STAGE];
-    __shared__ const uint16_t* s_src[STAGE];
-    __shared__ uint16_t* s_dst[STAGE];
+    __shared__ const uint8_t* s_src[STAGE];
+    __shared__ uint8_t* s_dst[STAGE];
     __shared__ int s_unres[STAGE];
     if (a.bc->overflow) return;               // the batch was rolled back by k_prepare
     const int Sb = a.bc->n_batch_subj, S_before = a.bc->S_before;
@@ -916,9 +903,9 @@ __global__ void __launch_bounds__(GEN_THREADS, 4) k_apply_generic(const ApplyArg
         if (t < n) {
             const SubjDesc d = a.desc[base + t];
             sd[t] = d;
-            const uint8_t c = a.cur[d.slot];
-            s_src[t] = d.slot >= S_before ? nullptr : a.masks + ((size_t)d.slot * 2 + c) * a.Rpad;
-            s_dst[t] = a.masks + ((size_t)d.slot * 2 + (c ^ 1)) * a.Rpad;
+            const uint8_t c = a.rows.cur[d.slot];
+            s_src[t] = d.slot >= S_before ? nullptr : a.rows.lo(d.slot, c);
+            s_dst[t] = a.rows.lo(d.slot, c ^ 1);
             s_unres[t] = a.wl.has_so[d.slot] ? 0 : -1;          // -1: no observer in the dictionary, never on the work list
         }
         __syncthreads();
@@ -927,7 +914,7 @@ __global__ void __launch_bounds__(GEN_THREADS, 4) k_apply_generic(const ApplyArg
         for (int i = 0; i < n; ++i) {
             if ((i & 7) == 0) {
 #pragma unroll
-                for (int u = 0; u < 8; ++u) pre[u] = (i + u < n && s_src[i + u]) ? s_src[i + u][r] : 0u;
+                for (int u = 0; u < 8; ++u) pre[u] = (i + u < n && s_src[i + u]) ? a.rows.get(s_src[i + u], r) : 0u;
             }
             const SubjDesc& d = sd[i];
             bool unres = false;
@@ -950,7 +937,9 @@ __global__ void __launch_bounds__(GEN_THREADS, 4) k_apply_generic(const ApplyArg
                     }
                     st |= v.have;
                 }
-                s_dst[i][r] = (uint16_t)st;
+                // (r < Rpad holds for the whole grid: every lane of the warp takes part in the store)
+                if (a.rows.hb == 4) row_store1_warp<4>(a.rows, s_dst[i], r, st);
+                else row_store1_warp<8>(a.rows, s_dst[i], r, st);
             }
             if (__any_sync(0xffffffffu, unres) && (t & 31) == 0 && s_unres[i] == 0) s_unres[i] = 1;
         }
@@ -1212,7 +1201,7 @@ __device__ __forceinline__ IVisit interval_visit(const ApplyArgs& a, int uniform
 struct PassSmem {
     SubjDesc sd[STAGE];
     SubjWalk sw[STAGE];
-    const uint16_t* s_old[STAGE];
+    const uint8_t* s_old[STAGE];
 };
 
 // MODE 0: FIX pass (next candidate for `a`, e* candidate)   1: SUM pass (fingerprint of {t_H <= e*})
@@ -1248,14 +1237,14 @@ __device__ __noinline__ void mixed_pass(const ResolveArgs& m, PassSmem& sm, cons
                 const SubjDesc d = a.desc[base + t];
                 sm.sd[t] = d;
                 const bool fresh = d.slot >= S_before;
-                sm.s_old[t] = fresh ? nullptr : a.masks + ((size_t)d.slot * 2 + a.cur[d.slot]) * a.Rpad;   // pre-batch row (not flipped yet)
+                sm.s_old[t] = fresh ? nullptr : a.rows.cur_lo(d.slot);   // pre-batch row (not flipped yet)
                 if (!fresh && m.uniform) sm.sw[t] = a.walk[base + t];
             }
             __syncthreads();
             if (!on) continue;
             for (int i = 0; i < n; ++i) {
                 const SubjDesc& d = sm.sd[i];
-                const uint32_t st = seq_state(a, d, base + i, r, (sm.s_old[i] ? sm.s_old[i][r] : 0u) & RM, false, true);   // when the (last) batch starts
+                const uint32_t st = seq_state(a, d, base + i, r, (sm.s_old[i] ? a.rows.get(sm.s_old[i], r) : 0u) & RM, false, true);   // when the (last) batch starts
                 const IVisit v = interval_visit(a, m.uniform, st & RM, d, &sm.sw[i], r, rs);
                 if (MODE == 0) {
                     if (!v.crossH) continue;                                  // never closes, or never in the band
@@ -1344,7 +1333,7 @@ __device__ __noinline__ bool emitted_in_batch(const ResolveArgs& e, int32_t s, i
     if (e.touch[s] != e.serial) return __popc(w_new & RM) >= a.H && !(w_new & CD_BIT_CALL);
     const int b = e.batch_index[s];
     const SubjDesc d = a.desc[b];
-    const uint32_t old = seq_state(a, d, b, r, (s >= a.bc->S_before ? 0u : (a.masks + ((size_t)s * 2 + (a.cur[s] ^ 1)) * a.Rpad)[r]) & RM, true, true);
+    const uint32_t old = seq_state(a, d, b, r, (s >= a.bc->S_before ? 0u : a.rows.get(a.rows.alt_lo(s), r)) & RM, true, true);
     if (__popc(old & RM) >= a.H) return true;                              // pending before the (last) batch
     SubjWalk wl;
     if (e.uniform) wl = a.walk[b];
@@ -1361,10 +1350,10 @@ __device__ __noinline__ bool emitted_in_batch(const ResolveArgs& e, int32_t s, i
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int INV_STAGE = 128;            // work-list subjects staged at a time: one thread each (GEN_THREADS >= INV_STAGE)
 struct InvSmem {
-    uint16_t* row[INV_STAGE];
+    uint8_t* row[INV_STAGE];                        // lo planes of the current rows
     uint64_t mix1[INV_STAGE], mix2[INV_STAGE];
     uint8_t ne[INV_STAGE];                          // edges (observers that are subjects) of staged slot i: entries [i * MAXK, i * MAXK + ne[i])
-    const uint16_t* e_row[INV_STAGE * MAXK];
+    const uint8_t* e_row[INV_STAGE * MAXK];
     int32_t e_so[INV_STAGE * MAXK];
     uint8_t e_k[INV_STAGE * MAXK];
     uint8_t flag[INV_STAGE];
@@ -1425,14 +1414,14 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
                     const int32_t sl = a.wl.slots[base + t];
                     const uint8_t fl = a.wl.in_tile[(size_t)sl * a.wl.n_tiles + tile];
                     sm.flag[t] = fl;
-                    sm.row[t] = a.masks + ((size_t)sl * 2 + a.cur[sl]) * a.Rpad;
+                    sm.row[t] = a.rows.cur_lo(sl);
                     const int32_t subject = a.slot_subject[sl];
                     sm.mix1[t] = fp_mix1(subject); sm.mix2[t] = fp_mix2(subject);
                     int ne = 0;
                     for (int k = 0; k < a.K; ++k) {
                         const int32_t s2 = a.wl.so_tab[(size_t)sl * SO_STRIDE + k];
                         if (s2 < 0) continue;
-                        sm.e_row[t * MAXK + ne] = a.masks + ((size_t)s2 * 2 + a.cur[s2]) * a.Rpad;
+                        sm.e_row[t * MAXK + ne] = a.rows.cur_lo(s2);
                         sm.e_so[t * MAXK + ne] = s2; sm.e_k[t * MAXK + ne] = (uint8_t)k;
                         ++ne;
                     }
@@ -1451,17 +1440,19 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
                         idx[q] = g + q < nd ? (int)sm.dense[g + q] : -1;
                         w2v[q] = make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu); e0v[q] = make_uint2(0u, 0u); e1v[q] = make_uint2(0u, 0u);
                         if (idx[q] < 0) continue;
-                        w2v[q] = *reinterpret_cast<const uint2*>(sm.row[idx[q]] + rb);
+                        w2v[q] = a.rows.load4(sm.row[idx[q]], rb);
                         const int eb = idx[q] * MAXK, ne = sm.ne[idx[q]];
-                        if (ne > 0) e0v[q] = *reinterpret_cast<const uint2*>(sm.e_row[eb] + rb);
-                        if (ne > 1) e1v[q] = *reinterpret_cast<const uint2*>(sm.e_row[eb + 1] + rb);
+                        if (ne > 0) e0v[q] = a.rows.load4(sm.e_row[eb], rb);
+                        if (ne > 1) e1v[q] = a.rows.load4(sm.e_row[eb + 1], rb);
                     }
 #pragma unroll
                     for (int q = 0; q < 4; ++q) {
                         const int i = idx[q];
                         if (i < 0) continue;
                         const int eb = i * MAXK, ee = eb + sm.ne[i];
-                        uint32_t w[4] = {w2v[q].x & 0xFFFFu, w2v[q].x >> 16, w2v[q].y & 0xFFFFu, w2v[q].y >> 16};
+                        uint32_t w[4];
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) w[j] = a.rows.word4(w2v[q], j);
                         uint32_t miss[4];                                   // rings an implicit report could still add, per receiver
                         uint32_t anymiss = 0;
 #pragma unroll
@@ -1475,8 +1466,10 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
                         for (int ei = eb; ei < ee; ++ei) {
                             const int k = sm.e_k[ei];
                             if (!((anymiss >> k) & 1u)) continue;
-                            const uint2 o2 = ei == eb ? e0v[q] : ei == eb + 1 ? e1v[q] : *reinterpret_cast<const uint2*>(sm.e_row[ei] + rb);
-                            const uint32_t wo[4] = {o2.x & 0xFFFFu, o2.x >> 16, o2.y & 0xFFFFu, o2.y >> 16};
+                            const uint2 o2 = ei == eb ? e0v[q] : ei == eb + 1 ? e1v[q] : a.rows.load4(sm.e_row[ei], rb);
+                            uint32_t wo[4];
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) wo[j] = a.rows.word4(o2, j);
 #pragma unroll
                             for (int j = 0; j < 4; ++j) {
                                 if (!((miss[j] >> k) & 1u)) continue;
@@ -1501,7 +1494,7 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
                             w[j] = nw;
                             if (raised) { ++res[j]; kh1[j] += sm.mix1[i]; kh2[j] += sm.mix2[i]; }   // moved preProposal -> proposal
                         }
-                        if (any) *reinterpret_cast<uint2*>(sm.row[i] + rb) = make_uint2(w[0] | (w[1] << 16), w[2] | (w[3] << 16));
+                        if (any) a.rows.store4(sm.row[i], rb, w);
                     }
                 }
             }
@@ -1578,9 +1571,9 @@ __device__ __noinline__ void phase_mixed_mark(const ResolveArgs& e, int32_t S) {
         const uint64_t rs = splitmix64(a.dl.perm_seed + (uint64_t)(a.rbegin + r));
         const int32_t s0 = (int32_t)(wi / rblocks) * spb, s1 = min(S, s0 + spb);
         for (int32_t s = s0; s < s1; ++s) {
-            uint16_t* p = a.masks + ((size_t)s * 2 + a.cur[s]) * a.Rpad + r;
-            const uint32_t w = *p;
-            if (!(w & CD_BIT_EMIT) && emitted_in_batch(e, s, r, w, rs)) *p = (uint16_t)(w | CD_BIT_EMIT);
+            uint8_t* row = a.rows.cur_lo(s);
+            const uint32_t w = a.rows.get(row, r);
+            if (!(w & CD_BIT_EMIT) && emitted_in_batch(e, s, r, w, rs)) a.rows.hi_or(row, r, CD_BIT_EMIT);
         }
     }
 }
@@ -1593,12 +1586,11 @@ __device__ void phase_inval_unmark(const ResolveArgs& e) {
         const int32_t sl = a.wl.slots[p / a.wl.n_tiles];
         const int tile = (int)(p % a.wl.n_tiles);
         if (!a.wl.in_tile[(size_t)sl * a.wl.n_tiles + tile]) continue;
-        uint16_t* row = a.masks + ((size_t)sl * 2 + a.cur[sl]) * a.Rpad;
+        uint8_t* row = a.rows.cur_lo(sl);
         for (int q = 0; q < TILE_R / GEN_THREADS; ++q) {
             const int64_t r = (int64_t)tile * TILE_R + q * GEN_THREADS + threadIdx.x;
             if (r >= a.R) continue;
-            const uint32_t w = row[r];
-            if (w & CD_BIT_CALL) row[r] = (uint16_t)(w & ~CD_BIT_CALL);
+            if (a.rows.get(row, r) & CD_BIT_CALL) a.rows.hi_clear(row, r, CD_BIT_CALL);
         }
     }
 }
@@ -1640,11 +1632,11 @@ __device__ void resolve_tail(const ResolveArgs& a, int32_t serial) {
 __device__ void phase_ref_compare(const ResolveArgs& e, const int64_t r0, const int Sb, const int S_before) {
     static_assert(TILE_R == 4 * GEN_THREADS, "a thread owns 4 receivers of a tile");
     const ApplyArgs& a = e.ap;
-    const uint32_t RM2 = ((1u << a.K) - 1u) * 0x10001u;
+    const uint32_t RM = (1u << a.K) - 1u;
     const int t = threadIdx.x;
     // work items: (tile, chunk of subjects); a block-wide OR-reduction is not needed — each thread owns its 4 receivers' bits
     constexpr int CH = 64;
-    __shared__ const uint16_t* s_row[CH];
+    __shared__ const uint8_t* s_row[CH];
     __shared__ uint32_t s_ref[CH];
     const int nch = (Sb + CH - 1) / CH;
     const int64_t items = (int64_t)a.n_tiles * nch;
@@ -1655,20 +1647,20 @@ __device__ void phase_ref_compare(const ResolveArgs& e, const int64_t r0, const 
         __syncthreads();
         if (t < nb) {
             const int32_t slot = a.desc[b0 + t].slot;
-            const uint16_t* row = slot >= S_before ? nullptr : a.masks + ((size_t)slot * 2 + a.cur[slot]) * a.Rpad;   // pre-batch row (not flipped yet); fresh: state 0 for everyone
+            const uint8_t* row = slot >= S_before ? nullptr : a.rows.cur_lo(slot);   // pre-batch row (not flipped yet); fresh: state 0 for everyone
             s_row[t] = row;
-            s_ref[t] = row ? (uint32_t)row[r0] * 0x10001u : 0u;
+            s_ref[t] = row ? a.rows.get(row, r0) & RM : 0u;
         }
         __syncthreads();
-        uint32_t dx = 0, dy = 0;
+        uint32_t bits = 0;
 #pragma unroll 8
         for (int i = 0; i < nb; ++i) {
-            const uint16_t* row = s_row[i];
+            const uint8_t* row = s_row[i];
             if (row == nullptr) continue;
-            const uint2 w = *reinterpret_cast<const uint2*>(row + rb);
-            dx |= (w.x ^ s_ref[i]) & RM2; dy |= (w.y ^ s_ref[i]) & RM2;
+            const uint2 g = a.rows.load4(row, rb);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) bits |= ((a.rows.word4(g, j) ^ s_ref[i]) & RM) ? 1u << j : 0u;
         }
-        const uint32_t bits = ((dx & 0xFFFFu) ? 1u : 0u) | ((dx >> 16) ? 2u : 0u) | ((dy & 0xFFFFu) ? 4u : 0u) | ((dy >> 16) ? 8u : 0u);
         if (bits) atomicOr(&e.mx_dev[rb >> 5], bits << (rb & 31));
     }
 }
@@ -1740,7 +1732,7 @@ __global__ void __launch_bounds__(GEN_THREADS) k_seq_check(const ResolveArgs* __
         for (int32_t sl = q0; sl < q1; ++sl) {
             if (sl >= S_before || !ap.wl.has_so[sl] || a.touch[sl] == a.serial) continue;      // (uniform across the block)
             if (!active || bDown == T32_NONE) continue;
-            const uint32_t us = (ap.masks + ((size_t)sl * 2 + ap.cur[sl]) * ap.Rpad)[r] & RM;
+            const uint32_t us = ap.rows.get(sl, r) & RM;
             const int cs = __popc(us);
             if (cs < ap.L || cs >= ap.H) continue;                         // not in this receiver's preProposal
             for (int k = 0; k < ap.K; ++k) {
@@ -1748,7 +1740,7 @@ __global__ void __launch_bounds__(GEN_THREADS) k_seq_check(const ResolveArgs* __
                 if (so < 0 || ((us >> k) & 1u)) continue;
                 const bool o_touched = a.touch[so] == a.serial;
                 const int bo_idx = o_touched ? a.batch_index[so] : 0;
-                const uint32_t uo = so < S_before ? ((ap.masks + ((size_t)so * 2 + ap.cur[so]) * ap.Rpad)[r] & RM) : 0u;
+                const uint32_t uo = so < S_before ? (ap.rows.get(so, r) & RM) : 0u;
                 const uint32_t bLo = observer_L_batch(uo, o_touched ? &ap.desc[bo_idx] : nullptr, o_touched ? &ap.pwalk[bo_idx] : nullptr, ap.L);
                 if (bLo != T32_NONE && max(bLo, bDown) <= last) bad = 1;  // an invalidation pass inside the prefix would report ring k
             }
@@ -2010,6 +2002,17 @@ int32_t bucketed_clear(CD* cd) {
     return RAPID_OK;
 }
 
+template <int HB>
+static void launch_uniform(dim3 grid, cudaStream_t s, const ApplyArgs& ap, bool counts_only, bool seq) {
+    if (seq) {
+        if (counts_only) k_apply_uniform<true, true, HB><<<grid, UNI_THREADS, 0, s>>>(ap);
+        else k_apply_uniform<false, true, HB><<<grid, UNI_THREADS, 0, s>>>(ap);
+    } else {
+        if (counts_only) k_apply_uniform<true, false, HB><<<grid, UNI_THREADS, 0, s>>>(ap);
+        else k_apply_uniform<false, false, HB><<<grid, UNI_THREADS, 0, s>>>(ap);
+    }
+}
+
 // Everything of one batch after k_prepare, enqueued on the handle's stream with NO host synchronisation: the apply kernel
 // (grid sized from an ESTIMATE of the number of batch subjects — the kernels take the real one from the device counters), the
 // cooperative resolve kernel, and the copy of the counter snapshot to pinned host memory.
@@ -2025,7 +2028,7 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
         int dev = 0, sms = TARGET_SMS, per_u = 8, per_g = 4, per_r = 2;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_u, k_apply_uniform<false, false>, UNI_THREADS, 0);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_u, k_apply_uniform<false, false, 4>, UNI_THREADS, 0);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_g, k_apply_generic, GEN_THREADS, 0);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_r, k_mixed_flip, GEN_THREADS, 0);
         int per_m = 2;
@@ -2090,7 +2093,7 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
     Partials part{b->p_cnt.p, b->p_cntp.p, b->p_minTH.p, b->p_minTLun.p, b->p_h1.p, b->p_h2.p, b->p_h1p.p, b->p_h2p.p, b->p_seq.p, b->p_flag.p, b->p_chunk.p, b->n_tiles};
 
     ApplyArgs ap;
-    ap.masks = cd->masks.p; ap.cur = cd->cur.p; ap.Rpad = cd->Rpad;
+    ap.rows = RowRef{cd->masks.p, cd->cur.p, cd->Rpad, cd->row_stride, cd->nbuf, cd->hb}; ap.Rpad = cd->Rpad;
     ap.K = cd->K; ap.H = cd->H; ap.L = cd->L; ap.R = cd->R; ap.rbegin = cd->rbegin;
     ap.rflags = cd->rflags.p; ap.dl = dl; ap.bc = cd->counts.p;
     ap.desc = b->desc.p; ap.walk = b->walk.p; ap.pwalk = b->pwalk.p; ap.slot_subject = cd->slot_subject.p;
@@ -2101,13 +2104,8 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
     RAPID_CUDA(cudaEventRecord(cd->evk0, s));
     if (swar) {
         dim3 grid((unsigned)b->n_tiles, (unsigned)n_chunks);
-        if (seq) {
-            if (counts_only) k_apply_uniform<true, true><<<grid, UNI_THREADS, 0, s>>>(ap);
-            else k_apply_uniform<false, true><<<grid, UNI_THREADS, 0, s>>>(ap);
-        } else {
-            if (counts_only) k_apply_uniform<true, false><<<grid, UNI_THREADS, 0, s>>>(ap);
-            else k_apply_uniform<false, false><<<grid, UNI_THREADS, 0, s>>>(ap);
-        }
+        if (cd->hb == 4) launch_uniform<4>(grid, s, ap, counts_only, seq);
+        else launch_uniform<8>(grid, s, ap, counts_only, seq);
         cd->last_path = counts_only ? 4 : 2;
     } else {
         dim3 grid((unsigned)(cd->Rpad / GEN_THREADS), (unsigned)n_chunks);

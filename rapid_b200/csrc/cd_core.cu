@@ -7,8 +7,8 @@
 //   MembershipService.java:300-354    batch driver (union of emissions, announcedProposal gating)
 //   MembershipService.java:644-675    filterAlertMessages
 // The Java keeps Map<Endpoint, Map<Integer, Endpoint>> per process; here the state of R virtual nodes is a
-// [subject slot][receiver] array of 16-bit ring masks in HBM and every receiver is one CUDA thread (sweep
-// kernel) or a SWAR lane of the subject-bucketed kernels (cd_bucketed.cu).
+// [subject slot][receiver] array of ring masks in HBM (RowRef: 16-bit words, or packed planes on bucketed handles) and every
+// receiver is one CUDA thread (sweep kernel) or a SWAR lane of the subject-bucketed kernels (cd_bucketed.cu).
 #include <algorithm>
 #include <climits>
 #include <cstdio>
@@ -181,7 +181,7 @@ __global__ void k_gather_proposal(RowRef rows, int32_t S, int64_t r, int H, uint
                                   int32_t* __restrict__ count) {
     const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= S) return;
-    const uint32_t w = rows.row(s)[r];
+    const uint32_t w = rows.get(s, r);
     const bool in = rule_ge_h ? (__popc(w & RM) >= H) : ((w & CD_BIT_EMIT) != 0);
     if (in) {
         const int32_t at = atomicAdd(count, 1);
@@ -194,7 +194,7 @@ __global__ void k_dump_masks(RowRef rows, int32_t S, int64_t r, uint32_t RM, con
     const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= S) return;
     out_ids[s] = slot_subject[s];
-    out_masks[s] = (uint16_t)(rows.row(s)[r] & RM);
+    out_masks[s] = (uint16_t)(rows.get(s, r) & RM);
 }
 
 // S < 0: the slot count lives on the device (bucketed handles), the grid covers the handle's capacity
@@ -220,7 +220,7 @@ __global__ void k_clear_receivers(int64_t R, int32_t* __restrict__ n_pre, int32_
 // =====================================================================================================
 // host side
 // =====================================================================================================
-static RowRef rowref(const CD* cd) { return RowRef{cd->masks.p, cd->cur.p, cd->Rpad, cd->nbuf}; }
+static RowRef rowref(const CD* cd) { return RowRef{cd->masks.p, cd->cur.p, cd->Rpad, cd->row_stride, cd->nbuf, cd->hb}; }
 
 static int32_t ensure_id_capacity(CD* cd) {
     const int64_t ntot = cd->view->n + cd->view->nj;
@@ -246,13 +246,13 @@ static int32_t ensure_slot_capacity(CD* cd, size_t need) {
     if (need <= cd->S_cap) return RAPID_OK;
     size_t ncap = need;                       // first allocation: exactly what was asked for (max_subjects)
     if (cd->S_cap) { ncap = cd->S_cap; while (ncap < need) ncap *= 2; }
-    const size_t row = cd->Rpad * (size_t)cd->nbuf;
-    const size_t old_elems = cd->S_cap * row;
+    const size_t row = cd->row_stride * (size_t)cd->nbuf;   // bytes per slot (both planes of every buffer of a bucketed handle)
+    const size_t old_bytes = cd->S_cap * row;
     // DevBuf::reserve(keep) rounds to a power of two of elements; force the exact size instead
-    DevBuf<uint16_t> nm;
+    DevBuf<uint8_t> nm;
     RAPID_CHECK(nm.reserve(ncap * row));
-    if (old_elems) RAPID_CUDA(cudaMemcpyAsync(nm.p, cd->masks.p, old_elems * sizeof(uint16_t), cudaMemcpyDeviceToDevice, cd->stream));
-    RAPID_CUDA(cudaMemsetAsync(nm.p + old_elems, 0, (ncap * row - old_elems) * sizeof(uint16_t), cd->stream));
+    if (old_bytes) RAPID_CUDA(cudaMemcpyAsync(nm.p, cd->masks.p, old_bytes, cudaMemcpyDeviceToDevice, cd->stream));
+    RAPID_CUDA(cudaMemsetAsync(nm.p + old_bytes, 0, ncap * row - old_bytes, cd->stream));
     DevBuf<uint8_t> nc;
     RAPID_CHECK(nc.reserve(ncap));
     RAPID_CUDA(cudaMemsetAsync(nc.p, 0, ncap, cd->stream));
@@ -787,6 +787,8 @@ int32_t rapid_cd_create(rapid_cd** out, const rapid_view* v, int32_t H, int32_t 
     // rows are 256-byte multiples; bucketed handles pad to whole 1024-receiver tiles so every uint4 access is in-bounds
     const int64_t pad = cd->bucketed ? 1024 : 128;
     cd->Rpad = (size_t)ceil_div<int64_t>(n_receivers, pad) * pad;
+    cd->hb = cd->bucketed ? row_hi_bits(K) : 0;
+    cd->row_stride = cd->bucketed ? cd->Rpad + cd->Rpad * cd->hb / 8 : cd->Rpad * sizeof(uint16_t);
     int32_t rc = RAPID_OK;
     do {
         if (cudaStreamCreateWithFlags(&cd->stream, cudaStreamNonBlocking) != cudaSuccess ||
@@ -858,7 +860,7 @@ int32_t rapid_cd_clear(rapid_cd* cd) {
             k_reset_slots<<<(unsigned)ceil_div<int32_t>(cd->S, 256), 256, 0, s>>>(cd->S, cd->counts.p, cd->slot_subject.p, cd->slot_of.p, cd->cur.p);
             RAPID_KERNEL_CHECK();
             // the sweep kernel reads in place and needs zeros
-            RAPID_CUDA(cudaMemsetAsync(cd->masks.p, 0, (size_t)cd->S * cd->nbuf * cd->Rpad * sizeof(uint16_t), s));
+            RAPID_CUDA(cudaMemsetAsync(cd->masks.p, 0, (size_t)cd->S * cd->nbuf * cd->row_stride, s));
         }
         cd->S = 0;
         k_clear_receivers<<<(unsigned)ceil_div<size_t>(R, 256), 256, 0, s>>>((int64_t)R, cd->n_pre.p, cd->n_prop.p, cd->rflags.p, cd->pend_h1.p,

@@ -2,18 +2,21 @@
 #pragma once
 
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
 
 namespace rapid {
 
-// ---- the 16-bit state word per (subject slot, receiver) ------------------------------------------
+// ---- the logical state word per (subject slot, receiver) -----------------------------------------
 // bits 0..K-1 : ring r has reported the subject  (reportsPerHost[subject].containsKey(r),
 //               MultiNodeCutDetector.java:92-101)
-// bit 14      : RAW mode only — emitted by the call in flight (returned list of aggregateForProposal)
+// bit 14      : sweep handles, RAW mode: emitted by the call in flight (returned list of aggregateForProposal);
+//               bucketed handles: transient marker of the invalidation pass (set and cleared inside one batch)
 // bit 15      : subject was emitted in a proposal (it left `proposal` at :118-121)
 // preProposal == { L <= popc < H },  proposal == { popc >= H and bit 15 clear }.
+// Kernels compute on this 16-bit word; how it is stored is the business of RowRef below.
 #define CD_BIT_CALL 0x4000u
 #define CD_BIT_EMIT 0x8000u
 
@@ -71,7 +74,9 @@ struct CD {
     size_t S_cap = 0;
     int64_t ntot_cap = 0;             // capacity of slot_of / first_idx (node + joiner ids)
 
-    DevBuf<uint16_t> masks;           // [S_cap][nbuf][Rpad]
+    int hb = 0;                       // bits per receiver of a row's hi plane (bucketed handles), 0: uint16 rows (sweep)
+    size_t row_stride = 0;            // bytes per (slot, buffer) row
+    DevBuf<uint8_t> masks;            // [S_cap][nbuf] rows of row_stride bytes (see RowRef)
     DevBuf<uint8_t> cur;              // [S_cap] which of the nbuf rows is current
     DevBuf<int32_t> slot_of;          // [ntot_cap] id -> slot, -1 if none
     DevBuf<int32_t> first_idx;        // [ntot_cap] scratch (INT_MAX)
@@ -133,19 +138,187 @@ struct CD {
     int64_t last_A = 0;
 };
 
-// row pointer helpers (device)
+// ---- state rows: the only code that knows how a row stores the logical words ---------------------------------------------
+// Sweep handles: one interleaved uint16_t[Rpad] row per slot (the sweep kernel reads and writes one receiver per thread in place).
+// Bucketed handles: every (slot, buffer) row is two planes, each padded to whole 1024-receiver tiles, back to back:
+//   lo plane  uint8_t[Rpad]        bits 0..7 of the word (rings 0..7)
+//   hi plane  Rpad lanes of HB bits, receiver r in bits [HB * r, HB * r + HB) of the plane
+//             HB = 4 (K <= 10): rings 8, 9, bit 14, bit 15            -> 1.5 B per receiver
+//             HB = 8 (K <= 14): rings 8..13, bit 14, bit 15           -> 2 B per receiver
+// At HB = 4 two receivers share a byte of the hi plane: a lane is written either as part of a thread-owned group of whole
+// bytes (the group accessors), or with an atomic on its aligned 32-bit word (hi_or / hi_clear) — never with a plain sub-byte store.
+__host__ __device__ inline int row_hi_bits(int K) { return K <= 10 ? 4 : 8; }
+
+template <int HB>
+__device__ __forceinline__ uint32_t hi_pack(uint32_t w) {      // logical word -> hi lane
+    return HB == 4 ? (((w >> 8) & 3u) | ((w >> 12) & 0xCu)) : ((w >> 8) & 0xFFu);
+}
+template <int HB>
+__device__ __forceinline__ uint32_t hi_unpack(uint32_t h) {    // hi lane -> bits 8.. of the logical word
+    return HB == 4 ? (((h & 3u) << 8) | ((h & 0xCu) << 12)) : (h << 8);
+}
+
 struct RowRef {
-    uint16_t* masks;
+    uint8_t* base;
     const uint8_t* cur;
     size_t Rpad;
+    size_t stride;                    // bytes per (slot, buffer) row
     int nbuf;
-    __device__ __forceinline__ uint16_t* row(int32_t slot) const {
-        return masks + ((size_t)slot * nbuf + (nbuf == 2 ? cur[slot] : 0)) * Rpad;
+    int hb;                           // 0: uint16 rows (sweep); 4 / 8: two planes (bucketed)
+
+    // lo plane of (slot, buffer); the hi plane follows it
+    __device__ __forceinline__ uint8_t* lo(int32_t slot, int buf) const { return base + ((size_t)slot * nbuf + buf) * stride; }
+    __device__ __forceinline__ uint8_t* cur_lo(int32_t slot) const { return lo(slot, nbuf == 2 ? cur[slot] : 0); }
+    __device__ __forceinline__ uint8_t* alt_lo(int32_t slot) const { return lo(slot, cur[slot] ^ 1); }   // the non-current row (nbuf == 2)
+    __device__ __forceinline__ uint16_t* row(int32_t slot) const {     // sweep handles
+        return reinterpret_cast<uint16_t*>(cur_lo(slot));
     }
-    __device__ __forceinline__ uint16_t* alt(int32_t slot) const {   // the non-current row (nbuf == 2)
-        return masks + ((size_t)slot * nbuf + (cur[slot] ^ 1)) * Rpad;
+
+    // scalar get of receiver r's word in the row whose lo plane is `l`
+    __device__ __forceinline__ uint32_t get(const uint8_t* l, int64_t r) const {
+        if (hb == 0) return reinterpret_cast<const uint16_t*>(l)[r];
+        if (hb == 4) return l[r] | hi_unpack<4>((l[Rpad + (r >> 1)] >> ((r & 1) * 4)) & 0xFu);
+        return l[r] | hi_unpack<8>(l[Rpad + r]);
+    }
+    __device__ __forceinline__ uint32_t get(int32_t slot, int64_t r) const { return get(cur_lo(slot), r); }
+
+    // receivers r .. r+3 (r % 4 == 0) of a bucketed row: one 32-bit lo load, one 16- or 32-bit hi load; x = lo lanes, y = hi lanes
+    __device__ __forceinline__ uint2 load4(const uint8_t* l, int64_t r) const {
+        return make_uint2(*reinterpret_cast<const uint32_t*>(l + r),
+                          hb == 4 ? (uint32_t)*reinterpret_cast<const uint16_t*>(l + Rpad + (r >> 1))
+                                  : *reinterpret_cast<const uint32_t*>(l + Rpad + r));
+    }
+    __device__ __forceinline__ uint32_t word4(uint2 g, int j) const {   // receiver r + j of a load4 group as a logical word
+        return ((g.x >> (8 * j)) & 0xFFu) | (hb == 4 ? hi_unpack<4>((g.y >> (4 * j)) & 0xFu) : hi_unpack<8>((g.y >> (8 * j)) & 0xFFu));
+    }
+    __device__ __forceinline__ void store4(uint8_t* l, int64_t r, const uint32_t w[4]) const {
+        uint32_t lw = 0, hw = 0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            lw |= (w[j] & 0xFFu) << (8 * j);
+            hw |= hb == 4 ? hi_pack<4>(w[j]) << (4 * j) : hi_pack<8>(w[j]) << (8 * j);
+        }
+        *reinterpret_cast<uint32_t*>(l + r) = lw;
+        if (hb == 4) *reinterpret_cast<uint16_t*>(l + Rpad + (r >> 1)) = (uint16_t)hw;
+        else *reinterpret_cast<uint32_t*>(l + Rpad + r) = hw;
+    }
+
+    // bucketed rows: set / clear bits 14 / 15 of receiver r's word (its neighbours may be written at the same time)
+    __device__ __forceinline__ uint32_t* hi_word(uint8_t* l, int64_t r, uint32_t bit, uint32_t* shift) const {
+        const int64_t p = r * hb + (hb - (bit == CD_BIT_EMIT ? 1 : 2));   // bit 15 is the lane's top bit, bit 14 the one below
+        *shift = (uint32_t)(p & 31);
+        return reinterpret_cast<uint32_t*>(l + Rpad) + (p >> 5);
+    }
+    __device__ __forceinline__ void hi_or(uint8_t* l, int64_t r, uint32_t bit) const {
+        uint32_t sh;
+        uint32_t* p = hi_word(l, r, bit, &sh);
+        atomicOr(p, 1u << sh);
+    }
+    __device__ __forceinline__ void hi_clear(uint8_t* l, int64_t r, uint32_t bit) const {
+        uint32_t sh;
+        uint32_t* p = hi_word(l, r, bit, &sh);
+        atomicAnd(p, ~(1u << sh));
     }
 };
+
+// 8 consecutive receivers of a bucketed row (r % 8 == 0), as SWAR lanes: lo = 8 byte lanes, hi = 8 lanes of HB bits
+template <int HB>
+struct Group8 {
+    using Hi = typename std::conditional<HB == 4, uint32_t, uint64_t>::type;
+    uint64_t lo;
+    Hi hi;
+};
+template <int HB>
+__device__ __forceinline__ const uint8_t* group8_hi(const RowRef& rows, const uint8_t* l, int64_t r) {   // the group's hi lanes
+    return l + rows.Rpad + (r * HB >> 3);
+}
+template <int HB>
+__device__ __forceinline__ Group8<HB> group8_load(const RowRef& rows, const uint8_t* l, int64_t r) {
+    Group8<HB> g;
+    g.lo = *reinterpret_cast<const uint64_t*>(l + r);
+    g.hi = *reinterpret_cast<const typename Group8<HB>::Hi*>(group8_hi<HB>(rows, l, r));
+    return g;
+}
+template <int HB>
+__device__ __forceinline__ void group8_store(const RowRef& rows, uint8_t* l, int64_t r, const Group8<HB>& g) {
+    *reinterpret_cast<uint64_t*>(l + r) = g.lo;
+    *reinterpret_cast<typename Group8<HB>::Hi*>(const_cast<uint8_t*>(group8_hi<HB>(rows, l, r))) = g.hi;
+}
+// lane j of a group as a logical word
+template <int HB>
+__device__ __forceinline__ uint32_t group8_word(const Group8<HB>& g, int j) {
+    return (uint32_t)((g.lo >> (8 * j)) & 0xFFu) | hi_unpack<HB>((uint32_t)(g.hi >> (HB * j)) & ((1u << HB) - 1u));
+}
+// lane j |= the logical bits `w`
+template <int HB>
+__device__ __forceinline__ void group8_or_word(Group8<HB>& g, int j, uint32_t w) {
+    g.lo |= (uint64_t)(w & 0xFFu) << (8 * j);
+    g.hi |= (typename Group8<HB>::Hi)hi_pack<HB>(w) << (HB * j);
+}
+// A logical word replicated over the lanes: x = its lo byte over 4 byte lanes, y = its hi lane over 32 bits (as the lanes repeat)
+template <int HB>
+__device__ __forceinline__ uint2 group8_rep(uint32_t w) {
+    return make_uint2((w & 0xFFu) * 0x01010101u, hi_pack<HB>(w) * (HB == 4 ? 0x11111111u : 0x01010101u));
+}
+// all-ones lanes for the receivers set in `act` (bit j = receiver j of the group)
+template <int HB>
+__device__ __forceinline__ Group8<HB> group8_mask(uint32_t act) {
+    Group8<HB> m;
+    m.lo = 0; m.hi = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+        if ((act >> j) & 1u) { m.lo |= 0xFFull << (8 * j); m.hi |= (typename Group8<HB>::Hi)((1u << HB) - 1u) << (HB * j); }
+    return m;
+}
+// the replicated word `rep` under the mask (the lanes outside it are zero)
+template <int HB>
+__device__ __forceinline__ Group8<HB> group8_fill(uint2 rep, const Group8<HB>& m) {
+    Group8<HB> g;
+    g.lo = (((uint64_t)rep.x << 32) | rep.x) & m.lo;
+    g.hi = (HB == 4 ? (typename Group8<HB>::Hi)rep.y : (typename Group8<HB>::Hi)(((uint64_t)rep.y << 32) | rep.y)) & m.hi;
+    return g;
+}
+// the lanes under the mask take the replicated word `rep`, the others keep theirs
+template <int HB>
+__device__ __forceinline__ void group8_merge(Group8<HB>& g, uint2 rep, const Group8<HB>& m) {
+    const Group8<HB> f = group8_fill<HB>(rep, m);
+    g.lo = (g.lo & ~m.lo) | f.lo;
+    g.hi = (g.hi & ~m.hi) | f.hi;
+}
+// Do all lanes under the (non-empty) mask hold the same word?  AND over them == OR over them, per plane.  *st = the OR.
+template <int B, typename T>
+__device__ __forceinline__ bool lanes_same(T x, T m, uint32_t* v) {
+    T a = x | ~m, o = x & m;
+#pragma unroll
+    for (int s = 4 * B; s >= B; s >>= 1) { a &= a >> s; o |= o >> s; }
+    const uint32_t lm = (1u << B) - 1u;
+    *v = (uint32_t)o & lm;
+    return ((uint32_t)a & lm) == *v;
+}
+template <int HB>
+__device__ __forceinline__ bool group8_same(const Group8<HB>& g, const Group8<HB>& m, uint32_t* st) {
+    uint32_t vl, vh;
+    const bool sl = lanes_same<8>(g.lo, m.lo, &vl);
+    const bool sh = lanes_same<HB>(g.hi, m.hi, &vh);
+    *st = vl | hi_unpack<HB>(vh);
+    return sl && sh;
+}
+
+// one receiver per thread, consecutive threads of a warp own consecutive receivers (r % 32 == lane): every lane of the warp
+// stores its word; at HB = 4 the hi lanes of 8 receivers are gathered by shuffles and one lane stores their 32-bit word
+template <int HB>
+__device__ __forceinline__ void row_store1_warp(const RowRef& rows, uint8_t* l, int64_t r, uint32_t w) {
+    l[r] = (uint8_t)w;
+    if (HB == 8) {
+        l[rows.Rpad + r] = (uint8_t)hi_pack<8>(w);
+    } else {
+        uint32_t h = hi_pack<4>(w) << (4 * (r & 7));
+        h |= __shfl_xor_sync(0xffffffffu, h, 1);
+        h |= __shfl_xor_sync(0xffffffffu, h, 2);
+        h |= __shfl_xor_sync(0xffffffffu, h, 4);
+        if ((r & 7) == 0) *reinterpret_cast<uint32_t*>(l + rows.Rpad + (r >> 1)) = h;
+    }
+}
 
 struct DeliveryDev {
     uint32_t flags = 0;
