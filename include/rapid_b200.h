@@ -148,6 +148,19 @@ int32_t rapid_view_joiner_tables(const rapid_view* v, int32_t* out);
 #define RAPID_DELIVERY_BITMAP   2u   /* bitmap[cell][ceil(R/32)]: bit (r&31) of word r>>5 set = delivered   */
 #define RAPID_DELIVERY_PERMUTED 4u   /* receiver r applies its cells in ascending
                                         splitmix64( splitmix64(perm_seed + receiver_begin + r) ^ cell_index ) */
+#define RAPID_DELIVERY_SHUFFLED_BATCHES 8u
+/* RAPID_DELIVERY_SHUFFLED_BATCHES — rapid_cd_apply_batches / rapid_cd_apply_batches_dev on SERVICE sweep handles (RAPID_CD_SWEEP)
+ * only, alone or with BLOCKED: every receiver meets the n batches of the sequence in its own pseudo-random order, as the
+ * reference's per-sender shuffled recipient lists make it (UnicastToAllBroadcaster.java:59-62), and the cells of each batch in
+ * array order.  Receiver r (global index g = receiver_begin + r) handles batch P_g(j) at its step j = 0..n-1:
+ *     if n <= 1: identity
+ *     w   = smallest integer >= 4 with 4^w >= n;   m = 2^w - 1     (w >= 4: narrower halves skew the orders of small n)
+ *     key = splitmix64(perm_seed + g)
+ *     f(i, x) = splitmix64(key ^ ((uint64)(i + 1) << 58) ^ x) & m          for rounds i = 0..3
+ *     E(v): a = v >> w; b = v & m; 4 times: (a, b) = (b, a ^ f(i, b)); return (a << w) | b
+ *     P_g(j): v = E(j); while v >= n: v = E(v); return v                  (a bijection of [0, n))
+ * announced_in[r] is the array index of the announcing batch.  Bucketed and RAW handles refuse it (RAPID_EUNSUPPORTED); with
+ * PERMUTED or BITMAP, or on a single-batch entry point, it is RAPID_EINVAL.  A refused call changes nothing. */
 typedef struct rapid_delivery {
     uint32_t        flags;
     const uint8_t*  blocked;     /* [R]                    (host) */

@@ -15,7 +15,7 @@ OK = 0
 EINVAL, ENOT_IN_RING, EALREADY_IN_RING, EUUID_SEEN, EHASH_COLLISION, ECUDA, ENCCL, ENOMEM, EUNSUPPORTED = range(-1, -10, -1)
 
 CD_SERVICE, CD_RAW, CD_SWEEP, CD_BUCKETED, CD_LOG = 0, 1, 2, 4, 8
-DELIVERY_BLOCKED, DELIVERY_BITMAP, DELIVERY_PERMUTED = 1, 2, 4
+DELIVERY_BLOCKED, DELIVERY_BITMAP, DELIVERY_PERMUTED, DELIVERY_SHUFFLED_BATCHES = 1, 2, 4, 8
 WIRE_REQUEST = 1
 WIRE_FAST_ROUND_PHASE2B, WIRE_PHASE1A, WIRE_PHASE1B, WIRE_PHASE2A, WIRE_PHASE2B = 5, 6, 7, 8, 9   # RapidRequest cases
 EDGE_UP, EDGE_DOWN = 0, 1

@@ -53,8 +53,12 @@ struct SweepArgs {
     const int64_t* batch_off;    // NULL: the cells are ONE BatchedAlertMessage; else batch b = cells [batch_off[b], batch_off[b+1])
     int32_t n_batches;
     int32_t* out_batch;          // with batch_off: index of the batch in which the receiver announced during this call, -1 otherwise
+    int64_t rbegin;              // SHUF: receiver r is global receiver rbegin + r (the key of its batch order)
 };
 
+// SHUF = false: every receiver meets the batches in array order.  SHUF = true (RAPID_DELIVERY_SHUFFLED_BATCHES): receiver r meets
+// them in the order batch_order_at(batch_order_init(perm_seed, rbegin + r, n_batches), j), j = 0, 1, ...
+template <bool SHUF>
 __global__ void __launch_bounds__(128) k_sweep(const SweepArgs a) {
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= a.R) return;
@@ -73,6 +77,8 @@ __global__ void __launch_bounds__(128) k_sweep(const SweepArgs a) {
     bool seen = flags & RF_SEEN_DOWN;
     uint64_t oh1 = 0, oh2 = 0;
     int32_t olen = 0;
+    // SHUF: whether an invalidation pass could add a report (see the rule at the pass); set at the start of the call
+    bool dirty = true;
 
     // proposal emission (:110-121): everything at >= H that has not been emitted yet leaves in one proposal
     auto emit = [&]() {
@@ -98,7 +104,10 @@ __global__ void __launch_bounds__(128) k_sweep(const SweepArgs a) {
         w |= bit;
         *p = (uint16_t)w;
         const int c = __popc(w & RM);
-        if (c == a.L) ++npre;                              // :104-107
+        if (c == a.L) {                                    // :104-107
+            ++npre;
+            if (SHUF) dirty = true;
+        }
         if (c == a.H) {                                    // :109-121
             --npre;
             if (npre == 0) emit();
@@ -110,18 +119,31 @@ __global__ void __launch_bounds__(128) k_sweep(const SweepArgs a) {
     const bool has_bitmap = a.dl.flags & RAPID_DELIVERY_BITMAP;
     const int32_t nb = a.batch_off ? a.n_batches : 1;
     int32_t ann_batch = -1;
-    for (int32_t b = 0; b < nb; ++b) {
+    BatchOrder order;
+    if (SHUF) order = batch_order_init(a.dl.perm_seed, a.rbegin + r, nb);
+    for (int32_t j = 0; j < nb; ++j) {
+        const int32_t b = SHUF ? (int32_t)batch_order_at(order, j) : j;
         const int64_t i0 = a.batch_off ? a.batch_off[b] : 0, i1 = a.batch_off ? a.batch_off[b + 1] : a.A;
         if (a.do_cells) {
             for (int64_t i = i0; i < i1; ++i) {
                 const int32_t slot = a.cell_slot[i];
                 if (slot < 0) continue;
                 if (has_bitmap && !((a.dl.bitmap[(size_t)i * a.dl.words + (r >> 5)] >> (r & 31)) & 1u)) continue;
-                if (a.status[i] == RAPID_EDGE_DOWN) seen = true;   // :88-90 (before the duplicate check)
+                if (a.status[i] == RAPID_EDGE_DOWN) {              // :88-90 (before the duplicate check)
+                    if (SHUF && !seen) dirty = true;
+                    seen = true;
+                }
                 report(slot, a.ring[i]);
             }
         }
-        if (a.do_inval && seen && npre > 0) {                  // :137-164
+        // Pass skipping (SHUF, where a receiver may run a pass after each of thousands of batches).  Before an emission, in service
+        // mode, U = preProposal u proposal only grows, and a pass adds implicit reports only for (n in preProposal, k) with
+        // obs_k(n) in U.  A pass adds no subject to U (its reports are about subjects already at >= L) and leaves every such pair
+        // reported, so the next pass can add something only if, since this one, a subject crossed L (entered U and preProposal) or
+        // seenLinkDownEvents became true.  dirty records exactly that, so a skipped pass is one that would have changed nothing,
+        // and the passes per receiver are bounded by #subjects + 1 instead of #batches.
+        if (a.do_inval && seen && npre > 0 && (!SHUF || dirty)) {   // :137-164
+            if (SHUF) dirty = false;
             for (int32_t s = 0; s < a.S; ++s) {
                 const uint32_t w0 = a.rows.row(s)[r];
                 const int c0 = __popc(w0 & RM);
@@ -369,9 +391,11 @@ static int32_t launch_sweep(CD* cd, int64_t A, const uint8_t* ring_dev, const ui
     a.dl = dl;
     a.n_pre = cd->n_pre.p; a.n_prop = cd->n_prop.p; a.rflags = cd->rflags.p;
     a.out_h1 = cd->out_h1.p; a.out_h2 = cd->out_h2.p; a.out_len = cd->out_len.p; a.out_ann = cd->out_ann.p;
+    a.rbegin = cd->rbegin;
     const int TB = 128;
     RAPID_CUDA(cudaEventRecord(cd->evk0, cd->stream));
-    k_sweep<<<(unsigned)ceil_div<int64_t>(cd->R, TB), TB, 0, cd->stream>>>(a);
+    if (dl.flags & RAPID_DELIVERY_SHUFFLED_BATCHES) k_sweep<true><<<(unsigned)ceil_div<int64_t>(cd->R, TB), TB, 0, cd->stream>>>(a);
+    else k_sweep<false><<<(unsigned)ceil_div<int64_t>(cd->R, TB), TB, 0, cd->stream>>>(a);
     RAPID_KERNEL_CHECK();
     RAPID_CUDA(cudaEventRecord(cd->evk1, cd->stream));
     cd->last_launches += 1;
@@ -379,10 +403,26 @@ static int32_t launch_sweep(CD* cd, int64_t A, const uint8_t* ring_dev, const ui
     return RAPID_OK;
 }
 
+// RAPID_DELIVERY_SHUFFLED_BATCHES is checked before anything is staged or applied, so a refusal leaves the handle as it was.
+// Bucketed handles refuse it: their one-pass fold of a sequence needs one last batch shared by every receiver (DESIGN §4.3.1).
+static int32_t check_shuffled(const CD* cd, const rapid_delivery* d, bool sequence) {
+    if (!d || !(d->flags & RAPID_DELIVERY_SHUFFLED_BATCHES)) return RAPID_OK;
+    if (!sequence) { set_error("RAPID_DELIVERY_SHUFFLED_BATCHES orders the batches of a sequence: use rapid_cd_apply_batches(_dev)"); return RAPID_EINVAL; }
+    if (d->flags & (RAPID_DELIVERY_PERMUTED | RAPID_DELIVERY_BITMAP)) {
+        set_error("RAPID_DELIVERY_SHUFFLED_BATCHES applies each batch's cells in array order: it cannot be combined with PERMUTED or BITMAP");
+        return RAPID_EINVAL;
+    }
+    if (cd->bucketed || cd->raw) {
+        set_error("RAPID_DELIVERY_SHUFFLED_BATCHES runs on the per-cell sweep kernel: create a SERVICE handle with RAPID_CD_SWEEP");
+        return RAPID_EUNSUPPORTED;
+    }
+    return RAPID_OK;
+}
+
 static int32_t upload_delivery(CD* cd, int64_t A, const rapid_delivery* d, bool on_device, DeliveryDev* out) {
     *out = DeliveryDev();
     if (!d || d->flags == 0) return RAPID_OK;
-    if (d->flags & ~(RAPID_DELIVERY_BLOCKED | RAPID_DELIVERY_BITMAP | RAPID_DELIVERY_PERMUTED)) { set_error("unknown delivery flags"); return RAPID_EINVAL; }
+    if (d->flags & ~(RAPID_DELIVERY_BLOCKED | RAPID_DELIVERY_BITMAP | RAPID_DELIVERY_PERMUTED | RAPID_DELIVERY_SHUFFLED_BATCHES)) { set_error("unknown delivery flags"); return RAPID_EINVAL; }
     out->flags = d->flags;
     out->perm_seed = d->perm_seed;
     out->words = (cd->R + 31) / 32;
@@ -910,6 +950,7 @@ int32_t rapid_cd_apply_batch_dev(rapid_cd* cd, int64_t cfg_id, int64_t n_cells, 
                                  const rapid_delivery* delivery_dev) {
     (void)src_dev;   // edgeSrc is stored by the Java but never read back (MultiNodeCutDetector.java:101)
     if (!cd || n_cells < 0 || (n_cells && (!dst_dev || !ring_dev || !status_dev))) { set_error("bad arguments"); return RAPID_EINVAL; }
+    RAPID_CHECK(check_shuffled(cd, delivery_dev, false));
     if (cd->raw) { set_error("RAW handles take rapid_cd_aggregate / rapid_cd_invalidate"); return RAPID_EINVAL; }
     DeviceGuard g(cd->device);
     DeliveryDev dl;
@@ -922,6 +963,7 @@ int32_t rapid_cd_apply_batch_dev_async(rapid_cd* cd, int64_t cfg_id, int64_t n_c
                                        const rapid_delivery* delivery_dev) {
     (void)src_dev;
     if (!cd || n_cells < 0 || (n_cells && (!dst_dev || !ring_dev || !status_dev))) { set_error("bad arguments"); return RAPID_EINVAL; }
+    RAPID_CHECK(check_shuffled(cd, delivery_dev, false));
     if (!cd->bucketed) { set_error("asynchronous batches run on the subject-bucketed kernels (SERVICE / BUCKETED handles)"); return RAPID_EUNSUPPORTED; }
     DeviceGuard g(cd->device);
     DeliveryDev dl;
@@ -960,6 +1002,7 @@ int32_t rapid_cd_apply_batch(rapid_cd* cd, int64_t cfg_id, int64_t n_cells, cons
                              int32_t* proposal_len, uint8_t* announced) {
     (void)src;
     if (!cd || n_cells < 0 || (n_cells && (!dst || !ring || !status))) { set_error("bad arguments"); return RAPID_EINVAL; }
+    RAPID_CHECK(check_shuffled(cd, delivery, false));
     if (cd->raw) { set_error("RAW handles take rapid_cd_aggregate / rapid_cd_invalidate"); return RAPID_EINVAL; }
     DeviceGuard g(cd->device);
     Staged st;
@@ -983,6 +1026,7 @@ int32_t rapid_cd_apply_batches(rapid_cd* cd, int64_t cfg_id, int64_t n_cells, co
                                uint8_t* announced, int32_t* announced_in) {
     (void)src;
     if (!cd || n_cells < 0 || (n_cells && (!dst || !ring || !status)) || n_batches < 0 || n_batches > 0x7ffffff0LL || !batch_off) { set_error("bad arguments"); return RAPID_EINVAL; }
+    RAPID_CHECK(check_shuffled(cd, delivery, true));
     if (cd->raw) { set_error("RAW handles take rapid_cd_aggregate / rapid_cd_invalidate"); return RAPID_EINVAL; }
     if (batch_off[0] != 0 || batch_off[n_batches] != n_cells) { set_error("batch_off must run from 0 to n_cells"); return RAPID_EINVAL; }
     for (int64_t b = 0; b < n_batches; ++b)
@@ -1018,6 +1062,7 @@ int32_t rapid_cd_apply_batches_dev(rapid_cd* cd, int64_t cfg_id, int64_t n_cells
                                    const int64_t* batch_off, const rapid_delivery* delivery_dev) {
     (void)src_dev;
     if (!cd || n_cells < 0 || (n_cells && (!dst_dev || !ring_dev || !status_dev)) || n_batches < 0 || n_batches > 0x7ffffff0LL || !batch_off) { set_error("bad arguments"); return RAPID_EINVAL; }
+    RAPID_CHECK(check_shuffled(cd, delivery_dev, true));
     if (cd->raw) { set_error("RAW handles take rapid_cd_aggregate / rapid_cd_invalidate"); return RAPID_EINVAL; }
     if (batch_off[0] != 0 || batch_off[n_batches] != n_cells) { set_error("batch_off must run from 0 to n_cells"); return RAPID_EINVAL; }
     for (int64_t b = 0; b < n_batches; ++b)

@@ -115,8 +115,8 @@ class VirtualCluster:
         except Exception:
             pass
 
-    def _delivery(self, blocked, bitmap, perm_seed):
-        if blocked is None and bitmap is None and perm_seed is None:
+    def _delivery(self, blocked, bitmap, perm_seed, batch_order_seed=None):
+        if blocked is None and bitmap is None and perm_seed is None and batch_order_seed is None:
             return None
         d = N.Delivery()
         keep = []
@@ -135,6 +135,9 @@ class VirtualCluster:
         if perm_seed is not None:
             d.flags |= N.DELIVERY_PERMUTED
             d.perm_seed = perm_seed & 0xFFFFFFFFFFFFFFFF
+        if batch_order_seed is not None:
+            d.flags |= N.DELIVERY_SHUFFLED_BATCHES
+            d.perm_seed = batch_order_seed & 0xFFFFFFFFFFFFFFFF
         self._keep = keep
         return d
 
@@ -186,10 +189,11 @@ class VirtualCluster:
         N.check(N.lib().rapid_cd_sync(self._h))
 
     def handleBatches(self, cfg_id, src, dst, ring, status, batch_off, cell_cfg=None, blocked=None, bitmap=None, perm_seed=None,
-                      read_outputs=True):
+                      read_outputs=True, batch_order_seed=None):
         """A sequence of BatchedAlertMessages (batch b = cells batch_off[b]:batch_off[b+1]) delivered in order, with the
         announcedProposal gating between them (MembershipService.java:318-319).  perm_seed: batch b reaches every receiver in
-        its own order, seeded perm_seed + b (bucketed handles).
+        its own order, seeded perm_seed + b (bucketed handles).  batch_order_seed: every receiver meets the batches in its own
+        order instead, seeded batch_order_seed (RAPID_DELIVERY_SHUFFLED_BATCHES; sweep handles, cells of a batch in array order).
         -> (AlertBatchResult, announced_in): announced_in[r] = index of the batch in which receiver r announced, -1 if none."""
         dst = N.as_i32(dst)
         A = len(dst)
@@ -197,7 +201,7 @@ class VirtualCluster:
         ring, status = N.as_u8(ring), N.as_u8(status)
         off = N.as_i64(batch_off)
         cc = None if cell_cfg is None else N.as_i64(cell_cfg)
-        d = self._delivery(blocked, bitmap, perm_seed)
+        d = self._delivery(blocked, bitmap, perm_seed, batch_order_seed)
         if not read_outputs:
             N.check(N.lib().rapid_cd_apply_batches(self._h, int(cfg_id), A, N.ptr(src), N.ptr(dst), N.ptr(ring), N.ptr(status), N.ptr(cc),
                                                    len(off) - 1, N.ptr(off), C.byref(d) if d is not None else None, None, None, None,
@@ -210,10 +214,11 @@ class VirtualCluster:
                                                N.ptr(ln), N.ptr(ann), N.ptr(ain)))
         return AlertBatchResult(h1, h2, ln, ann), ain
 
-    def handleBatchesDevice(self, cfg_id, n_cells, dst_dev, ring_dev, status_dev, batch_off, cell_cfg_dev=0, blocked_dev=0, perm_seed=None):
+    def handleBatchesDevice(self, cfg_id, n_cells, dst_dev, ring_dev, status_dev, batch_off, cell_cfg_dev=0, blocked_dev=0, perm_seed=None,
+                            batch_order_seed=None):
         """handleBatches with the cell arrays resident in device memory (raw device pointers; batch_off on the host)."""
         d = None
-        if blocked_dev or perm_seed is not None:
+        if blocked_dev or perm_seed is not None or batch_order_seed is not None:
             d = N.Delivery()
             d.flags = 0
             if blocked_dev:
@@ -222,6 +227,9 @@ class VirtualCluster:
             if perm_seed is not None:
                 d.flags |= N.DELIVERY_PERMUTED
                 d.perm_seed = perm_seed & 0xFFFFFFFFFFFFFFFF
+            if batch_order_seed is not None:
+                d.flags |= N.DELIVERY_SHUFFLED_BATCHES
+                d.perm_seed = batch_order_seed & 0xFFFFFFFFFFFFFFFF
         off = N.as_i64(batch_off)
         N.check(N.lib().rapid_cd_apply_batches_dev(self._h, int(cfg_id), int(n_cells), None, dst_dev, ring_dev, status_dev,
                                                    cell_cfg_dev or None, len(off) - 1, N.ptr(off), C.byref(d) if d is not None else None))

@@ -40,9 +40,15 @@ ClusterSimulation rules (tests/simref.py restates them independently, tests/simr
   (tags name endpoints).  Refused with ValueError and no change if the tag is still a member (HOSTNAME_ALREADY_IN_RING), is
   already pending, or if the NodeId was ever given to this simulation (UUID_ALREADY_IN_RING: creation, addJoiners, rejoin).
   Otherwise the tag becomes a pending joiner under the join rules above, and its flags are cleared on admission.
-* Delivery model (a limit): every receiver gets the senders' batches in the same (ascending sender) order; only the cell
-  order within a batch is per receiver.  The reference shuffles batch order per receiver (UnicastToAllBroadcaster.java:59-62).
-  Every node sees every vote, so one tally stands for every node's.
+* Delivery model (batch_order): with "sender" (the default) every receiver gets the senders' batches in the same (ascending
+  sender) order and only the cell order within a batch is per receiver, as step 3 says.  With "shuffled" every receiver meets the
+  interval's batches in its own pseudo-random order, as the reference's per-sender shuffled recipient lists make it
+  (UnicastToAllBroadcaster.java:59-62), and the cells of each batch in array order (one message is parsed in one order): the
+  configuration's VirtualCluster is a sweep handle and step 3 passes batch_order_seed = interval_seed(seed, cfg, interval)
+  (RAPID_DELIVERY_SHUFFLED_BATCHES) instead of the cell-order seeds.  Nothing else in the interval changes.  Receivers that
+  meet the batches in different orders can announce different proposals; the records count them: intervals[i]["proposals"]
+  is the number of distinct proposals announced in the interval, history[c]["distinct_proposals"] the number over the
+  configuration.  Every node sees every vote, so one tally stands for every node's.
 """
 import time
 
@@ -88,7 +94,10 @@ class ClusterSimulation:
     configuration, intervals one per interval."""
 
     def __init__(self, endpoints, node_ids, K=10, H=9, L=4, seed=0, failure_threshold=FAILURE_THRESHOLD, fallback_intervals=1,
-                 device=0):
+                 device=0, batch_order="sender"):
+        if batch_order not in ("sender", "shuffled"):
+            raise ValueError("batch_order is 'sender' or 'shuffled', not %r" % (batch_order,))
+        self.batch_order = batch_order
         import torch                                              # device buffers of the scenario's flags
         self._torch = torch
         self.K, self.H, self.L, self.seed, self.device = int(K), int(H), int(L), int(seed), device
@@ -207,7 +216,7 @@ class ClusterSimulation:
     def _new_handles(self):
         n = self.view.n
         self.N = n
-        self.cl = VirtualCluster(self.view, self.H, self.L, kernel="bucketed")
+        self.cl = VirtualCluster(self.view, self.H, self.L, kernel="sweep" if self.batch_order == "shuffled" else "bucketed")
         self.acc = PaxosAcceptors(self.cfg, n, device=self.device)
         if self.fp is None or n > self._fp_cap:
             self.fp, self._fp_cap = FastPaxos(self.cfg, n, device=self.device), n
@@ -219,6 +228,7 @@ class ClusterSimulation:
         self.first_proposal = None
         self.votes = 0
         self.announced = 0
+        self.proposal_fps = set()                                 # (h1, h2, len) of every proposal announced in the configuration
         self._ann = None                                          # announcedProposal flags, read at most once per interval
         self._dirty = True
         self._cfg_t = {"detect_ms": 0.0, "classic_ms": 0.0, "view_change_ms": 0.0, "handles_ms": 0.0, "device_ms": 0.0}
@@ -258,13 +268,15 @@ class ClusterSimulation:
         if joiners or leavers:
             na, nc = self.fd.mergeAlerts(joiners, self._member_ids(leavers), cfg)
             dev_ms += self.fd.lastDeviceMs()
-        rec = {"cfg": cfg, "interval": i, "alerts": na, "cells": nc, "announced": 0, "event": "quiet", "leavers": len(leavers)}
+        rec = {"cfg": cfg, "interval": i, "alerts": na, "cells": nc, "announced": 0, "event": "quiet", "leavers": len(leavers),
+               "proposals": 0}
         decided = None
         if nc:
             rec["event"] = "alerts"
             p = self.fd.cellsDevice()
+            order = {"batch_order_seed" if self.batch_order == "shuffled" else "perm_seed": interval_seed(self.seed, cfg, i)}
             self.cl.handleBatchesDevice(cfg, nc, p[1], p[2], p[3], self.fd.senderBatches(), cell_cfg_dev=p[4],
-                                        blocked_dev=self.d_blocked.data_ptr(), perm_seed=interval_seed(self.seed, cfg, i))
+                                        blocked_dev=self.d_blocked.data_ptr(), **order)
             dev_ms += self.cl.lastDeviceMs()[0]
             self.acc.registerFastRoundVotesFrom(self.cl)
             t = self.fp.tallyCluster(self.cl)
@@ -274,6 +286,11 @@ class ClusterSimulation:
             rec["announced"] = int(self._announced_flags().sum()) - self.announced if t.decided else t.votes_received - self.votes
             self.votes = t.votes_received
             if rec["announced"]:
+                out = self.cl.readOutputs()                       # the proposals announced in this interval
+                now = out.proposal_len > 0
+                fps = set(zip(out.proposal_hash[now].tolist(), out.proposal_hash2[now].tolist(), out.proposal_len[now].tolist()))
+                rec["proposals"] = len(fps)
+                self.proposal_fps |= fps
                 rec["event"] = "proposals"
                 self.announced += rec["announced"]
                 if self.first_proposal is None:
@@ -292,6 +309,7 @@ class ClusterSimulation:
                 decided = ("classic", value)
         self._cfg_t["device_ms"] += dev_ms
         rec["device_ms"] = dev_ms
+        rec["host_ms"] = (time.perf_counter() - t0) * 1e3               # host clock of the whole interval, view change excluded
         self.interval_in_cfg += 1
         if decided is not None:
             rec["event"] = "decided-" + decided[0]
@@ -361,13 +379,13 @@ class ClusterSimulation:
         self.fd.reset()
         self.cl.close()
         self.acc.close()
-        times, announced, votes = self._cfg_t, self.announced, self.votes
+        times, announced, votes, distinct = self._cfg_t, self.announced, self.votes, len(self.proposal_fps)
         self._new_handles()
         self._register(self.pending)
         times["handles_ms"] += (time.perf_counter() - t1) * 1e3
         self.history.append({"cfg_before": before, "cfg_after": self.cfg, "size_before": size_before, "size": self.view.n,
                              "cut": cut_tags, "path": path, "intervals": i + 1, "announced": announced,
-                             "votes": votes, "members": sorted(self.tags.tolist()), **times})
+                             "votes": votes, "members": sorted(self.tags.tolist()), "distinct_proposals": distinct, **times})
 
     # ---- whole runs --------------------------------------------------------------------------------------------------------------
     def run(self, max_intervals):
