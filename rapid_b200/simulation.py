@@ -2,8 +2,7 @@
 (alert generation -> per-sender alert batches -> cut detection -> fast round -> classic fallback -> decideViewChange,
 MembershipService.java:300-354, :385-444, FastPaxos.java:94-203), composed from the classes of this package.
 
-ClusterSimulation rules (tests/simref.py restates them independently, tests/simref_leave.py the leave and rejoin rules; DESIGN.md
-§4.11):
+ClusterSimulation rules (tests/simref.py restates them independently; DESIGN.md §4.11):
 
 * Nodes are named by TAGS: the members given at creation are 0..n-1 in the given order, joiners get the next tags in the
   order addJoiners() lists them.  Tags never change; the device ids of a configuration are dense (view.applyCut renumbers),

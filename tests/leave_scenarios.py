@@ -1,15 +1,9 @@
-"""ClusterTest's leave and rejoin scenarios (ClusterTest.java:417-521) written once for any set of simulations run in lockstep:
-tests/simref_leave.py's LeaveRejoinSimulation alone (test_oracle_cluster_leave_rejoin.py) or together with the device's
-ClusterSimulation (test_gpu_cluster_leave_rejoin.py).  Every step is applied to every simulation; the scenario's own
-assertions are made on the first one, and the callers compare the runs.  NOT a pytest module."""
-import random
-
-import numpy as np
-
-from simref_leave import LeaveRejoinSimulation
+"""ClusterTest's leave and rejoin scenarios (ClusterTest.java:417-521) written once for the reference of tests/simref.py alone
+(test_oracle_cluster_leave_rejoin.py) or in lockstep with the device's ClusterSimulation (test_gpu_cluster_leave_rejoin.py),
+through simref's harness.  Every step is applied to every simulation; the scenario's own assertions are made on the first one,
+and the callers compare the runs.  NOT a pytest module."""
+from simref import CRASHED, flags, join, leave, make, random_hosts, rejoin, run, steps
 from rapid_b200 import workloads as W
-
-CRASHED = 1
 
 
 def fresh_id(k):
@@ -18,72 +12,21 @@ def fresh_id(k):
     return int(hi[0]), int(lo[0])
 
 
-def random_hosts(n, count, seed, lo=0):
-    return sorted(random.Random(seed).sample(range(lo, n), count))
-
-
-def make(orc, rb, n, seed, n_joiners=0):
-    """(oracle,) or (oracle, device) with members 0..n-1; joiners n..n+n_joiners-1 are known to the oracle and join by join_one"""
-    sims = [LeaveRejoinSimulation(orc, n, seed=seed, n_joiners=n_joiners)]
-    if rb is not None:
-        sims.append(rb.ClusterSimulation(W.packed_endpoints(0, n), W.node_ids(0, n), seed=seed))
-    return tuple(sims)
-
-
-def members(s):
-    return sorted(s.members if isinstance(s, LeaveRejoinSimulation) else s.members())
-
-
-def join_one(sims, t):
-    for s in sims:
-        if isinstance(s, LeaveRejoinSimulation):
-            s.addJoiners([t])
-        else:
-            hosts, ports = W.endpoints(t, 1)
-            assert s.addJoiners(hosts, ports, *W.node_ids(t, 1)) == [t]
-
-
-def flags(sims, tags, f):
-    for s in sims:
-        for t in tags:
-            s.setFlags(t, f)
-
-
-def leave(sims, tags):
-    for s in sims:
-        s.leave(tags)
-
-
-def rejoin(sims, tag, node_id):
-    for s in sims:
-        s.rejoin(tag, *node_id)
-
-
-def run(sims, max_intervals=30):
-    outs = [s.run(max_intervals) for s in sims]
-    assert all(o["converged"] for o in outs), outs
-    return outs[0]
-
-
-def steps(sims, count):
-    return [[s.interval() for s in sims][0] for _ in range(count)]
-
-
 # ---- the scenarios ---------------------------------------------------------------------------------------------------------------
 def leaving(orc, rb, seed=31):
     """testLeaving (:509-521): a cluster grown by single joins from 2 to 11 members; member 0 leaves, the other 10 agree on the
     cut [0], decided in the leave's interval"""
     sims = make(orc, rb, 2, seed, n_joiners=9)
     for t in range(2, 11):
-        join_one(sims, t)
+        join(sims, [t])
         run(sims)
-        assert members(sims[0]) == list(range(t + 1))
+        assert sorted(sims[0].members()) == list(range(t + 1))
     before = len(sims[0].history)
     leave(sims, [0])
     run(sims)
     h = sims[0].history[before:]
     assert [c["cut"] for c in h] == [[0]] and h[0]["intervals"] == 1 and h[0]["path"] == "fast"
-    assert members(sims[0]) == list(range(1, 11))
+    assert sorted(sims[0].members()) == list(range(1, 11))
     return sims
 
 
@@ -93,10 +36,10 @@ def rejoin_single_node(orc, rb, tag=3, seed=32):
     for rnd in range(2):
         flags(sims, [tag], CRASHED)
         run(sims)
-        assert tag not in members(sims[0]) and sims[0].history[-1]["cut"] == [tag]
+        assert tag not in sims[0].members() and sims[0].history[-1]["cut"] == [tag]
         rejoin(sims, tag, fresh_id(rnd))
         run(sims)
-        assert members(sims[0]) == list(range(10)) and sims[0].history[-1]["cut"] == [tag]
+        assert sorted(sims[0].members()) == list(range(10)) and sims[0].history[-1]["cut"] == [tag]
     return sims
 
 
@@ -118,7 +61,7 @@ def rejoin_same_configuration(orc, rb, tag=6, seed=33, refuse=True):
     assert sims[0].history[-1]["cut"] == [tag] and sims[0].history[-1]["intervals"] == 11
     rejoin(sims, tag, fresh_id(7))
     run(sims)
-    assert members(sims[0]) == list(range(10))
+    assert sorted(sims[0].members()) == list(range(10))
     return sims
 
 
@@ -134,11 +77,11 @@ def rejoin_multiple_nodes(orc, rb, mode, seed=34):
         else:
             leave(sims, gone)
         run(sims, 40)
-        assert members(sims[0]) == [t for t in range(n) if t not in gone]
+        assert sorted(sims[0].members()) == [t for t in range(n) if t not in gone]
         for j, t in enumerate(gone):
             rejoin(sims, t, fresh_id(100 * rnd + j))
         run(sims, 40)
-        assert members(sims[0]) == list(range(n))
+        assert sorted(sims[0].members()) == list(range(n))
     return sims
 
 
@@ -172,7 +115,7 @@ def adjacent_leavers(orc, rb, n=50, seed=36):
     o, y = adjacent_pair(sims[0].view, n, 5)
     leave(sims, [y, o])
     run(sims)
-    assert members(sims[0]) == [t for t in range(n) if t not in (o, y)]
+    assert sorted(sims[0].members()) == [t for t in range(n) if t not in (o, y)]
     return sims
 
 
@@ -189,7 +132,7 @@ def leaver_with_crashed_observers(orc, rb, n=100, tag=40, seed=37):
     h = sims[0].history
     assert sorted(t for c in h[:-1] for t in c["cut"]) == obs
     assert h[-1]["cut"] == [tag] and h[-1]["intervals"] == 11
-    assert members(sims[0]) == [t for t in range(n) if t not in obs and t != tag]
+    assert sorted(sims[0].members()) == [t for t in range(n) if t not in obs and t != tag]
     return sims
 
 
@@ -208,7 +151,7 @@ def refusals(orc, rb, seed=38, refuse=True):
     NodeId this simulation was given is refused, with a new one it is admitted"""
     n = 12
     sims = make(orc, rb, n, seed, n_joiners=1)
-    join_one(sims, n)
+    join(sims, [n])
     flags(sims, [4], CRASHED)
     hi, lo = W.node_ids(0, n + 1)
     if refuse:
@@ -218,7 +161,7 @@ def refusals(orc, rb, seed=38, refuse=True):
                          (n, fresh_id(2))):                                       # pending
             refused(sims, lambda s: s.rejoin(tag, *nid))
     run(sims)
-    assert members(sims[0]) == [t for t in range(n + 1) if t != 4]
+    assert sorted(sims[0].members()) == [t for t in range(n + 1) if t != 4]
     if refuse:
         for j in (n, 4, 9):                                                       # a joiner's, its own old one, a member's
             nid = (int(hi[j]), int(lo[j]))
@@ -226,5 +169,5 @@ def refusals(orc, rb, seed=38, refuse=True):
         refused(sims, lambda s: s.leave([4]))                                     # not a member any more
     rejoin(sims, 4, fresh_id(3))
     run(sims)
-    assert members(sims[0]) == list(range(n + 1))
+    assert sorted(sims[0].members()) == list(range(n + 1))
     return sims

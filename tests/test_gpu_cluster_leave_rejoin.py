@@ -1,30 +1,21 @@
 """Graceful leaves and rejoins on the device: rapid_fdet_merge_alerts (join and leave alerts merged into the failure-detector
 interval) on its own against the device view's getObserversOf / getRingNumbers; ClusterSimulation.leave / rejoin against
-tests/simref_leave.py interval by interval and configuration by configuration on ClusterTest's leave and rejoin scenarios
+tests/simref.py interval by interval and configuration by configuration on ClusterTest's leave and rejoin scenarios
 (leave_scenarios.py) and at 10^4 nodes; and, checked on their outcome, 1 % leaving at 10^6 nodes and rolling restarts at 10^5."""
 import numpy as np
 import pytest
 
 import leave_scenarios as S
+from simref import CRASHED, flags, leave, make, rejoin, run, same_run
 from rapid_b200 import workloads as W
 
 pytestmark = pytest.mark.gpu
-
-CRASHED = 1
-HISTORY_KEYS = ("cfg_before", "cfg_after", "size_before", "size", "cut", "path", "intervals", "announced", "votes", "members")
-INTERVAL_KEYS = ("cfg", "interval", "alerts", "cells", "announced", "event", "leavers")
 
 
 @pytest.fixture(scope="module")
 def rb():
     import rapid_b200
     return rapid_b200
-
-
-def assert_same_run(ref, dev):
-    assert [{k: r[k] for k in INTERVAL_KEYS} for r in dev.intervals] == [{k: r[k] for k in INTERVAL_KEYS} for r in ref.intervals]
-    assert [{k: h[k] for k in HISTORY_KEYS} for h in dev.history] == [{k: h[k] for k in HISTORY_KEYS} for h in ref.history]
-    assert sorted(dev.members()) == sorted(ref.members)
 
 
 # ---- the merge on its own ------------------------------------------------------------------------------------------------------
@@ -181,63 +172,63 @@ def test_join_alerts_is_the_merge_without_leavers(rb):
     assert (a.senderBatches() == b.senderBatches()).all()
 
 
-# ---- the driver against simref_leave ----------------------------------------------------------------------------------------------
+# ---- the driver against simref -----------------------------------------------------------------------------------------------------
 def test_leaving(orc, rb):
     ref, dev = S.leaving(orc, rb)
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
 
 
 def test_rejoin_single_node(orc, rb):
     ref, dev = S.rejoin_single_node(orc, rb)
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
 
 
 def test_rejoin_single_node_same_configuration(orc, rb):
     ref, dev = S.rejoin_same_configuration(orc, rb)
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
 
 
 @pytest.mark.parametrize("mode", ["crash", "leave"])
 def test_rejoin_multiple_nodes(orc, rb, mode):
     ref, dev = S.rejoin_multiple_nodes(orc, rb, mode)
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
 
 
 @pytest.mark.parametrize("how", ["leave", "crash"])
 def test_leave_against_crash_on_the_same_draw(orc, rb, how):
     ref, dev = S.leave_against_crash(orc, rb, how)
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
 
 
 def test_adjacent_leavers(orc, rb):
     ref, dev = S.adjacent_leavers(orc, rb)
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
 
 
 def test_leaver_whose_observers_crashed(orc, rb):
     ref, dev = S.leaver_with_crashed_observers(orc, rb)
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
 
 
 def test_refusals(orc, rb):
     ref, dev = S.refusals(orc, rb)
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
 
 
 def test_ten_thousand_nodes_leaves_rejoins_and_crashes(orc, rb):
     n = 10_000
-    sims = S.make(orc, rb, n, 41)
+    sims = make(orc, rb, n, 41)
     drawn = W.pick_smallest(n, n // 100, 41).tolist()
     gone, crashed = drawn[::2], drawn[1::2]
-    S.flags(sims, crashed, CRASHED)
-    S.leave(sims, gone)
-    S.run(sims, 15)
-    assert S.members(sims[1]) == sorted(set(range(n)) - set(drawn))
+    flags(sims, crashed, CRASHED)
+    leave(sims, gone)
+    run(sims, 15)
+    assert sorted(sims[1].members()) == sorted(set(range(n)) - set(drawn))
     for j, t in enumerate(drawn):
-        S.rejoin(sims, t, S.fresh_id(j))
-    S.run(sims, 15)
-    assert S.members(sims[1]) == list(range(n))
-    assert_same_run(*sims)
+        rejoin(sims, t, S.fresh_id(j))
+    run(sims, 15)
+    assert sorted(sims[1].members()) == list(range(n))
+    same_run(*sims)
 
 
 # ---- at scale ----------------------------------------------------------------------------------------------------------------------

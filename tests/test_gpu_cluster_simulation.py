@@ -8,19 +8,15 @@ receiver by receiver against an oracle window: the deciding interval's cut-detec
 interval(), and replaying 10^4-10^5 sender batches through the oracle per interval is beyond a test's time.  Receiver-level
 parity of the same kernels at these sizes is held by test_gpu_cut_detection.py, test_gpu_full_scale.py and test_gpu_tally_cd.py,
 and of the whole driver by the 10^4-node comparison with simref here."""
-import random
-
 import numpy as np
 import pytest
 
-from simref import OracleSimulation
+from simref import CRASHED, flags, join, make, random_hosts, run, same_run
 from rapid_b200 import workloads as W
 
 pytestmark = pytest.mark.gpu
 
-CRASHED, INGRESS_BLOCKED = 1, 2
-HISTORY_KEYS = ("cfg_before", "cfg_after", "size_before", "size", "cut", "path", "intervals", "announced", "votes", "members")
-INTERVAL_KEYS = ("cfg", "interval", "alerts", "cells", "announced", "event")
+INGRESS_BLOCKED = 2
 
 
 @pytest.fixture(scope="module")
@@ -29,46 +25,12 @@ def rb():
     return rapid_b200
 
 
-def random_hosts(n, count, seed, lo=0):
-    return sorted(random.Random(seed).sample(range(lo, n), count))
-
-
-def device_sim(rb, n, seed, n_joiners=0, **kw):
-    s = rb.ClusterSimulation(W.packed_endpoints(0, n), W.node_ids(0, n), seed=seed, **kw)
-    if n_joiners:
-        hosts, ports = W.endpoints(n, n_joiners)
-        hi, lo = W.node_ids(n, n_joiners)
-        assert s.addJoiners(hosts, ports, hi, lo) == list(range(n, n + n_joiners))
-    return s
-
-
-def pair(orc, rb, n, seed, n_joiners=0):
-    ref = OracleSimulation(orc, n, seed=seed, n_joiners=n_joiners)
-    dev = device_sim(rb, n, seed, n_joiners)
-    if n_joiners:
-        ref.addJoiners(range(n, n + n_joiners))
-    return ref, dev
-
-
-def set_flags(sims, tags, flag):
-    for s in sims:
-        for t in tags:
-            s.setFlags(t, flag)
-
-
-def assert_same_run(ref, dev):
-    assert [{k: r[k] for k in INTERVAL_KEYS} for r in dev.intervals] == [{k: r[k] for k in INTERVAL_KEYS} for r in ref.intervals]
-    assert [{k: h[k] for k in HISTORY_KEYS} for h in dev.history] == [{k: h[k] for k in HISTORY_KEYS} for h in ref.history]
-    assert sorted(dev.members()) == sorted(ref.members)
-
-
 # ---- ClusterTest's scenarios, device vs simref ---------------------------------------------------------------------------------
 def test_one_failure_out_of_five_nodes(orc, rb):
-    ref, dev = pair(orc, rb, 5, 1)
-    set_flags((ref, dev), [2], CRASHED)
-    a, b = ref.run(20), dev.run(20)
-    assert a["converged"] and b["converged"]
-    assert_same_run(ref, dev)
+    ref, dev = sims = make(orc, rb, 5, 1)
+    flags(sims, [2], CRASHED)
+    run(sims, 20)
+    same_run(ref, dev)
     assert dev.members() == [0, 1, 3, 4] and [h["path"] for h in dev.history] == ["fast"]
 
 
@@ -77,11 +39,10 @@ def test_one_failure_out_of_five_nodes(orc, rb):
                                             (50, 10, 9, INGRESS_BLOCKED), (50, 10, 10, INGRESS_BLOCKED)])
 def test_failure_scenarios(orc, rb, n, f, seed, flag):                            # ClusterTest.java:275-336
     failing = random_hosts(n, f, seed)
-    ref, dev = pair(orc, rb, n, seed)
-    set_flags((ref, dev), failing, flag)
-    a, b = ref.run(30), dev.run(30)
-    assert a["converged"] and b["converged"]
-    assert_same_run(ref, dev)
+    ref, dev = sims = make(orc, rb, n, seed)
+    flags(sims, failing, flag)
+    run(sims)
+    same_run(ref, dev)
     assert dev.members() == [m for m in range(n) if m not in failing]
     if f == 16:
         assert dev.history[0]["path"] == "classic"                               # 34 voters < 38
@@ -90,25 +51,26 @@ def test_failure_scenarios(orc, rb, n, f, seed, flag):                          
 @pytest.mark.parametrize("seed", [13, 14, 15])
 def test_concurrent_node_joins_and_fails(orc, rb, seed):                         # :228-243
     n, nj = 30, 10
-    ref, dev = pair(orc, rb, n, seed, n_joiners=nj)
-    set_flags((ref, dev), range(2, 7), CRASHED)
-    assert ref.run(30)["converged"] and dev.run(30)["converged"]
-    assert_same_run(ref, dev)
+    ref, dev = sims = make(orc, rb, n, seed, n_joiners=nj)
+    join(sims, range(n, n + nj))
+    flags(sims, range(2, 7), CRASHED)
+    run(sims)
+    same_run(ref, dev)
     assert sorted(dev.members()) == sorted([m for m in range(n) if not 2 <= m < 7] + list(range(n, n + nj)))
 
 
 def test_inject_asymmetric_drops(orc, rb):                                       # :342-360
     n = 50
     failing = random_hosts(n, 10, seed=12, lo=1)
-    ref, dev = pair(orc, rb, n, 12)
-    set_flags((ref, dev), failing, INGRESS_BLOCKED)
+    ref, dev = sims = make(orc, rb, n, 12)
+    flags(sims, failing, INGRESS_BLOCKED)
     for _ in range(10):
         assert dev.interval()["event"] == ref.interval()["event"] == "quiet"
-    set_flags((ref, dev), failing, 0)
+    flags(sims, failing, 0)
     while not ref.history:
         ref.interval()
         dev.interval()
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
     assert dev.history[0]["cut"] == failing and dev.history[0]["path"] == "fast"
 
 
@@ -116,7 +78,7 @@ def test_edge_failures(orc, rb):
     """the probes of every observer of one live node fail (setEdgeFail on the detector that watches it): it is cut although
     alive, on the device as in simref"""
     n, y = 50, 7
-    ref, dev = pair(orc, rb, n, 16)
+    ref, dev = make(orc, rb, n, 16)
     obs = ref.view.getObserversOf(y)
     assert obs == dev.view.getObserversOf(y)
     for s in (ref, dev):
@@ -125,18 +87,18 @@ def test_edge_failures(orc, rb):
     while not ref.history:
         assert ref.interval()["event"] != "stalled" and len(ref.intervals) < 15
         dev.interval()
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
     assert dev.history[0]["cut"] == [y] and dev.history[0]["path"] == "fast" and dev.history[0]["intervals"] == 11
 
 
 def test_a_stalling_draw_is_reported(orc, rb):
     n, f, seed = 50, 16, 131
     failing = random_hosts(n, f, seed)
-    ref, dev = pair(orc, rb, n, seed)
-    set_flags((ref, dev), failing, CRASHED)
+    ref, dev = sims = make(orc, rb, n, seed)
+    flags(sims, failing, CRASHED)
     a, b = ref.run(15), dev.run(15)
     assert b["stalled"] and b["stuck"] == a["stuck"] == failing and b["intervals"] == 15
-    assert_same_run(ref, dev)
+    same_run(ref, dev)
 
 
 # ---- the primitives ------------------------------------------------------------------------------------------------------------
@@ -246,10 +208,10 @@ def test_silent_acceptors(rb):
 def test_ten_thousand_nodes_against_simref(orc, rb):
     n = 10_000
     crashed = W.pick_smallest(n, n // 100, 21).tolist()
-    ref, dev = pair(orc, rb, n, 21)
-    set_flags((ref, dev), crashed, CRASHED)
-    assert ref.run(15)["converged"] and dev.run(15)["converged"]
-    assert_same_run(ref, dev)
+    ref, dev = sims = make(orc, rb, n, 21)
+    flags(sims, crashed, CRASHED)
+    run(sims, 15)
+    same_run(ref, dev)
 
 
 def _no_dark_draw(obs, n, frac, seed, L=4):
@@ -279,9 +241,9 @@ def _no_dark_draw(obs, n, frac, seed, L=4):
 def test_hundred_thousand_nodes_churn(rb):
     n, nj = 100_000, 200
     crashed = W.pick_smallest(n, n // 100, 22).tolist()
-    s = device_sim(rb, n, 22, n_joiners=nj)
-    for t in crashed:
-        s.setFlags(t, CRASHED)
+    s = rb.ClusterSimulation(W.packed_endpoints(0, n), W.node_ids(0, n), seed=22)
+    join((s,), range(n, n + nj))
+    flags((s,), crashed, CRASHED)
     out = s.run(15)
     assert out["converged"]
     assert sorted(s.members()) == sorted(set(range(n)) - set(crashed) | set(range(n, n + nj)))
@@ -300,9 +262,8 @@ def test_ten_thousand_nodes_thirty_percent_crashed(rb):
     v.close()
     crashed = _no_dark_draw(obs, n, 0.30, 23)
     assert len(crashed) == 3_000
-    s = device_sim(rb, n, 23)
-    for t in crashed:
-        s.setFlags(t, CRASHED)
+    s = rb.ClusterSimulation(W.packed_endpoints(0, n), W.node_ids(0, n), seed=23)
+    flags((s,), crashed, CRASHED)
     out = s.run(15)
     assert out["converged"] and sorted(s.members()) == sorted(set(range(n)) - set(crashed))
     h = s.history
@@ -317,9 +278,8 @@ def test_one_million_nodes_one_percent_crashed(rb):
     """the Fig. 8 shape at 10^6: one fast-path view change whose cut is the crashed set"""
     n = 1_000_000
     crashed = W.pick_smallest(n, n // 100, 24).tolist()
-    s = device_sim(rb, n, 24)
-    for t in crashed:
-        s.setFlags(t, CRASHED)
+    s = rb.ClusterSimulation(W.packed_endpoints(0, n), W.node_ids(0, n), seed=24)
+    flags((s,), crashed, CRASHED)
     out = s.run(15)
     assert out["converged"] and len(s.history) == 1
     h = s.history[0]

@@ -1,14 +1,12 @@
 """RAPID_DELIVERY_SHUFFLED_BATCHES on the device: the sweep kernel's per-receiver batch order (k_sweep<true>) against the oracle's
 literal handlers walked in the same order (tests/shuffled_ref.py) receiver by receiver; the flag's refusals; and
-ClusterSimulation(batch_order="shuffled") against tests/simref_shuffled.py, record by record."""
-import random
-
+ClusterSimulation(batch_order="shuffled") against tests/simref.py, record by record."""
 import numpy as np
 import pytest
 
 import shuffled_ref as S
 from helpers import OracleWorld
-from simref_shuffled import ShuffledSimulation
+from simref import CRASHED, flags, join, leave, make, random_hosts, run, same_run
 from rapid_b200 import workloads as W
 
 pytestmark = pytest.mark.gpu
@@ -156,41 +154,14 @@ def test_refusals_change_nothing(rb, world):
     assert any(m for m, _, _ in raw_state)
 
 
-# ---- ClusterSimulation(batch_order="shuffled") against simref_shuffled ------------------------------------------------------------
-HISTORY_KEYS = ("cfg_before", "cfg_after", "size_before", "size", "cut", "path", "intervals", "announced", "votes", "members",
-                "distinct_proposals")
-INTERVAL_KEYS = ("cfg", "interval", "alerts", "cells", "announced", "event", "leavers", "proposals")
-
-
-def pair(orc, rb, n, seed, n_joiners=0, batch_order="shuffled"):
-    ref = ShuffledSimulation(orc, n, seed=seed, n_joiners=n_joiners, batch_order=batch_order)
-    dev = rb.ClusterSimulation(W.packed_endpoints(0, n), W.node_ids(0, n), seed=seed, batch_order=batch_order)
-    if n_joiners:
-        hosts, ports = W.endpoints(n, n_joiners)
-        hi, lo = W.node_ids(n, n_joiners)
-        dev.addJoiners(hosts, ports, hi, lo)
-        ref.addJoiners(range(n, n + n_joiners))
-    return ref, dev
-
-
-def same_run(ref, dev):
-    assert [{k: r[k] for k in INTERVAL_KEYS} for r in dev.intervals] == [{k: r[k] for k in INTERVAL_KEYS} for r in ref.intervals]
-    assert [{k: h[k] for k in HISTORY_KEYS} for h in dev.history] == [{k: h[k] for k in HISTORY_KEYS} for h in ref.history]
-    assert sorted(dev.members()) == sorted(ref.members)
-
-
-def crash(sims, tags, flag=1):
-    for s in sims:
-        for t in tags:
-            s.setFlags(t, flag)
-
-
+# ---- ClusterSimulation(batch_order="shuffled") against simref ---------------------------------------------------------------------
 @pytest.mark.parametrize("n,f,seed,flag,nj", [(5, 1, 1, 1, 0), (50, 12, 3, 1, 0), (50, 16, 6, 1, 0), (50, 10, 9, 2, 0),
                                                (30, 5, 13, 1, 10), (1000, 10, 21, 1, 0)])
 def test_cluster_scenarios_shuffled(orc, rb, n, f, seed, flag, nj):
-    failing = [2] if n == 5 else sorted(random.Random(seed).sample(range(n), f))
-    ref, dev = pair(orc, rb, n, seed, nj)
-    crash((ref, dev), failing, flag)
+    failing = [2] if n == 5 else random_hosts(n, f, seed)
+    ref, dev = sims = make(orc, rb, n, seed, nj, batch_order="shuffled")
+    join(sims, range(n, n + nj))
+    flags(sims, failing, flag)
     a, b = ref.run(30), dev.run(30)
     assert a["converged"] == b["converged"]
     same_run(ref, dev)
@@ -198,28 +169,28 @@ def test_cluster_scenarios_shuffled(orc, rb, n, f, seed, flag, nj):
 
 @pytest.mark.parametrize("n,f,seed,nj", [(50, 16, 6, 0), (30, 5, 13, 10)])
 def test_cluster_scenarios_sender_mode_records(orc, rb, n, f, seed, nj):
-    """the new record keys in the default mode, against simref_shuffled(batch_order="sender")"""
-    failing = sorted(random.Random(seed).sample(range(n), f))
-    ref, dev = pair(orc, rb, n, seed, nj, batch_order="sender")
-    crash((ref, dev), failing)
-    assert ref.run(30)["converged"] and dev.run(30)["converged"]
+    """the new record keys in the default mode, against simref(batch_order="sender")"""
+    failing = random_hosts(n, f, seed)
+    ref, dev = sims = make(orc, rb, n, seed, nj, batch_order="sender")
+    join(sims, range(n, n + nj))
+    flags(sims, failing, CRASHED)
+    run(sims)
     same_run(ref, dev)
 
 
 def test_ten_thousand_nodes_shuffled(orc, rb):
     n, seed = 10_000, 21
     failing = W.pick_smallest(n, n // 100, seed).tolist()
-    ref, dev = pair(orc, rb, n, seed)
-    crash((ref, dev), failing)
-    assert ref.run(15)["converged"] and dev.run(15)["converged"]
+    ref, dev = sims = make(orc, rb, n, seed, batch_order="shuffled")
+    flags(sims, failing, CRASHED)
+    run(sims, 15)
     same_run(ref, dev)
 
 
 def test_leave_shuffled(orc, rb):
-    ref, dev = pair(orc, rb, 50, 31)
-    for s in (ref, dev):
-        s.leave([4, 17])
-    assert ref.run(30)["converged"] and dev.run(30)["converged"]
+    ref, dev = sims = make(orc, rb, 50, 31, batch_order="shuffled")
+    leave(sims, [4, 17])
+    run(sims)
     same_run(ref, dev)
     assert 4 not in dev.members() and 17 not in dev.members()
 
@@ -228,10 +199,10 @@ def test_conflicting_proposals_go_to_the_classic_round(orc, rb):
     """the behaviour the mode exists for: receivers that meet the batches in different orders announce three different cuts, no
     fast quorum forms, and the classic round decides"""
     n, seed = 50, 12
-    failing = sorted(random.Random(seed).sample(range(n), 12))
-    ref, dev = pair(orc, rb, n, seed)
-    crash((ref, dev), failing)
-    assert ref.run(30)["converged"] and dev.run(30)["converged"]
+    failing = random_hosts(n, 12, seed)
+    ref, dev = sims = make(orc, rb, n, seed, batch_order="shuffled")
+    flags(sims, failing, CRASHED)
+    run(sims)
     same_run(ref, dev)
     assert dev.history[0]["distinct_proposals"] == 3 and dev.history[0]["path"] == "classic"
     assert max(r["proposals"] for r in dev.intervals) >= 2

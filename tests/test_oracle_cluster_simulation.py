@@ -3,29 +3,18 @@
 with the real ping-pong detectors (FdSim) raising the alerts, joins through the failure-detector interval, the seeded
 fallback and the configuration-by-configuration view change.  test_gpu_cluster_simulation.py checks the device driver
 against the same runs."""
-import random
-
 import pytest
 
-from simref import OracleSimulation
+from simref import CRASHED, OracleSimulation, flags, random_hosts
 
-CRASHED, INGRESS_BLOCKED = 1, 2
-
-
-def random_hosts(n, count, seed, lo=0):
-    return sorted(random.Random(seed).sample(range(lo, n), count))
-
-
-def crash(s, tags, flag=CRASHED):
-    for t in tags:
-        s.setFlags(t, flag)
+INGRESS_BLOCKED = 2
 
 
 def test_one_failure_out_of_five_nodes(orc):                                     # ClusterTest.java:212-224
     s = OracleSimulation(orc, 5, seed=1)
-    crash(s, [2])
+    flags((s,), [2], CRASHED)
     out = s.run(20)
-    assert out["converged"] and s.members == [0, 1, 3, 4]
+    assert out["converged"] and s.members() == [0, 1, 3, 4]
     assert [h["path"] for h in s.history] == ["fast"] and s.history[0]["cut"] == [2]
     assert s.history[0]["intervals"] == 11                                        # ten failed probes, the notification on the 11th
 
@@ -35,9 +24,9 @@ def test_fail_random_quarter_of_nodes(orc, seed):                               
     n, f = 50, 12
     failing = random_hosts(n, f, seed)
     s = OracleSimulation(orc, n, seed=seed)
-    crash(s, failing)
+    flags((s,), failing, CRASHED)
     out = s.run(30)
-    assert out["converged"] and s.members == [m for m in range(n) if m not in failing]
+    assert out["converged"] and s.members() == [m for m in range(n) if m not in failing]
     assert s.view.getMembershipSize() == n - f
     assert sorted(t for h in s.history for t in h["cut"]) == failing
 
@@ -47,10 +36,11 @@ def test_fail_random_third_of_nodes(orc, seed):                                 
     n, f = 50, 16
     failing = random_hosts(n, f, seed)
     s = OracleSimulation(orc, n, seed=seed)
-    crash(s, failing)
+    flags((s,), failing, CRASHED)
     out = s.run(30)
-    assert out["converged"] and s.members == [m for m in range(n) if m not in failing]
+    assert out["converged"] and s.members() == [m for m in range(n) if m not in failing]
     assert s.history[0]["path"] == "classic"                                     # 34 voters < 38: the fallback decides
+    assert all(h["distinct_proposals"] >= 1 for h in s.history)
 
 
 @pytest.mark.parametrize("seed", [9, 10])
@@ -58,9 +48,9 @@ def test_fail_ten_random_nodes_that_stay_alive(orc, seed):                      
     n, f = 50, 10
     failing = random_hosts(n, f, seed)
     s = OracleSimulation(orc, n, seed=seed)
-    crash(s, failing, INGRESS_BLOCKED)                                           # alive and voting; nobody answers their probes
+    flags((s,), failing, INGRESS_BLOCKED)                                        # alive and voting; nobody answers their probes
     out = s.run(30)
-    assert out["converged"] and s.members == [m for m in range(n) if m not in failing]
+    assert out["converged"] and s.members() == [m for m in range(n) if m not in failing]
     assert all(h["path"] == "fast" for h in s.history)
 
 
@@ -70,26 +60,27 @@ def test_concurrent_node_joins_and_fails(orc, seed):                            
     failing = list(range(2, 2 + f))
     joiners = list(range(n, n + nj))
     s = OracleSimulation(orc, n, seed=seed, n_joiners=nj)
-    crash(s, failing)
+    flags((s,), failing, CRASHED)
     s.addJoiners(joiners)
     out = s.run(30)
     assert out["converged"]
-    assert sorted(s.members) == sorted([m for m in range(n) if m not in failing] + joiners)
+    assert sorted(s.members()) == sorted([m for m in range(n) if m not in failing] + joiners)
     assert s.view.getMembershipSize() == n - f + nj
+    assert all(h["distinct_proposals"] >= 1 for h in s.history)
 
 
 def test_inject_asymmetric_drops(orc):                                           # :342-360
     n, f = 50, 10
     failing = random_hosts(n, f, seed=12, lo=1)
     s = OracleSimulation(orc, n, seed=12)
-    crash(s, failing, INGRESS_BLOCKED)
+    flags((s,), failing, INGRESS_BLOCKED)
     for _ in range(10):
         assert s.interval()["event"] == "quiet"
-    crash(s, failing, 0)                                                         # the drops end; the detectors have counted ten
+    flags((s,), failing, 0)                                                      # the drops end; the detectors have counted ten
     while not s.history:
         assert s.interval()["event"] != "stalled" and s.i < 5
     assert s.history[0]["cut"] == failing and s.history[0]["path"] == "fast"
-    assert s.members == [m for m in range(n) if m not in failing]
+    assert s.members() == [m for m in range(n) if m not in failing]
 
 
 def test_edge_failures_cut_a_live_node(orc):
@@ -102,7 +93,7 @@ def test_edge_failures_cut_a_live_node(orc):
     while not s.history:
         assert s.interval()["event"] != "stalled" and s.i < 15
     assert s.history[0]["cut"] == [y] and s.history[0]["path"] == "fast" and s.history[0]["intervals"] == 11
-    assert s.members == [m for m in range(n) if m != y]
+    assert s.members() == [m for m in range(n) if m != y]
 
 
 def test_a_third_of_the_nodes_can_block_the_cut(orc):
@@ -111,7 +102,7 @@ def test_a_third_of_the_nodes_can_block_the_cut(orc):
     n, f, seed = 50, 16, 131
     failing = random_hosts(n, f, seed)
     s = OracleSimulation(orc, n, seed=seed)
-    crash(s, failing)
+    flags((s,), failing, CRASHED)
     out = s.run(15)
     assert out["stalled"] and not out["converged"] and out["stuck"] == failing
     assert s.history == [] and out["intervals"] == 15

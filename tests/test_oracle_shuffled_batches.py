@@ -1,7 +1,6 @@
 """RAPID_DELIVERY_SHUFFLED_BATCHES on the CPU: the batch order P_g (include/rapid_b200.h) restated three times (NumPy, plain
 Python, and the C++ next to the oracle's handlers) and checked to be a permutation with uniform small cases; the shuffled delivery over the oracle's handlers (tests/shuffled_ref.py) against
-independent pyref.PyBatchHandlers fed batch by batch in each receiver's order; and tests/simref_shuffled.py in "sender" mode
-against tests/simref.py on ClusterTest's scenarios."""
+independent pyref.PyBatchHandlers fed batch by batch in each receiver's order."""
 import itertools
 import random
 
@@ -11,8 +10,6 @@ import pytest
 import pyref
 import shuffled_ref as S
 from helpers import OracleWorld
-from simref import OracleSimulation
-from simref_shuffled import ShuffledSimulation
 from test_oracle_vs_python_restatement import same_reports
 
 K = 10
@@ -102,28 +99,3 @@ def test_shuffled_delivery_against_python_handlers(orc, seed):
             for t in failed + [n]:
                 assert same_reports(sim.reportMask(r, t), py[r].cd.reportMask(t), H)
 
-
-HISTORY_KEYS = ("cfg_before", "cfg_after", "size_before", "size", "cut", "path", "intervals", "announced", "votes", "members")
-INTERVAL_KEYS = ("cfg", "interval", "alerts", "cells", "announced", "event")
-
-
-def _crash(sims, tags, flag=1):
-    for s in sims:
-        for t in tags:
-            s.setFlags(t, flag)
-
-
-@pytest.mark.parametrize("n,f,seed,flag,nj", [(5, 1, 1, 1, 0), (50, 12, 3, 1, 0), (50, 16, 6, 1, 0), (50, 10, 9, 2, 0),
-                                               (30, 5, 13, 1, 10)])
-def test_sender_mode_runs_as_simref(orc, n, f, seed, flag, nj):
-    a = OracleSimulation(orc, n, seed=seed, n_joiners=nj)
-    b = ShuffledSimulation(orc, n, seed=seed, n_joiners=nj, batch_order="sender")
-    failing = sorted(random.Random(seed).sample(range(n), f)) if n > 5 else [2]
-    _crash((a, b), failing, flag)
-    if nj:
-        a.addJoiners(range(n, n + nj))
-        b.addJoiners(range(n, n + nj))
-    assert a.run(30) == b.run(30)
-    assert [{k: r[k] for k in INTERVAL_KEYS} for r in a.intervals] == [{k: r[k] for k in INTERVAL_KEYS} for r in b.intervals]
-    assert [{k: h[k] for k in HISTORY_KEYS} for h in a.history] == [{k: h[k] for k in HISTORY_KEYS} for h in b.history]
-    assert all(h["distinct_proposals"] >= 1 for h in b.history)
