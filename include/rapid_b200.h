@@ -51,8 +51,8 @@ extern "C" {
 #define RAPID_EDGE_UP   0   /* rapid.proto EdgeStatus */
 #define RAPID_EDGE_DOWN 1
 
-#define RAPID_MAX_K 14      /* ring-report bits 0..13 of the logical 16-bit per-(subject,receiver) state word (stored in 12 bits
-                               per receiver by bucketed handles when K <= 10, in 16 otherwise) */
+#define RAPID_MAX_K 14      /* ring-report bits 0..13 of the logical 16-bit per-(subject,receiver) state word (bucketed handles
+                               store the ring bits only: 10 bits per receiver when K <= 10, 16 otherwise) */
 
 typedef struct rapid_view rapid_view;   /* MembershipView: K rings in HBM (SoA)                       */
 typedef struct rapid_cd   rapid_cd;     /* MultiNodeCutDetector state of R virtual nodes in HBM       */

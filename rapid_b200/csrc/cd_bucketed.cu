@@ -3,9 +3,9 @@
 // Reference semantics: MultiNodeCutDetector.java:84-128 applied per cell in arrival order, then :137-164, driven
 // by MembershipService.java:300-354.  The Java walks the batch once per process and probes a hash map per cell.
 // Here the batch is regrouped BY SUBJECT once (counting sort by subject slot inside cd_prepare.cu), and every receiver's
-// state word for a subject (12 bits at K <= 10, see RowRef) is read ONCE, updated in a register and written ONCE:
+// state word for a subject (10 ring bits at K <= 10, see RowRef) is read ONCE, updated in a register and written ONCE:
 //
-//   traffic = 3 bytes x (#subjects in the batch) x (#receivers)          (SURVEY.md §8d "4·S·R" with 16-bit words)
+//   traffic = 2.5 bytes x (#subjects in the batch) x (#receivers)        (SURVEY.md §8d "4·S·R" with 16-bit words)
 //
 // instead of 4 bytes x #cells x #receivers for a per-cell sweep.  What makes that legal is that the sequential
 // rule "emit when updatesInProgress returns to 0" only depends on, per subject, the two moments at which its
@@ -33,7 +33,7 @@
 //   k_finalize1            classification per receiver (EMIT_ALL / NOEMIT / MIXED) from the partial accumulators
 //   k_mixed_flip           cooperative, always launched: [moments on demand] -> [interval analysis to its fixpoint] -> row flip
 //   k_inval_finalize2      invalidateFailingEdges over the work list + the receivers' closing bookkeeping
-//   k_marks                cooperative, returns at once unless some receiver went through the interval analysis: bit-15 marks,
+//   k_marks                cooperative, returns at once unless some receiver went through the interval analysis: emit marks,
 //                          counter snapshot
 #include <cooperative_groups.h>
 
@@ -345,8 +345,8 @@ struct ApplyArgs {
 __device__ __forceinline__ void note_unresolved(const ApplyArgs& a, int tile, int32_t slot) { worklist_note(a.wl, tile, slot); }
 
 // ---- uniform delivery: every active receiver gets every valid cell in array order -------------------------------------
-// One thread owns 8 consecutive receivers: per subject one group load and one group store (RowRef: 64-bit lo plane + 32-bit hi
-// plane at HB = 4, so a warp writes one whole 256-byte and one whole 128-byte line).  The common case is
+// One thread owns 8 consecutive receivers: per subject one group load and one group store (RowRef: 64-bit lo plane + 16-bit hi
+// plane at HB = 2, so a warp writes 256 + 64 bytes, all of them whole 32-byte sectors).  The common case is
 // that all of a thread's ACTIVE receivers hold the same state for the subject (they saw the same history): the
 // visit is computed once, merged into the new word with a SWAR mask, and accumulated in registers ("com").  Only
 // when active neighbours disagree (partitions) do we fall back to a per-receiver visit whose accumulators live in
@@ -618,7 +618,7 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
                         uint32_t at_last = sst;
                         const bool mun = visit_acc<PERM, SEQ>(m, sst & RM, d, &sw[PERM ? 0 : t], &spw[SEQ ? t : 0], RM, L, H, nullptr, 0u, seq_last, &at_last);
                         s_mst[t] = sst;
-                        s_mrep[t] = group8_rep<HB>((SEQ ? (at_last | (sst & ~RM)) : sst) | s_nw[t]);
+                        s_mrep[t] = group8_rep<HB>((SEQ ? at_last : sst) | s_nw[t]);
                         s_mun[t] = mun ? 1 : 0;
                         memo = true;
                     }
@@ -728,7 +728,7 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
                 } else if (same) {
                     uint32_t at_last = st;
                     unres = visit_acc<PERM, SEQ>(com, st & RM, d, &sw[PERM ? 0 : i], &spw[SEQ ? i : 0], RM, L, H, u, umask, seq_last, &at_last);
-                    group8_merge<HB>(w, group8_rep<HB>((SEQ ? (at_last | (st & ~RM)) : st) | s_nw[i]), am);
+                    group8_merge<HB>(w, group8_rep<HB>((SEQ ? at_last : st) | s_nw[i]), am);
                 } else {
                     if (!had_exc) {
                         had_exc = true;
@@ -938,7 +938,7 @@ __global__ void __launch_bounds__(GEN_THREADS, 4) k_apply_generic(const ApplyArg
                     st |= v.have;
                 }
                 // (r < Rpad holds for the whole grid: every lane of the warp takes part in the store)
-                if (a.rows.hb == 4) row_store1_warp<4>(a.rows, s_dst[i], r, st);
+                if (a.rows.hb == 2) row_store1_warp<2>(a.rows, s_dst[i], r, st);
                 else row_store1_warp<8>(a.rows, s_dst[i], r, st);
             }
             if (__any_sync(0xffffffffu, unres) && (t & 31) == 0 && s_unres[i] == 0) s_unres[i] = 1;
@@ -969,11 +969,13 @@ __global__ void __launch_bounds__(GEN_THREADS, 4) k_apply_generic(const ApplyArg
 //   flip        the rows written by the apply kernel become current
 //   inval       invalidateFailingEdges over the (tile, subject) work list
 //   finalize2   emissions of the invalidation pass, announced flags
-//   [marks]     bit 15 for receivers that announced only the explicit part
+//   [marks]     emit marks for receivers that announced only the explicit part
 //   tail        the last block snapshots the batch counters for the host and resets the per-batch fields
 // ==================================================================================================================
 struct ResolveArgs {
     ApplyArgs ap;
+    MarkPlane emit;               // bit 15 of the logical words (see MarkPlane)
+    MarkPlane trans;              // bit 14: raised by this batch's invalidation pass
     BatchCounts* bc;
     BatchCounts* snap;
     int n_chunks;                 // subject chunks of the apply launch (layout of the partials)
@@ -1329,8 +1331,8 @@ __device__ __noinline__ bool emitted_in_batch(const ResolveArgs& e, int32_t s, i
     const ApplyArgs& a = e.ap;
     const uint32_t RM = (1u << a.K) - 1u;
     // untouched by the batch: it left (with the first explicit proposal) iff it was pending, i.e. at >= H and NOT raised there by
-    // this batch's invalidation pass (bit 14, cleared by the unmark phase once the batch is done)
-    if (e.touch[s] != e.serial) return __popc(w_new & RM) >= a.H && !(w_new & CD_BIT_CALL);
+    // this batch's invalidation pass (the transient plane, cleared by the unmark phase once the batch is done)
+    if (e.touch[s] != e.serial) return __popc(w_new & RM) >= a.H && !e.trans.test(s, r);
     const int b = e.batch_index[s];
     const SubjDesc d = a.desc[b];
     const uint32_t old = seq_state(a, d, b, r, (s >= a.bc->S_before ? 0u : a.rows.get(a.rows.alt_lo(s), r)) & RM, true, true);
@@ -1473,9 +1475,13 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
 #pragma unroll
                             for (int j = 0; j < 4; ++j) {
                                 if (!((miss[j] >> k) & 1u)) continue;
-                                if ((wo[j] & CD_BIT_EMIT) || __popc(wo[j] & RM) < a.L) continue;   // observer not in proposal U preProposal
+                                // observer not in proposal U preProposal.  (No observer here has left in an emitted proposal of an
+                                // EARLIER batch: only a receiver that announced holds emit marks, it is frozen from then on, and a
+                                // receiver in this pass is active — it had not announced when the batch started.  Its own marks of
+                                // this batch are written by phase_mixed_mark, after the pass.)
+                                if (__popc(wo[j] & RM) < a.L) continue;
                                 // a receiver that already announced explicit proposals in this batch: those subjects left
-                                // `proposal` (bit 14 = raised to >= H by this very pass: in the band at entry, not pending)
+                                // `proposal` (the transient plane = raised to >= H by this very pass: in the band at entry, not pending)
                                 if (MX) {
                                     const int64_t r = rb + j;
                                     if (emitted_in_batch(e, sm.e_so[ei], r, wo[j], splitmix64(a.dl.perm_seed + (uint64_t)(a.rbegin + r)))) continue;
@@ -1484,16 +1490,18 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
                             }
                         }
                         bool any = false;
+                        uint32_t trans = 0;
 #pragma unroll
                         for (int j = 0; j < 4; ++j) {
                             if (!implicit[j]) continue;
                             any = true;
-                            uint32_t nw = w[j] | implicit[j];
-                            const bool raised = __popc(nw & RM) >= a.H;
-                            if (raised && mixed) nw |= CD_BIT_CALL;            // transient marker, cleared by the unmark phase
-                            w[j] = nw;
+                            w[j] |= implicit[j];
+                            const bool raised = __popc(w[j] & RM) >= a.H;
+                            if (raised && mixed) trans |= 1u << j;             // transient marker, cleared by the unmark phase
                             if (raised) { ++res[j]; kh1[j] += sm.mix1[i]; kh2[j] += sm.mix2[i]; }   // moved preProposal -> proposal
                         }
+                        // (the neighbouring thread's 4 receivers share the byte: atomic on the aligned word)
+                        if (trans) atomicOr(e.trans.word(a.wl.slots[base + i], rb), trans << (rb & 31));
                         if (any) a.rows.store4(sm.row[i], rb, w);
                     }
                 }
@@ -1542,7 +1550,7 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
                 e.pend_h1[r] = ph1; e.pend_h2[r] = ph2; e.pend_cnt[r] = pc;
             }
             flags[j] &= ~RF_K3;
-            if ((flags[j] & RF_MIXED_EMIT) && (flags[j] & RF_ANN_NOW) && !(flags[j] & RF_RULE_GE_H)) ++my_inval;   // needs bit-15 marks
+            if ((flags[j] & RF_MIXED_EMIT) && (flags[j] & RF_ANN_NOW) && !(flags[j] & RF_RULE_GE_H)) ++my_inval;   // needs emit marks
             ann |= ((flags[j] & RF_ANNOUNCED) ? 1u : 0u) << (8 * j);
         }
         if (touched) {
@@ -1556,42 +1564,47 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
     }
 }
 
-// RF_MIXED_EMIT receivers whose invalidation pass did not emit announce only the explicit part: give it bit 15 so that
-// rapid_cd_get_proposal can list it later (the pre-batch rows are gone by then).
+// RF_MIXED_EMIT receivers whose invalidation pass did not emit announce only the explicit part: record it in the emit plane so
+// that rapid_cd_get_proposal can list it later (the pre-batch rows are gone by then).  Every slot < S of such a receiver gets its
+// bit written, set or clear (the plane is never cleared, see k_gather_proposal).  A warp owns 32 consecutive receivers, i.e. one
+// word per slot: lane 0 merges the warp's ballot under the mask of its marked lanes, and nothing else writes that word in the pass.
 __device__ __noinline__ void phase_mixed_mark(const ResolveArgs& e, int32_t S) {
+    static_assert(GEN_THREADS % 32 == 0, "a warp owns one word of the plane");
     const ApplyArgs& a = e.ap;
     const int spb = 64;
     const int rblocks = (int)(a.Rpad / GEN_THREADS), sblocks = (S + spb - 1) / spb;
     const int64_t items = (int64_t)rblocks * sblocks;
     for (int64_t wi = blockIdx.x; wi < items; wi += gridDim.x) {
         const int64_t r = (wi % rblocks) * GEN_THREADS + threadIdx.x;
-        if (r >= a.R) continue;
-        const uint32_t f = e.rflags[r];
-        if (!(f & RF_MIXED_EMIT) || !(f & RF_ANN_NOW) || (f & RF_RULE_GE_H)) continue;
+        const uint32_t f = r < a.R ? e.rflags[r] : 0u;
+        const bool marked = (f & RF_MIXED_EMIT) && (f & RF_ANN_NOW) && !(f & RF_RULE_GE_H);
+        const uint32_t mm = __ballot_sync(0xffffffffu, marked);
+        if (mm == 0) continue;                                          // (warp-uniform)
         const uint64_t rs = splitmix64(a.dl.perm_seed + (uint64_t)(a.rbegin + r));
         const int32_t s0 = (int32_t)(wi / rblocks) * spb, s1 = min(S, s0 + spb);
         for (int32_t s = s0; s < s1; ++s) {
-            uint8_t* row = a.rows.cur_lo(s);
-            const uint32_t w = a.rows.get(row, r);
-            if (!(w & CD_BIT_EMIT) && emitted_in_batch(e, s, r, w, rs)) a.rows.hi_or(row, r, CD_BIT_EMIT);
+            const bool em = marked && emitted_in_batch(e, s, r, a.rows.get(s, r), rs);
+            const uint32_t b = __ballot_sync(0xffffffffu, em);
+            if ((threadIdx.x & 31) == 0) {
+                uint32_t* p = e.emit.word(s, r);
+                *p = (*p & ~mm) | b;
+            }
         }
     }
 }
 
+// the transient plane back to all zero: 128 bytes per listed (subject, tile) pair, the only places the pass can have set bits
 __device__ void phase_inval_unmark(const ResolveArgs& e) {
     const ApplyArgs& a = e.ap;
     const int n_list = min(*(volatile int32_t*)a.wl.count, a.wl.cap);
-    const int64_t items = (int64_t)n_list * a.wl.n_tiles;
-    for (int64_t p = blockIdx.x; p < items; p += gridDim.x) {
+    constexpr int TW = TILE_R / 32;                                     // words of a tile
+    const int64_t items = (int64_t)n_list * a.wl.n_tiles * TW;
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < items; q += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t p = q / TW;
         const int32_t sl = a.wl.slots[p / a.wl.n_tiles];
         const int tile = (int)(p % a.wl.n_tiles);
         if (!a.wl.in_tile[(size_t)sl * a.wl.n_tiles + tile]) continue;
-        uint8_t* row = a.rows.cur_lo(sl);
-        for (int q = 0; q < TILE_R / GEN_THREADS; ++q) {
-            const int64_t r = (int64_t)tile * TILE_R + q * GEN_THREADS + threadIdx.x;
-            if (r >= a.R) continue;
-            if (a.rows.get(row, r) & CD_BIT_CALL) a.rows.hi_clear(row, r, CD_BIT_CALL);
-        }
+        e.trans.p[(size_t)sl * e.trans.words + (size_t)tile * TW + (size_t)(q % TW)] = 0u;
     }
 }
 
@@ -1841,11 +1854,11 @@ __global__ void __launch_bounds__(GEN_THREADS, 2) k_marks(const ResolveArgs* __r
     phase_inval_finalize2<true>(a, 1, sm, s_red);                        // the receivers k_inval_finalize2 left out
     grid.sync();
     if (*(volatile int32_t*)&a.bc->n_inval > 0) {
-        // receivers that announce only the explicit part: persist it as bit 15 while the pre-batch rows still exist
+        // receivers that announce only the explicit part: persist it in the emit plane while the pre-batch rows still exist
         phase_mixed_mark(a, *(volatile int32_t*)&a.bc->n_slots);
         grid.sync();
     }
-    phase_inval_unmark(a);                                              // only now: the marks above still needed bit 14
+    phase_inval_unmark(a);                                              // only now: the marks above still needed the transient plane
     resolve_tail(a, a.serial);
 }
 
@@ -2028,7 +2041,7 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
         int dev = 0, sms = TARGET_SMS, per_u = 8, per_g = 4, per_r = 2;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_u, k_apply_uniform<false, false, 4>, UNI_THREADS, 0);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_u, k_apply_uniform<false, false, 2>, UNI_THREADS, 0);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_g, k_apply_generic, GEN_THREADS, 0);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_r, k_mixed_flip, GEN_THREADS, 0);
         int per_m = 2;
@@ -2104,7 +2117,7 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
     RAPID_CUDA(cudaEventRecord(cd->evk0, s));
     if (swar) {
         dim3 grid((unsigned)b->n_tiles, (unsigned)n_chunks);
-        if (cd->hb == 4) launch_uniform<4>(grid, s, ap, counts_only, seq);
+        if (cd->hb == 2) launch_uniform<2>(grid, s, ap, counts_only, seq);
         else launch_uniform<8>(grid, s, ap, counts_only, seq);
         cd->last_path = counts_only ? 4 : 2;
     } else {
@@ -2116,7 +2129,8 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
     RAPID_CUDA(cudaEventRecord(cd->evk1, s));
 
     ResolveArgs ra;
-    ra.ap = ap; ra.bc = cd->counts.p; ra.snap = cd->counts_snap.p; ra.n_chunks = n_chunks;
+    ra.ap = ap; ra.bc = cd->counts.p;
+    ra.emit = MarkPlane{cd->emit_marks.p, cd->Rpad / 32}; ra.trans = MarkPlane{cd->trans_marks.p, cd->Rpad / 32}; ra.snap = cd->counts_snap.p; ra.n_chunks = n_chunks;
     ra.uniform = uniform ? 1 : 0; ra.counts_only = counts_only ? 1 : 0; ra.cur_w = cd->cur.p;
     ra.seq = seq ? 1 : 0; ra.seq_dev = nullptr;
     ra.n_pre = cd->n_pre.p; ra.rflags = cd->rflags.p; ra.pend_h1 = cd->pend_h1.p; ra.pend_h2 = cd->pend_h2.p;

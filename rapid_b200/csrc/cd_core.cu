@@ -196,15 +196,19 @@ __global__ void k_clear_call(RowRef rows, int32_t S, int64_t R) {
     if (w & CD_BIT_CALL) *p = (uint16_t)(w & ~CD_BIT_CALL);
 }
 
-// the announced proposal of one receiver: (id, ring-0 key) pairs
-__global__ void k_gather_proposal(RowRef rows, int32_t S, int64_t r, int H, uint32_t RM, int rule_ge_h,
+// the announced proposal of one receiver: (id, ring-0 key) pairs.  Bucketed handles (emit.p != nullptr) keep bit 15 in the emit
+// plane.  That plane is written for every slot < S when the receiver announces, and never cleared: slots assigned later may carry
+// marks of an earlier configuration epoch.  A mark always comes with >= H, and a receiver that has announced is frozen, so its
+// word in a slot assigned later stays zero.  Requiring both therefore lists exactly the marked subjects of this epoch.
+__global__ void k_gather_proposal(RowRef rows, MarkPlane emit, int32_t S, int64_t r, int H, uint32_t RM, int rule_ge_h,
                                   const int32_t* __restrict__ slot_subject, const int64_t* __restrict__ key0,
                                   int32_t* __restrict__ out_ids, int64_t* __restrict__ out_keys, int32_t cap,
                                   int32_t* __restrict__ count) {
     const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= S) return;
     const uint32_t w = rows.get(s, r);
-    const bool in = rule_ge_h ? (__popc(w & RM) >= H) : ((w & CD_BIT_EMIT) != 0);
+    const bool ge_h = __popc(w & RM) >= H;
+    const bool in = rule_ge_h ? ge_h : emit.p ? (ge_h && emit.test(s, r)) : ((w & CD_BIT_EMIT) != 0);
     if (in) {
         const int32_t at = atomicAdd(count, 1);
         if (at < cap) { const int32_t id = slot_subject[s]; out_ids[at] = id; out_keys[at] = key0[id]; }
@@ -243,6 +247,7 @@ __global__ void k_clear_receivers(int64_t R, int32_t* __restrict__ n_pre, int32_
 // host side
 // =====================================================================================================
 static RowRef rowref(const CD* cd) { return RowRef{cd->masks.p, cd->cur.p, cd->Rpad, cd->row_stride, cd->nbuf, cd->hb}; }
+static MarkPlane emit_plane(const CD* cd) { return MarkPlane{cd->bucketed ? cd->emit_marks.p : nullptr, cd->Rpad / 32}; }
 
 static int32_t ensure_id_capacity(CD* cd) {
     const int64_t ntot = cd->view->n + cd->view->nj;
@@ -279,9 +284,26 @@ static int32_t ensure_slot_capacity(CD* cd, size_t need) {
     RAPID_CHECK(nc.reserve(ncap));
     RAPID_CUDA(cudaMemsetAsync(nc.p, 0, ncap, cd->stream));
     if (cd->S_cap) RAPID_CUDA(cudaMemcpyAsync(nc.p, cd->cur.p, cd->S_cap, cudaMemcpyDeviceToDevice, cd->stream));
+    // bucketed handles: the two mark planes grow with the rows (zero-filled: the transient plane's invariant)
+    const size_t words = cd->Rpad / 32, old_words = cd->S_cap * words;
+    auto grow_plane = [&](const DevBuf<uint32_t>& from, DevBuf<uint32_t>& to) -> int32_t {
+        RAPID_CHECK(to.reserve(ncap * words));
+        if (old_words) RAPID_CUDA(cudaMemcpyAsync(to.p, from.p, old_words * sizeof(uint32_t), cudaMemcpyDeviceToDevice, cd->stream));
+        RAPID_CUDA(cudaMemsetAsync(to.p + old_words, 0, (ncap * words - old_words) * sizeof(uint32_t), cd->stream));
+        return RAPID_OK;
+    };
+    DevBuf<uint32_t> ne, nt;
+    if (cd->bucketed) {
+        RAPID_CHECK(grow_plane(cd->emit_marks, ne));
+        RAPID_CHECK(grow_plane(cd->trans_marks, nt));
+    }
     RAPID_CUDA(cudaStreamSynchronize(cd->stream));
     std::swap(cd->masks.p, nm.p); std::swap(cd->masks.cap, nm.cap);
     std::swap(cd->cur.p, nc.p); std::swap(cd->cur.cap, nc.cap);
+    if (cd->bucketed) {
+        std::swap(cd->emit_marks.p, ne.p); std::swap(cd->emit_marks.cap, ne.cap);
+        std::swap(cd->trans_marks.p, nt.p); std::swap(cd->trans_marks.cap, nt.cap);
+    }
     cd->S_cap = ncap;
     return RAPID_OK;
 }
@@ -892,6 +914,9 @@ int32_t rapid_cd_clear(rapid_cd* cd) {
         // Bucketed handles never read the state of a slot before the batch that assigns it has written it (slots >= S_before
         // are write-only), so clear() is O(#slots + #receivers): forget the dictionary, reset the receivers' scalars, the work
         // list and the device counters — ONE launch, no host round trip (the slot count lives on the device).
+        // The mark planes need nothing either: the transient plane is all zero between batches, and the emit plane is only read
+        // for a receiver that announced in the new epoch, whose mark pass rewrites every slot it had, together with ">= H"
+        // (k_gather_proposal), which the zero words of slots assigned after that never meet.
         cd->S = 0;
         RAPID_CHECK(bucketed_clear(cd));
         cd->log_cells = 0; cd->log_blocked_bytes = 0; cd->log_batches.clear(); cd->log_complete = true;
@@ -1187,7 +1212,7 @@ int32_t rapid_cd_get_proposal(const rapid_cd* cd, int64_t receiver, int32_t* out
     RAPID_CHECK(d_cnt.reserve(1));
     RAPID_CUDA(cudaMemsetAsync(d_cnt.p, 0, sizeof(int32_t), cd->stream));
     k_gather_proposal<<<(unsigned)ceil_div<int32_t>(S, 256), 256, 0, cd->stream>>>(
-        rowref(cd), S, receiver, cd->H, (1u << cd->K) - 1u, (flags & RF_RULE_GE_H) ? 1 : 0, cd->slot_subject.p, cd->view->key.p /* ring 0 row */,
+        rowref(cd), emit_plane(cd), S, receiver, cd->H, (1u << cd->K) - 1u, (flags & RF_RULE_GE_H) ? 1 : 0, cd->slot_subject.p, cd->view->key.p /* ring 0 row */,
         d_ids.p, d_keys.p, S, d_cnt.p);
     RAPID_KERNEL_CHECK();
     int32_t n = 0;

@@ -16,7 +16,8 @@ namespace rapid {
 //               bucketed handles: transient marker of the invalidation pass (set and cleared inside one batch)
 // bit 15      : subject was emitted in a proposal (it left `proposal` at :118-121)
 // preProposal == { L <= popc < H },  proposal == { popc >= H and bit 15 clear }.
-// Kernels compute on this 16-bit word; how it is stored is the business of RowRef below.
+// Kernels compute on this 16-bit word; how it is stored is the business of RowRef below.  Sweep handles keep bits 14 and 15 in
+// their uint16 rows; bucketed rows hold the ring bits only, and their two marks live in side planes (MarkPlane).
 #define CD_BIT_CALL 0x4000u
 #define CD_BIT_EMIT 0x8000u
 
@@ -38,7 +39,7 @@ struct BatchCounts {
     int32_t bad_ring;      // index of a cell with ring >= K, or -1 (the cell is dropped, the rest of the batch applies)
     int32_t bad_dst;       // index of a cell with dst outside [0, n + joiners), or -1 (dropped likewise)
     int32_t n_mixed;       // bucketed: receivers needing exact interval resolution
-    int32_t n_inval;       // bucketed: receivers that announce only the explicit part (bit-15 marks needed)
+    int32_t n_inval;       // bucketed: receivers that announce only the explicit part (emit marks needed)
     int32_t S_before;      // n_slots when the batch started: slots >= S_before are "fresh" (known-zero state, never read);
                            // between batches S_before == n_slots (the prepare kernel takes the slot count from here)
     int32_t overflow;      // the batch needs more subject slots than the handle holds: NOTHING was applied
@@ -74,9 +75,11 @@ struct CD {
     size_t S_cap = 0;
     int64_t ntot_cap = 0;             // capacity of slot_of / first_idx (node + joiner ids)
 
-    int hb = 0;                       // bits per receiver of a row's hi plane (bucketed handles), 0: uint16 rows (sweep)
+    int hb = 0;                       // bits per receiver of a row's hi plane (bucketed handles: 2 or 8), 0: uint16 rows (sweep)
     size_t row_stride = 0;            // bytes per (slot, buffer) row
     DevBuf<uint8_t> masks;            // [S_cap][nbuf] rows of row_stride bytes (see RowRef)
+    DevBuf<uint32_t> emit_marks;      // [S_cap][Rpad / 32] bucketed handles: the emit plane (see MarkPlane)
+    DevBuf<uint32_t> trans_marks;     // [S_cap][Rpad / 32] ... and the transient plane
     DevBuf<uint8_t> cur;              // [S_cap] which of the nbuf rows is current
     DevBuf<int32_t> slot_of;          // [ntot_cap] id -> slot, -1 if none
     DevBuf<int32_t> first_idx;        // [ntot_cap] scratch (INT_MAX)
@@ -140,22 +143,23 @@ struct CD {
 
 // ---- state rows: the only code that knows how a row stores the logical words ---------------------------------------------
 // Sweep handles: one interleaved uint16_t[Rpad] row per slot (the sweep kernel reads and writes one receiver per thread in place).
-// Bucketed handles: every (slot, buffer) row is two planes, each padded to whole 1024-receiver tiles, back to back:
+// Bucketed handles: every (slot, buffer) row holds ring bits only, as two planes, each padded to whole 1024-receiver tiles, back
+// to back:
 //   lo plane  uint8_t[Rpad]        bits 0..7 of the word (rings 0..7)
-//   hi plane  Rpad lanes of HB bits, receiver r in bits [HB * r, HB * r + HB) of the plane
-//             HB = 4 (K <= 10): rings 8, 9, bit 14, bit 15            -> 1.5 B per receiver
-//             HB = 8 (K <= 14): rings 8..13, bit 14, bit 15           -> 2 B per receiver
-// At HB = 4 two receivers share a byte of the hi plane: a lane is written either as part of a thread-owned group of whole
-// bytes (the group accessors), or with an atomic on its aligned 32-bit word (hi_or / hi_clear) — never with a plain sub-byte store.
-__host__ __device__ inline int row_hi_bits(int K) { return K <= 10 ? 4 : 8; }
+//   hi plane  Rpad lanes of HB bits, receiver r in bits [HB * r, HB * r + HB) of the plane: bits 8.. of the word
+//             HB = 2 (K <= 10): rings 8, 9                            -> 1.25 B per receiver
+//             HB = 8 (K <= 14): rings 8..13                           -> 2 B per receiver
+// Their marks (bits 14 and 15 of the logical word) live in the MarkPlanes below.  At HB = 2 four receivers share a byte of the hi
+// plane: a lane is only ever written as part of a thread-owned group of whole bytes (the group accessors, store4, the warp-wide
+// row_store1_warp) — never with a plain sub-byte store.
+__host__ __device__ inline int row_hi_bits(int K) { return K <= 10 ? 2 : 8; }
 
 template <int HB>
 __device__ __forceinline__ uint32_t hi_pack(uint32_t w) {      // logical word -> hi lane
-    return HB == 4 ? (((w >> 8) & 3u) | ((w >> 12) & 0xCu)) : ((w >> 8) & 0xFFu);
+    return (w >> 8) & ((1u << HB) - 1u);
 }
-template <int HB>
 __device__ __forceinline__ uint32_t hi_unpack(uint32_t h) {    // hi lane -> bits 8.. of the logical word
-    return HB == 4 ? (((h & 3u) << 8) | ((h & 0xCu) << 12)) : (h << 8);
+    return h << 8;
 }
 
 struct RowRef {
@@ -164,7 +168,7 @@ struct RowRef {
     size_t Rpad;
     size_t stride;                    // bytes per (slot, buffer) row
     int nbuf;
-    int hb;                           // 0: uint16 rows (sweep); 4 / 8: two planes (bucketed)
+    int hb;                           // 0: uint16 rows (sweep); 2 / 8: two planes (bucketed)
 
     // lo plane of (slot, buffer); the hi plane follows it
     __device__ __forceinline__ uint8_t* lo(int32_t slot, int buf) const { return base + ((size_t)slot * nbuf + buf) * stride; }
@@ -177,54 +181,37 @@ struct RowRef {
     // scalar get of receiver r's word in the row whose lo plane is `l`
     __device__ __forceinline__ uint32_t get(const uint8_t* l, int64_t r) const {
         if (hb == 0) return reinterpret_cast<const uint16_t*>(l)[r];
-        if (hb == 4) return l[r] | hi_unpack<4>((l[Rpad + (r >> 1)] >> ((r & 1) * 4)) & 0xFu);
-        return l[r] | hi_unpack<8>(l[Rpad + r]);
+        if (hb == 2) return l[r] | hi_unpack((l[Rpad + (r >> 2)] >> ((r & 3) * 2)) & 3u);
+        return l[r] | hi_unpack(l[Rpad + r]);
     }
     __device__ __forceinline__ uint32_t get(int32_t slot, int64_t r) const { return get(cur_lo(slot), r); }
 
-    // receivers r .. r+3 (r % 4 == 0) of a bucketed row: one 32-bit lo load, one 16- or 32-bit hi load; x = lo lanes, y = hi lanes
+    // receivers r .. r+3 (r % 4 == 0) of a bucketed row: one 32-bit lo load, one 8- or 32-bit hi load; x = lo lanes, y = hi lanes
+    // (at HB = 2 the group owns exactly one byte of the hi plane)
     __device__ __forceinline__ uint2 load4(const uint8_t* l, int64_t r) const {
         return make_uint2(*reinterpret_cast<const uint32_t*>(l + r),
-                          hb == 4 ? (uint32_t)*reinterpret_cast<const uint16_t*>(l + Rpad + (r >> 1))
-                                  : *reinterpret_cast<const uint32_t*>(l + Rpad + r));
+                          hb == 2 ? (uint32_t)l[Rpad + (r >> 2)] : *reinterpret_cast<const uint32_t*>(l + Rpad + r));
     }
     __device__ __forceinline__ uint32_t word4(uint2 g, int j) const {   // receiver r + j of a load4 group as a logical word
-        return ((g.x >> (8 * j)) & 0xFFu) | (hb == 4 ? hi_unpack<4>((g.y >> (4 * j)) & 0xFu) : hi_unpack<8>((g.y >> (8 * j)) & 0xFFu));
+        return ((g.x >> (8 * j)) & 0xFFu) | hi_unpack(hb == 2 ? (g.y >> (2 * j)) & 3u : (g.y >> (8 * j)) & 0xFFu);
     }
     __device__ __forceinline__ void store4(uint8_t* l, int64_t r, const uint32_t w[4]) const {
         uint32_t lw = 0, hw = 0;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             lw |= (w[j] & 0xFFu) << (8 * j);
-            hw |= hb == 4 ? hi_pack<4>(w[j]) << (4 * j) : hi_pack<8>(w[j]) << (8 * j);
+            hw |= hb == 2 ? hi_pack<2>(w[j]) << (2 * j) : hi_pack<8>(w[j]) << (8 * j);
         }
         *reinterpret_cast<uint32_t*>(l + r) = lw;
-        if (hb == 4) *reinterpret_cast<uint16_t*>(l + Rpad + (r >> 1)) = (uint16_t)hw;
+        if (hb == 2) l[Rpad + (r >> 2)] = (uint8_t)hw;
         else *reinterpret_cast<uint32_t*>(l + Rpad + r) = hw;
-    }
-
-    // bucketed rows: set / clear bits 14 / 15 of receiver r's word (its neighbours may be written at the same time)
-    __device__ __forceinline__ uint32_t* hi_word(uint8_t* l, int64_t r, uint32_t bit, uint32_t* shift) const {
-        const int64_t p = r * hb + (hb - (bit == CD_BIT_EMIT ? 1 : 2));   // bit 15 is the lane's top bit, bit 14 the one below
-        *shift = (uint32_t)(p & 31);
-        return reinterpret_cast<uint32_t*>(l + Rpad) + (p >> 5);
-    }
-    __device__ __forceinline__ void hi_or(uint8_t* l, int64_t r, uint32_t bit) const {
-        uint32_t sh;
-        uint32_t* p = hi_word(l, r, bit, &sh);
-        atomicOr(p, 1u << sh);
-    }
-    __device__ __forceinline__ void hi_clear(uint8_t* l, int64_t r, uint32_t bit) const {
-        uint32_t sh;
-        uint32_t* p = hi_word(l, r, bit, &sh);
-        atomicAnd(p, ~(1u << sh));
     }
 };
 
 // 8 consecutive receivers of a bucketed row (r % 8 == 0), as SWAR lanes: lo = 8 byte lanes, hi = 8 lanes of HB bits
 template <int HB>
 struct Group8 {
-    using Hi = typename std::conditional<HB == 4, uint32_t, uint64_t>::type;
+    using Hi = typename std::conditional<HB == 2, uint16_t, uint64_t>::type;
     uint64_t lo;
     Hi hi;
 };
@@ -247,27 +234,29 @@ __device__ __forceinline__ void group8_store(const RowRef& rows, uint8_t* l, int
 // lane j of a group as a logical word
 template <int HB>
 __device__ __forceinline__ uint32_t group8_word(const Group8<HB>& g, int j) {
-    return (uint32_t)((g.lo >> (8 * j)) & 0xFFu) | hi_unpack<HB>((uint32_t)(g.hi >> (HB * j)) & ((1u << HB) - 1u));
+    return (uint32_t)((g.lo >> (8 * j)) & 0xFFu) | hi_unpack((uint32_t)(g.hi >> (HB * j)) & ((1u << HB) - 1u));
 }
 // lane j |= the logical bits `w`
 template <int HB>
 __device__ __forceinline__ void group8_or_word(Group8<HB>& g, int j, uint32_t w) {
     g.lo |= (uint64_t)(w & 0xFFu) << (8 * j);
-    g.hi |= (typename Group8<HB>::Hi)hi_pack<HB>(w) << (HB * j);
+    using Hi = typename Group8<HB>::Hi;
+    g.hi = (Hi)(g.hi | ((Hi)hi_pack<HB>(w) << (HB * j)));
 }
 // A logical word replicated over the lanes: x = its lo byte over 4 byte lanes, y = its hi lane over 32 bits (as the lanes repeat)
 template <int HB>
 __device__ __forceinline__ uint2 group8_rep(uint32_t w) {
-    return make_uint2((w & 0xFFu) * 0x01010101u, hi_pack<HB>(w) * (HB == 4 ? 0x11111111u : 0x01010101u));
+    return make_uint2((w & 0xFFu) * 0x01010101u, hi_pack<HB>(w) * (HB == 2 ? 0x55555555u : 0x01010101u));
 }
 // all-ones lanes for the receivers set in `act` (bit j = receiver j of the group)
 template <int HB>
 __device__ __forceinline__ Group8<HB> group8_mask(uint32_t act) {
+    using Hi = typename Group8<HB>::Hi;
     Group8<HB> m;
     m.lo = 0; m.hi = 0;
 #pragma unroll
     for (int j = 0; j < 8; ++j)
-        if ((act >> j) & 1u) { m.lo |= 0xFFull << (8 * j); m.hi |= (typename Group8<HB>::Hi)((1u << HB) - 1u) << (HB * j); }
+        if ((act >> j) & 1u) { m.lo |= 0xFFull << (8 * j); m.hi = (Hi)(m.hi | ((Hi)((1u << HB) - 1u) << (HB * j))); }
     return m;
 }
 // the replicated word `rep` under the mask (the lanes outside it are zero)
@@ -275,7 +264,7 @@ template <int HB>
 __device__ __forceinline__ Group8<HB> group8_fill(uint2 rep, const Group8<HB>& m) {
     Group8<HB> g;
     g.lo = (((uint64_t)rep.x << 32) | rep.x) & m.lo;
-    g.hi = (HB == 4 ? (typename Group8<HB>::Hi)rep.y : (typename Group8<HB>::Hi)(((uint64_t)rep.y << 32) | rep.y)) & m.hi;
+    g.hi = (HB == 2 ? (typename Group8<HB>::Hi)rep.y : (typename Group8<HB>::Hi)(((uint64_t)rep.y << 32) | rep.y)) & m.hi;
     return g;
 }
 // the lanes under the mask take the replicated word `rep`, the others keep theirs
@@ -283,14 +272,16 @@ template <int HB>
 __device__ __forceinline__ void group8_merge(Group8<HB>& g, uint2 rep, const Group8<HB>& m) {
     const Group8<HB> f = group8_fill<HB>(rep, m);
     g.lo = (g.lo & ~m.lo) | f.lo;
-    g.hi = (g.hi & ~m.hi) | f.hi;
+    g.hi = (typename Group8<HB>::Hi)((g.hi & ~m.hi) | f.hi);
 }
-// Do all lanes under the (non-empty) mask hold the same word?  AND over them == OR over them, per plane.  *st = the OR.
+// Do all lanes under the (non-empty) mask hold the same word?  AND over them == OR over them, per plane.  *v = the OR.
+// (T holds exactly 8 lanes of B bits.)
 template <int B, typename T>
 __device__ __forceinline__ bool lanes_same(T x, T m, uint32_t* v) {
-    T a = x | ~m, o = x & m;
+    static_assert(B == (int)sizeof(T), "8 lanes of B bits fill the word");
+    T a = (T)(x | ~m), o = (T)(x & m);
 #pragma unroll
-    for (int s = 4 * B; s >= B; s >>= 1) { a &= a >> s; o |= o >> s; }
+    for (int s = 4 * B; s >= B; s >>= 1) { a &= (T)(a >> s); o |= (T)(o >> s); }
     const uint32_t lm = (1u << B) - 1u;
     *v = (uint32_t)o & lm;
     return ((uint32_t)a & lm) == *v;
@@ -300,25 +291,41 @@ __device__ __forceinline__ bool group8_same(const Group8<HB>& g, const Group8<HB
     uint32_t vl, vh;
     const bool sl = lanes_same<8>(g.lo, m.lo, &vl);
     const bool sh = lanes_same<HB>(g.hi, m.hi, &vh);
-    *st = vl | hi_unpack<HB>(vh);
+    *st = vl | hi_unpack(vh);
     return sl && sh;
 }
 
 // one receiver per thread, consecutive threads of a warp own consecutive receivers (r % 32 == lane): every lane of the warp
-// stores its word; at HB = 4 the hi lanes of 8 receivers are gathered by shuffles and one lane stores their 32-bit word
+// stores its word; at HB = 2 the hi lanes of 16 receivers are gathered by shuffles and one lane stores their 32-bit word
 template <int HB>
 __device__ __forceinline__ void row_store1_warp(const RowRef& rows, uint8_t* l, int64_t r, uint32_t w) {
     l[r] = (uint8_t)w;
     if (HB == 8) {
         l[rows.Rpad + r] = (uint8_t)hi_pack<8>(w);
     } else {
-        uint32_t h = hi_pack<4>(w) << (4 * (r & 7));
+        uint32_t h = hi_pack<2>(w) << (2 * (r & 15));
         h |= __shfl_xor_sync(0xffffffffu, h, 1);
         h |= __shfl_xor_sync(0xffffffffu, h, 2);
         h |= __shfl_xor_sync(0xffffffffu, h, 4);
-        if ((r & 7) == 0) *reinterpret_cast<uint32_t*>(l + rows.Rpad + (r >> 1)) = h;
+        h |= __shfl_xor_sync(0xffffffffu, h, 8);
+        if ((r & 15) == 0) *reinterpret_cast<uint32_t*>(l + rows.Rpad + (r >> 2)) = h;
     }
 }
+
+// ---- mark planes of bucketed handles: one bit per (slot, receiver), slot-major, Rpad bits per slot, single-buffered -----------
+// The apply kernels never touch them.
+//   emit plane       bit 15: the subject left in the explicit-only proposal a receiver announced through the interval analysis.
+//                    Written (set or clear, every slot < S) in the batch in which that receiver announces; read only while its
+//                    announced rule is the explicit one, together with ">= H" (see k_gather_proposal).
+//   transient plane  bit 14: raised to >= H by the invalidation pass of the batch in flight.  All zero between batches: the
+//                    batch that sets bits clears them before it ends (phase_inval_unmark).
+// Neighbouring receivers share a word: bits are set with atomicOr, or written by the one warp that owns the word in the pass.
+struct MarkPlane {
+    uint32_t* p;
+    size_t words;                     // 32-bit words per slot (Rpad / 32)
+    __device__ __forceinline__ uint32_t* word(int32_t slot, int64_t r) const { return p + (size_t)slot * words + (size_t)(r >> 5); }
+    __device__ __forceinline__ bool test(int32_t slot, int64_t r) const { return (*word(slot, r) >> (r & 31)) & 1u; }
+};
 
 struct DeliveryDev {
     uint32_t flags = 0;
