@@ -125,6 +125,22 @@ int32_t rapid_view_set_joiner_ids(rapid_view* v, int32_t first_joiner_id, int64_
 int32_t rapid_view_current_config_id(const rapid_view* v, int64_t* out);
 /* expected observers of every registered joiner: out[j*K+k] for joiner id n + j. */
 int32_t rapid_view_joiner_tables(const rapid_view* v, int32_t* out);
+/* Expansion of the monitoring overlay.  The observer graph of the view's n >= 3 members is A = sum_k (P_k + P_k^T), P_k the
+ * permutation "successor on ring k": A[v][obs[v][k]] += 1 and A[v][subj[v][k]] += 1 for every k, multiplicities kept (a node that
+ * observes another on m rings contributes m).  A is symmetric, its rows sum to 2K, its top eigenvalue is 2K with the all-ones
+ * vector.  For A restricted to the complement of that vector: *lambda2 = the largest eigenvalue, *lambda_min = the smallest;
+ * max(|lambda2|, |lambda_min|) / 2K is the expander figure of the Rapid paper (< 0.45 at K = 10).  Registered joiners are not part
+ * of the graph.  Computed on the device by Lanczos with full re-orthogonalisation in fp64 (basis in HBM: steps * n * 8 bytes of
+ * scratch for the duration of the call), from the start vector  x[v] = 2 u - 1, u = (splitmix64(seed + v) >> 11) * 2^-53,  mean
+ * removed, normalised.  It stops when *residual <= tol * 2K or after max_steps operator applications (or n - 1, the dimension of
+ * the complement), whichever comes first; reaching max_steps is not an error.  *residual = the larger |beta_m * s_m| of the two
+ * reported Ritz values: each lies within it of an eigenvalue of A.  *steps = operator applications spent, *device_ms = CUDA events
+ * around them.  Every out pointer may be NULL.  The same seed on the same view returns the same bits.  The view is not modified.
+ * RAPID_EINVAL, and nothing is written, if n < 3 (n = 2 is bipartite with +-2K, n = 1 has no complement), tol <= 0 or max_steps
+ * outside [2, RAPID_OVERLAY_MAX_STEPS]. */
+#define RAPID_OVERLAY_MAX_STEPS 512
+int32_t rapid_view_overlay_spectrum(const rapid_view* v, uint64_t seed, double tol, int32_t max_steps, double* lambda2,
+                                    double* lambda_min, double* residual, int32_t* steps, float* device_ms);
 
 /* ------------------------------------------------------------------------------------------------
  * MultiNodeCutDetector for R virtual nodes ("receivers")   (MultiNodeCutDetector.java,

@@ -127,6 +127,21 @@ final class GpuMembershipView {
         return out[0];
     }
 
+    /**
+     * Expansion of the monitoring overlay (rapid_view_overlay_spectrum): {lambda2, lambdaMin, residual, steps, lambda / 2K} of the
+     * members' observer graph below its trivial eigenvalue 2K; lambda / 2K is the paper's expander figure.
+     */
+    double[] overlaySpectrum(final long seed, final double tol, final int maxSteps) {
+        final long[] out = new long[5];
+        if (Native.viewOverlaySpectrum(handle, seed, Double.doubleToRawLongBits(tol), maxSteps, out) != 0) {
+            throw new IllegalStateException(Native.lastError());
+        }
+        final double lambda2 = Double.longBitsToDouble(out[0]);
+        final double lambdaMin = Double.longBitsToDouble(out[1]);
+        return new double[]{lambda2, lambdaMin, Double.longBitsToDouble(out[2]), out[3],
+                            Math.max(Math.abs(lambda2), Math.abs(lambdaMin)) / (2.0 * K)};
+    }
+
     /** id of a known endpoint (member or registered joiner), -1 otherwise; never registers anything */
     int tryIdOf(final Endpoint e) {
         final Integer id = ids.get(e);

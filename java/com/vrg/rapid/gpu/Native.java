@@ -36,6 +36,9 @@ public final class Native {
     public static native int viewSetJoinerIds(long view, int firstJoinerId, long[] idHigh, long[] idLow);
     /** getCurrentConfigurationId from the device-resident identifiersSeen + ring 0 */
     public static native int viewCurrentConfigId(long view, long[] out1);
+    /** rapid_view_overlay_spectrum: tolBits = Double.doubleToRawLongBits(tol); out5 = raw bits of lambda2, lambda_min and residual
+     *  (Double.longBitsToDouble), the steps spent, raw bits of the device milliseconds (as a double). */
+    public static native int viewOverlaySpectrum(long view, long seed, long tolBits, int maxSteps, long[] out5);
 
     // ---- MultiNodeCutDetector / alert-batch handler ----
     public static native long cdCreate(long view, int h, int l, long receivers, long receiverBegin, int modeFlags,

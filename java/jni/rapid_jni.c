@@ -150,6 +150,22 @@ JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_viewCurrentConfigId(JNIEnv*
     return rc;
 }
 
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_viewOverlaySpectrum(JNIEnv* env, jclass c, jlong view, jlong seed, jlong tolBits,
+                                                                         jint maxSteps, jlongArray out5) {
+    double tol, d[4] = {0.0, 0.0, 0.0, 0.0};
+    int32_t steps = 0;
+    float ms = 0.f;
+    jlong out[5];
+    memcpy(&tol, &tolBits, sizeof(tol));
+    const int32_t rc = rapid_view_overlay_spectrum(H(rapid_view, view), (uint64_t)seed, tol, maxSteps, &d[0], &d[1], &d[2], &steps, &ms);
+    d[3] = ms;
+    memcpy(&out[0], &d[0], 3 * sizeof(double));
+    out[3] = steps;
+    memcpy(&out[4], &d[3], sizeof(double));
+    if (rc == RAPID_OK) (*env)->SetLongArrayRegion(env, out5, 0, 5, out);
+    return rc;
+}
+
 /* ---------------------------------------------------------------- cut detector */
 JNIEXPORT jlong JNICALL Java_com_vrg_rapid_gpu_Native_cdCreate(JNIEnv* env, jclass c, jlong view, jint h, jint l, jlong receivers,
                                                                jlong begin, jint flags, jlong maxSubjects) {

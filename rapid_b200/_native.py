@@ -75,6 +75,7 @@ SIGNATURES = {
     "rapid_view_set_node_ids": [_vp, _p, _p],
     "rapid_view_set_joiner_ids": [_vp, _i32, _i64, _p, _p],
     "rapid_view_current_config_id": [_vp, _p],
+    "rapid_view_overlay_spectrum": [_vp, _u64, C.c_double, _i32, _p, _p, _p, _p, _p],
     "rapid_cd_debug_stats": [_vp, _p, _p, _p, _p],
     "rapid_cd_debug_grid": [_vp, _p, _p],
     "rapid_cd_create": [_pp, _vp, _i32, _i32, _i64, _i64, _u32, _i64],

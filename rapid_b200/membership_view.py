@@ -4,11 +4,15 @@ Method names and error behaviour follow rapid/src/main/java/com/vrg/rapid/Member
 tests read like the reference's MembershipViewTest; node ids (ints) stand for Endpoint objects.
 All results come from librapid_b200.so (CUDA); nothing is computed here.
 """
+import collections
 import ctypes as C
 
 import numpy as np
 
 from . import _native as N
+
+
+OverlaySpectrum = collections.namedtuple("OverlaySpectrum", "lambda2 lambda_min residual steps device_ms lambda_ ratio")
 
 
 class MembershipView:
@@ -149,3 +153,15 @@ class MembershipView:
         out = C.c_int64(0)
         N.check(N.lib().rapid_view_num_joiners(self._h, C.byref(out)))
         return out.value
+
+    def overlaySpectrum(self, seed=0, tol=1e-3, max_steps=256):
+        """Expansion of the monitoring overlay (rapid_view_overlay_spectrum): lambda2 and lambda_min, the largest and smallest
+        eigenvalue of the members' observer graph A = sum_k (P_k + P_k^T) below the trivial 2K; lambda_ = max(|lambda2|,
+        |lambda_min|) and ratio = lambda_ / 2K, the Rapid paper's expander figure; residual bounds the error of the two values
+        (the call stops at residual <= tol * 2K or after max_steps operator applications, steps says how many it spent)."""
+        l2, lmin, res = C.c_double(0), C.c_double(0), C.c_double(0)
+        steps, ms = C.c_int32(0), C.c_float(0)
+        N.check(N.lib().rapid_view_overlay_spectrum(self._h, int(seed) & 0xFFFFFFFFFFFFFFFF, float(tol), int(max_steps), C.byref(l2),
+                                                    C.byref(lmin), C.byref(res), C.byref(steps), C.byref(ms)))
+        lam = max(abs(l2.value), abs(lmin.value))
+        return OverlaySpectrum(l2.value, lmin.value, res.value, steps.value, ms.value, lam, lam / (2.0 * self.K))

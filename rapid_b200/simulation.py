@@ -48,6 +48,11 @@ ClusterSimulation rules (tests/simref.py restates them independently; DESIGN.md 
   meet the batches in different orders can announce different proposals; the records count them: intervals[i]["proposals"]
   is the number of distinct proposals announced in the interval, history[c]["distinct_proposals"] the number over the
   configuration.  Every node sees every vote, so one tally stands for every node's.
+* Overlay quality (overlay_quality=True; off by default, and then no record changes): every configuration record gains
+  overlay_ratio and overlay_residual, MembershipView.overlaySpectrum() (default seed, tolerance and step limit) of the view
+  AFTER that view change: lambda / 2K of its monitoring overlay and the bound on the error of lambda (DESIGN.md §4.13);
+  initial_overlay holds the same pair for the view the simulation started with.  Both are None for a view of fewer than 3
+  members, which has no such figure.
 """
 import time
 
@@ -93,7 +98,7 @@ class ClusterSimulation:
     configuration, intervals one per interval."""
 
     def __init__(self, endpoints, node_ids, K=10, H=9, L=4, seed=0, failure_threshold=FAILURE_THRESHOLD, fallback_intervals=1,
-                 device=0, batch_order="sender"):
+                 device=0, batch_order="sender", overlay_quality=False):
         if batch_order not in ("sender", "shuffled"):
             raise ValueError("batch_order is 'sender' or 'shuffled', not %r" % (batch_order,))
         self.batch_order = batch_order
@@ -120,6 +125,8 @@ class ClusterSimulation:
         self.fd = EdgeFailureDetectors(self.view, failure_threshold)
         self.fp = None
         self._new_handles()
+        self.overlay_quality = bool(overlay_quality)
+        self.initial_overlay = self._overlay() if self.overlay_quality else None
 
     # ---- scenario ------------------------------------------------------------------------------------------------------------
     def setFlags(self, node, flags):
@@ -354,6 +361,13 @@ class ClusterSimulation:
             self._ann = self.cl.readAnnounced()
         return self._ann
 
+    def _overlay(self):
+        """(ratio, residual) of the current view's monitoring overlay; (None, None) below 3 members"""
+        if self.view.n < 3:
+            return None, None
+        sp = self.view.overlaySpectrum()
+        return sp.ratio, sp.residual
+
     def _view_change(self, path, value, i):
         t0 = time.perf_counter()
         r = self._proposer if path == "classic" else self.acc.findValue(value)
@@ -385,6 +399,8 @@ class ClusterSimulation:
         self.history.append({"cfg_before": before, "cfg_after": self.cfg, "size_before": size_before, "size": self.view.n,
                              "cut": cut_tags, "path": path, "intervals": i + 1, "announced": announced,
                              "votes": votes, "members": sorted(self.tags.tolist()), "distinct_proposals": distinct, **times})
+        if self.overlay_quality:
+            self.history[-1]["overlay_ratio"], self.history[-1]["overlay_residual"] = self._overlay()
 
     # ---- whole runs --------------------------------------------------------------------------------------------------------------
     def run(self, max_intervals):
