@@ -539,6 +539,52 @@ int32_t rapid_px_phase2b_wire(rapid_px* px, const rapid_wire* w, int32_t* decide
 int32_t rapid_fp_tally_wire(rapid_fp* fp, const rapid_wire* w, int32_t* decided, uint64_t* decided_hash, uint64_t* decided_hash2,
                             int32_t* decided_len, int32_t* decided_count, int32_t* votes_received);
 
+/* Wire-format egress: the messages the virtual nodes send, serialized on the device exactly as the protobuf runtime serializes
+ * them (fields in field-number order, proto3 defaults omitted, a set submessage written even when empty, int32 / int64 values
+ * sign-extended: a negative port, configurationId or NodeId half takes 10 bytes), each alone or (flags = RAPID_WIRE_REQUEST)
+ * wrapped in a RapidRequest.  Message i = header i ++ body body_id[i] (no body when -1): the list-carrying kinds end with their
+ * list, and every message that carries one list shares one copy of its bytes (the distinct (h1, h2, len) fingerprints).  The
+ * encoder's outputs are the handle's own: a decode does not touch them nor an encode the last decode.  A refused encode
+ * (RAPID_EINVAL, nothing written) leaves the previous encode's outputs as they were.
+ *
+ * One BatchedAlertMessage{sender, messages} per sender of the fdet's last interval (tick, then merge), senders in node order:
+ * AlertMessage{edgeSrc = sender, edgeDst, edgeStatus, configurationId, ringNumber ascending and packed}, an UP (join) alert also
+ * with nodeId = the joiner's NodeId (rapid_view_set_joiner_ids; zero halves if the view holds none) and an empty metadata, as
+ * MembershipService.java:245-253 builds it; DOWN alerts as :486-492.  No bodies.  RAPID_EINVAL: fd created on another view or
+ * device, or no interval since its reset (or the view changed since).  *n_bytes = all the bytes of the messages. */
+int32_t rapid_wire_encode_alert_batches(rapid_wire* w, const rapid_fdet* fd, uint32_t flags, int64_t* n_messages, int64_t* n_bytes);
+/* One FastRoundPhase2bMessage{sender, configurationId = cfg_id, endpoints} per receiver of cd that announced in its last call
+ * (the receivers rapid_fp_tally_cd counts), in receiver order; receiver r's sender is the node at ring-0 position
+ * receiver_begin + r, its endpoints its proposal in canonical ring-0 order (rapid_cd_get_proposal).  One body per distinct
+ * proposal, numbered by its lowest receiver.  RAPID_EINVAL: cd created on another view or device, a RAW handle, or a handle that
+ * has applied no batch yet or was created before the view's members last changed. */
+int32_t rapid_wire_encode_votes(rapid_wire* w, const rapid_cd* cd, int64_t cfg_id, uint32_t flags, int64_t* n_messages, int64_t* n_bodies);
+/* One Phase1bMessage{sender, configurationId, rnd, vrnd, vval} per answer of the acceptors' last rapid_pxa_phase1a / one
+ * Phase2bMessage{sender, configurationId, rnd, endpoints} per answer of their last rapid_pxa_phase2a, as Paxos.java:136-142 /
+ * :207-212 build them (rnd and vrnd always set), in acceptor order; silent acceptors and those that did not answer send nothing.
+ * Acceptor g (acceptor_begin + local index) is the node at ring-0 position g of w's view, as a detector receiver is.  An empty
+ * vval has no body.  Each distinct list is taken from the lists this handle fetched before in the same membership (the votes it
+ * encoded: every registered vote and every Phase2a value is some announced proposal), else from the announced proposal of
+ * receiver g - receiver_begin of cd (may be NULL), which must match the list's fingerprint.  RAPID_EINVAL, nothing written: no
+ * answers of that kind pending, acceptors on another device or beyond the view, cd on another view / device / membership, or a
+ * list found in neither place. */
+int32_t rapid_wire_encode_phase1b(rapid_wire* w, const rapid_pxa* pxa, const rapid_cd* cd, uint32_t flags, int64_t* n_messages,
+                                  int64_t* n_bodies);
+int32_t rapid_wire_encode_phase2b(rapid_wire* w, const rapid_pxa* pxa, const rapid_cd* cd, uint32_t flags, int64_t* n_messages,
+                                  int64_t* n_bodies);
+/* The last encode: messages, header bytes, bodies, body bytes (all 0 before the first encode). */
+int32_t rapid_wire_encoded_counts(const rapid_wire* w, int64_t* n_messages, int64_t* header_bytes, int64_t* n_bodies, int64_t* body_bytes);
+/* Its outputs on the device (valid until the next encode on the handle) / host copies: headers[header_bytes],
+ * header_off[n_messages + 1], body_id[n_messages], bodies[body_bytes], body_off[n_bodies + 1].  Each may be NULL. */
+int32_t rapid_wire_encoded_dev(const rapid_wire* w, const uint8_t** headers, const int64_t** header_off, const int32_t** body_id,
+                               const uint8_t** bodies, const int64_t** body_off);
+int32_t rapid_wire_read_encoded(const rapid_wire* w, uint8_t* headers, int64_t* header_off, int32_t* body_id, uint8_t* bodies,
+                                int64_t* body_off);
+/* sizes[n_messages]: the whole size of every message, header + body, computed on the device. */
+int32_t rapid_wire_read_encoded_sizes(const rapid_wire* w, int64_t* sizes);
+/* sender[n_messages]: the view id of every message's sender. */
+int32_t rapid_wire_read_encoded_senders(const rapid_wire* w, int32_t* sender);
+
 /* ------------------------------------------------------------------------------------------------
  * Alert generation  (SURVEY.md §8 f4): PingPongFailureDetector.java:38-121 — one detector per entry of
  * getSubjectsOf(node), i.e. K per member (MembershipService.java:697-707) — and the AlertMessage a notifier

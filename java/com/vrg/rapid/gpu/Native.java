@@ -127,6 +127,26 @@ public final class Native {
     public static native int pxPhase2bWire(long px, long wire, long[] out5);
     public static native int fpTallyWire(long fp, long wire, long[] out6);
 
+    // ---- wire-format egress (the virtual nodes' messages -> rapid.proto bytes, encoded on the device) ----
+    /** one BatchedAlertMessage per sender of the fdet's last interval; out2 = {nMessages, nBytes} */
+    public static native int wireEncodeAlertBatches(long wire, long fdet, boolean asRequest, long[] out2);
+    /** one FastRoundPhase2bMessage per receiver of cd that announced in its last call; out2 = {nMessages, nBodies} */
+    public static native int wireEncodeVotes(long wire, long cd, long cfgId, boolean asRequest, long[] out2);
+    /** one Phase1bMessage / Phase2bMessage per answer of the pxa's last Phase1a / Phase2a; lists from the votes encoded before, else
+     *  from cd's receivers (cd may be 0); out2 = {nMessages, nBodies} */
+    public static native int wireEncodePhase1b(long wire, long pxa, long cd, boolean asRequest, long[] out2);
+    public static native int wireEncodePhase2b(long wire, long pxa, long cd, boolean asRequest, long[] out2);
+    /** the view id of every message's sender */
+    public static native int wireReadEncodedSenders(long wire, int[] sender);
+    /** the last encode: out4 = {nMessages, headerBytes, nBodies, bodyBytes} */
+    public static native int wireEncodedCounts(long wire, long[] out4);
+    /** its device pointers: out5 = {headers, headerOff, bodyId, bodies, bodyOff} */
+    public static native int wireEncodedDev(long wire, long[] out5);
+    /** host copies (each may be null): message i = headers[headerOff[i] .. headerOff[i+1]) ++ body bodyId[i] (none if -1) */
+    public static native int wireReadEncoded(long wire, byte[] headers, long[] headerOff, int[] bodyId, byte[] bodies, long[] bodyOff);
+    /** bytes of every message of the last encode, header + body */
+    public static native int wireReadEncodedSizes(long wire, long[] sizes);
+
     // ---- alert generation: the K PingPongFailureDetectors of every virtual node ----
     public static native long fdetCreate(long view, int failureThreshold, int bootstrapThreshold);
     public static native int fdetDestroy(long fdet);

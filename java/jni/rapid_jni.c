@@ -546,6 +546,96 @@ JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireDecodeConsensus(JNIEnv*
     (*env)->SetLongArrayRegion(env, out2, 0, 2, v);
     return rc;
 }
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireEncodeAlertBatches(JNIEnv* env, jclass c, jlong w, jlong fd, jboolean asRequest,
+                                                                            jlongArray out2) {
+    int64_t n = 0, bytes = 0;
+    const int32_t rc = rapid_wire_encode_alert_batches(H(rapid_wire, w), H(rapid_fdet, fd), asRequest ? RAPID_WIRE_REQUEST : 0, &n, &bytes);
+    const jlong v[2] = {(jlong)n, (jlong)bytes};
+    (*env)->SetLongArrayRegion(env, out2, 0, 2, v);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireEncodeVotes(JNIEnv* env, jclass c, jlong w, jlong cd, jlong cfg, jboolean asRequest,
+                                                                     jlongArray out2) {
+    int64_t n = 0, nb = 0;
+    const int32_t rc = rapid_wire_encode_votes(H(rapid_wire, w), H(rapid_cd, cd), cfg, asRequest ? RAPID_WIRE_REQUEST : 0, &n, &nb);
+    const jlong v[2] = {(jlong)n, (jlong)nb};
+    (*env)->SetLongArrayRegion(env, out2, 0, 2, v);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireEncodedCounts(JNIEnv* env, jclass c, jlong w, jlongArray out4) {
+    int64_t a = 0, b = 0, d = 0, e = 0;
+    const int32_t rc = rapid_wire_encoded_counts(H(rapid_wire, w), &a, &b, &d, &e);
+    const jlong v[4] = {(jlong)a, (jlong)b, (jlong)d, (jlong)e};
+    (*env)->SetLongArrayRegion(env, out4, 0, 4, v);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireEncodedDev(JNIEnv* env, jclass c, jlong w, jlongArray out5) {
+    const uint8_t *hdr = NULL, *bodies = NULL;
+    const int64_t *hoff = NULL, *boff = NULL;
+    const int32_t* bid = NULL;
+    const int32_t rc = rapid_wire_encoded_dev(H(rapid_wire, w), &hdr, &hoff, &bid, &bodies, &boff);
+    const jlong v[5] = {(jlong)(intptr_t)hdr, (jlong)(intptr_t)hoff, (jlong)(intptr_t)bid, (jlong)(intptr_t)bodies, (jlong)(intptr_t)boff};
+    (*env)->SetLongArrayRegion(env, out5, 0, 5, v);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireEncodePhase1b(JNIEnv* env, jclass c, jlong w, jlong pxa, jlong cd, jboolean asRequest,
+                                                                       jlongArray out2) {
+    int64_t n = 0, nb = 0;
+    const int32_t rc = rapid_wire_encode_phase1b(H(rapid_wire, w), H(rapid_pxa, pxa), H(rapid_cd, cd), asRequest ? RAPID_WIRE_REQUEST : 0, &n, &nb);
+    const jlong v[2] = {(jlong)n, (jlong)nb};
+    (*env)->SetLongArrayRegion(env, out2, 0, 2, v);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireEncodePhase2b(JNIEnv* env, jclass c, jlong w, jlong pxa, jlong cd, jboolean asRequest,
+                                                                       jlongArray out2) {
+    int64_t n = 0, nb = 0;
+    const int32_t rc = rapid_wire_encode_phase2b(H(rapid_wire, w), H(rapid_pxa, pxa), H(rapid_cd, cd), asRequest ? RAPID_WIRE_REQUEST : 0, &n, &nb);
+    const jlong v[2] = {(jlong)n, (jlong)nb};
+    (*env)->SetLongArrayRegion(env, out2, 0, 2, v);
+    return rc;
+}
+/* the read-backs write counts of the last encode: a Java array shorter than that is refused before anything is written */
+static int enc_short(JNIEnv* env, jarray a, int64_t need) { return a && (int64_t)(*env)->GetArrayLength(env, a) < need; }
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireReadEncoded(JNIEnv* env, jclass c, jlong w, jbyteArray headers, jlongArray headerOff,
+                                                                     jintArray bodyId, jbyteArray bodies, jlongArray bodyOff) {
+    int64_t n = 0, hb = 0, nb = 0, bb = 0;
+    int32_t rc = rapid_wire_encoded_counts(H(rapid_wire, w), &n, &hb, &nb, &bb);
+    if (rc) return rc;
+    if (enc_short(env, headers, hb) || enc_short(env, headerOff, n + 1) || enc_short(env, bodyId, n) || enc_short(env, bodies, bb) ||
+        enc_short(env, bodyOff, nb + 1)) return RAPID_EINVAL;
+    jbyte* h = headers ? (*env)->GetByteArrayElements(env, headers, NULL) : NULL;
+    jlong* ho = headerOff ? (*env)->GetLongArrayElements(env, headerOff, NULL) : NULL;
+    jint* bi = bodyId ? (*env)->GetIntArrayElements(env, bodyId, NULL) : NULL;
+    jbyte* b = bodies ? (*env)->GetByteArrayElements(env, bodies, NULL) : NULL;
+    jlong* bo = bodyOff ? (*env)->GetLongArrayElements(env, bodyOff, NULL) : NULL;
+    rc = rapid_wire_read_encoded(H(rapid_wire, w), (uint8_t*)h, (int64_t*)ho, (int32_t*)bi, (uint8_t*)b, (int64_t*)bo);
+    if (h) (*env)->ReleaseByteArrayElements(env, headers, h, 0);
+    if (ho) (*env)->ReleaseLongArrayElements(env, headerOff, ho, 0);
+    if (bi) (*env)->ReleaseIntArrayElements(env, bodyId, bi, 0);
+    if (b) (*env)->ReleaseByteArrayElements(env, bodies, b, 0);
+    if (bo) (*env)->ReleaseLongArrayElements(env, bodyOff, bo, 0);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireReadEncodedSizes(JNIEnv* env, jclass c, jlong w, jlongArray sizes) {
+    int64_t n = 0;
+    int32_t rc = rapid_wire_encoded_counts(H(rapid_wire, w), &n, NULL, NULL, NULL);
+    if (rc) return rc;
+    if (!sizes || enc_short(env, sizes, n)) return RAPID_EINVAL;
+    jlong* s = (*env)->GetLongArrayElements(env, sizes, NULL);
+    rc = rapid_wire_read_encoded_sizes(H(rapid_wire, w), (int64_t*)s);
+    (*env)->ReleaseLongArrayElements(env, sizes, s, 0);
+    return rc;
+}
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireReadEncodedSenders(JNIEnv* env, jclass c, jlong w, jintArray sender) {
+    int64_t n = 0;
+    int32_t rc = rapid_wire_encoded_counts(H(rapid_wire, w), &n, NULL, NULL, NULL);
+    if (rc) return rc;
+    if (!sender || enc_short(env, sender, n)) return RAPID_EINVAL;
+    jint* s = (*env)->GetIntArrayElements(env, sender, NULL);
+    rc = rapid_wire_read_encoded_senders(H(rapid_wire, w), (int32_t*)s);
+    (*env)->ReleaseIntArrayElements(env, sender, s, 0);
+    return rc;
+}
 JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_wireReadConsensus(JNIEnv* env, jclass c, jlong w, jintArray sender, jlongArray cfg,
                                                                        jintArray rndRound, jintArray rndNode, jintArray vrndRound,
                                                                        jintArray vrndNode, jlongArray hash, jlongArray hash2, jintArray len) {

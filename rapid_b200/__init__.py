@@ -10,10 +10,10 @@ from .membership_view import MembershipView
 from .cut_detector import MultiNodeCutDetector, VirtualCluster, proposal_fingerprint, UP, DOWN
 from .fast_paxos import FastPaxos, NcclComm, quorum
 from .classic_paxos import Paxos, PaxosAcceptors
-from .wire import WireDecoder
+from .wire import EncodedMessages, WireDecoder
 from .failure_detector import EdgeFailureDetectors
 from .simulation import ClusterSimulation
 
-__all__ = ["MembershipView", "MultiNodeCutDetector", "VirtualCluster", "FastPaxos", "NcclComm", "quorum", "Paxos", "PaxosAcceptors", "WireDecoder", "EdgeFailureDetectors", "ClusterSimulation",
+__all__ = ["MembershipView", "MultiNodeCutDetector", "VirtualCluster", "FastPaxos", "NcclComm", "quorum", "Paxos", "PaxosAcceptors", "WireDecoder", "EncodedMessages", "EdgeFailureDetectors", "ClusterSimulation",
            "proposal_fingerprint", "UP", "DOWN", "RapidError", "NodeNotInRingException",
            "NodeAlreadyInRingException", "UUIDAlreadySeenException", "HashCollisionError"]

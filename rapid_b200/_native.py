@@ -134,6 +134,15 @@ SIGNATURES = {
     "rapid_px_phase1b_wire": [_vp, _vp, _p, _p, _p, _p, _p, _p],
     "rapid_px_phase2b_wire": [_vp, _vp, _p, _p, _p, _p, _p],
     "rapid_fp_tally_wire": [_vp, _vp, _p, _p, _p, _p, _p, _p],
+    "rapid_wire_encode_alert_batches": [_vp, _vp, _u32, _p, _p],
+    "rapid_wire_encode_votes": [_vp, _vp, _i64, _u32, _p, _p],
+    "rapid_wire_encoded_counts": [_vp, _p, _p, _p, _p],
+    "rapid_wire_encoded_dev": [_vp, _p, _p, _p, _p, _p],
+    "rapid_wire_read_encoded": [_vp, _p, _p, _p, _p, _p],
+    "rapid_wire_read_encoded_sizes": [_vp, _p],
+    "rapid_wire_encode_phase1b": [_vp, _vp, _vp, _u32, _p, _p],
+    "rapid_wire_encode_phase2b": [_vp, _vp, _vp, _u32, _p, _p],
+    "rapid_wire_read_encoded_senders": [_vp, _p],
     "rapid_fdet_create": [_pp, _vp, _i32, _i32],
     "rapid_fdet_destroy": [_vp],
     "rapid_fdet_reset": [_vp],

@@ -837,6 +837,7 @@ int32_t rapid_cd_create(rapid_cd** out, const rapid_view* v, int32_t H, int32_t 
     DeviceGuard g(view->device);
     rapid_cd* cd = new rapid_cd();
     cd->view = view;
+    cd->member_epoch = view->member_epoch;
     cd->device = view->device;
     cd->K = K; cd->H = H; cd->L = L;
     cd->mode = mode_flags;

@@ -68,6 +68,7 @@ struct CD {
     uint32_t mode = 0;
     bool raw = false, bucketed = false;
     int64_t R = 0, rbegin = 0;
+    uint64_t member_epoch = 0;        // the view's member_epoch at creation: receivers are ring-0 positions of THAT view
     size_t Rpad = 0;
     int nbuf = 1;                     // 2 = double-buffered rows (bucketed handles)
     int32_t S = 0;                    // slots in use (host mirror; bucketed handles: as of the last synchronisation point)

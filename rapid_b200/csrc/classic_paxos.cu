@@ -22,13 +22,6 @@
 
 namespace rapid {
 
-// (round, node_index) -> one signed 64-bit word whose order is compareRanks' (Paxos.java:333-339)
-RAPID_HD int64_t pack_rank(int32_t round, int32_t node) {
-    return (int64_t)(((uint64_t)(uint32_t)round << 32) | (uint64_t)((uint32_t)node ^ 0x80000000u));
-}
-RAPID_HD int32_t rank_round(int64_t p) { return (int32_t)((uint64_t)p >> 32); }
-RAPID_HD int32_t rank_node(int64_t p) { return (int32_t)((uint32_t)(uint64_t)p ^ 0x80000000u); }
-
 struct PxScal {
     long long max_rank;
     int32_t first_nonempty, first_collected, n_collected, distinct, kth_min, chosen;
@@ -743,6 +736,13 @@ using namespace rapid;
 
 struct rapid_px : rapid::PX {};
 struct rapid_pxa : rapid::PXA {};
+
+void rapid::pxa_answers_dev(const rapid_pxa* a, PxaAnswers* out) {
+    out->device = a->device; out->kind = a->last_kind; out->cfg = a->cfg; out->R = a->R; out->begin = a->begin;
+    out->n = a->n_out; out->rank = a->last_rank;
+    out->sender = a->o_sender.p; out->vrnd = a->o_vr.p; out->h1 = a->o_h1.p; out->h2 = a->o_h2.p; out->len = a->o_len.p;
+    out->v_h1 = a->last_h1; out->v_h2 = a->last_h2; out->v_len = a->last_len;
+}
 
 // Gather the pending answers of `want` kind (1 Phase1b, 2 Phase2b) of this rank's shards and, with a comm, of every rank's into
 // px->sh_* in ascending sender.  Every refusal that depends on the shards is decided from the gathered header table, which is

@@ -12,6 +12,7 @@
 #include "common.cuh"
 #include "radix.cuh"
 #include "scan.cuh"
+#include "wire_internal.cuh"
 
 namespace rapid {
 
@@ -261,6 +262,14 @@ static int32_t fd_tick_device(FD* fd, const uint8_t* d_flags, const uint8_t* d_e
 using namespace rapid;
 
 struct rapid_fdet : rapid::FD {};
+
+void rapid::fdet_interval_dev(const rapid_fdet* fd, FdetInterval* out) {
+    out->view = fd->view; out->device = fd->device;
+    out->have = fd->tick_flags != nullptr && fd->view_epoch == fd->view->member_epoch && fd->n == fd->view->n;
+    out->n_alerts = fd->n_alerts;
+    out->obs = fd->a_obs.p; out->subj = fd->a_subj.p; out->mask = fd->a_mask.p;
+    out->cell_status = fd->c_status.p; out->cell_cfg = fd->c_cfg.p;
+}
 
 extern "C" {
 

@@ -482,6 +482,7 @@ struct Wire {
     DevBuf<uint64_t> c_h1, c_h2;
     DevBuf<int32_t> i_off, i_len, i_msg, i_id;
     DevBuf<uint64_t> i_m1, i_m2;
+    WireEnc* enc = nullptr;           // the encoder's outputs and scratch (wire_encode.cu)
 };
 
 static const int TB = 128;
@@ -620,6 +621,10 @@ int32_t rapid::wire_consensus_dev(const rapid_wire* w, int32_t kind, WireMsgs* o
     return RAPID_OK;
 }
 
+void rapid::wire_enc_ctx(rapid_wire* w, WireEncCtx* out) {
+    out->view = w->view; out->device = w->device; out->stream = w->stream; out->enc = &w->enc;
+}
+
 extern "C" {
 
 int32_t rapid_wire_create(rapid_wire** out, rapid_view* v) {
@@ -651,6 +656,7 @@ int32_t rapid_wire_destroy(rapid_wire* w) {
     if (w->stream) { cudaStreamSynchronize(w->stream); cudaStreamDestroy(w->stream); }
     if (w->ev0) cudaEventDestroy(w->ev0);
     if (w->ev1) cudaEventDestroy(w->ev1);
+    wire_enc_free(w->enc);
     delete w;
     return RAPID_OK;
 }

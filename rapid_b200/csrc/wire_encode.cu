@@ -1,0 +1,772 @@
+// Wire-format egress (DESIGN §4.14): the messages a virtual cluster sends, serialized on the device as the protobuf runtime
+// serializes them (rapid.proto:13-17, 95-129), optionally wrapped in RapidRequest.
+//
+// A message is a HEADER plus, for the kinds whose last field is a list, a BODY shared by every message that carries the same
+// list: canonical bytes = header ++ body, because fields are serialized in field-number order and the list is the highest.
+// Bodies are the distinct (h1, h2, len) fingerprints of the lists (the identity the tally already counts votes by), found on the
+// device with an open-addressing table; each is encoded once, one thread per list ENTRY, from the canonical list of its lowest
+// receiver.  Every kind is count -> exclusive scan -> emit, the scheme of the decoder (wire.cu), with the int32 scans of scan.cuh.
+// Outputs are double-buffered: an encode writes the spare set and swaps on success, so a refused or failed encode leaves the
+// previous outputs as they were.
+#include <limits.h>
+
+#include <algorithm>
+#include <functional>
+#include <map>
+#include <tuple>
+#include <vector>
+
+#include "cd_internal.cuh"
+#include "common.cuh"
+#include "scan.cuh"
+#include "wire_internal.cuh"
+
+namespace rapid {
+
+// ------------------------------------------------------------------ protobuf primitives
+RAPID_HD int32_t vsz(uint64_t v) {                  // bytes of a varint
+    int32_t n = 1;
+    while (v >= 0x80) { v >>= 7; ++n; }
+    return n;
+}
+// an int32 / int64 / enum field is the varint of the value sign-extended to 64 bits: a negative one takes 10 bytes
+RAPID_HD uint64_t sx(int64_t v) { return (uint64_t)v; }
+RAPID_HD int32_t msg_field(int32_t content) { return 1 + vsz((uint64_t)content) + content; }   // tag (field <= 15), length, content
+
+__device__ __forceinline__ uint8_t* put_varint(uint8_t* p, uint64_t v) {
+    while (v >= 0x80) { *p++ = (uint8_t)(v | 0x80); v >>= 7; }
+    *p++ = (uint8_t)v;
+    return p;
+}
+
+// the view's endpoint table (members, then registered joiners)
+struct EpTab {
+    const uint8_t* hb;
+    const int32_t* hoff;
+    const int32_t* port;
+};
+// Endpoint content: hostname (1, omitted when empty), port (2, omitted when 0)
+__device__ __forceinline__ int32_t ep_size(const EpTab& t, int32_t id) {
+    const int32_t hl = t.hoff[id + 1] - t.hoff[id], port = t.port[id];
+    return (hl ? 1 + vsz((uint64_t)hl) + hl : 0) + (port ? 1 + vsz(sx(port)) : 0);
+}
+// a SET Endpoint field: serialized even when its content is empty
+__device__ uint8_t* put_ep_field(uint8_t* p, uint8_t tag, const EpTab& t, int32_t id) {
+    const int32_t hl = t.hoff[id + 1] - t.hoff[id], port = t.port[id];
+    *p++ = tag;
+    p = put_varint(p, (uint64_t)ep_size(t, id));
+    if (hl) {
+        *p++ = 0x0A;
+        p = put_varint(p, (uint64_t)hl);
+        const uint8_t* s = t.hb + t.hoff[id];
+        for (int32_t i = 0; i < hl; ++i) p[i] = s[i];
+        p += hl;
+    }
+    if (port) { *p++ = 0x10; p = put_varint(p, sx(port)); }
+    return p;
+}
+
+struct EncScal {
+    int32_t n_msgs, n_bodies, n_heads, n_entries;
+    int32_t hdr_bytes, body_bytes, alert_bytes, pad_;
+    unsigned long long bytes64;        // the entries' bytes summed in 64 bits: an encode whose offsets would not fit int32 is refused
+};
+
+// ------------------------------------------------------------------ alert batches (rapid.proto:95-110)
+struct AlertIn {
+    int32_t n;
+    const int32_t* obs;
+    const int32_t* subj;
+    const uint16_t* mask;
+    const uint8_t* status;             // per cell
+    const int64_t* cfg;                // per cell
+    const int32_t* cpos;               // first cell of each alert
+    const int64_t* nid_hi;             // NodeIds by view id, NULL: the view holds none (zero halves)
+    const int64_t* nid_lo;
+};
+
+__device__ __forceinline__ int32_t nid_size(int64_t hi, int64_t lo) { return (hi ? 1 + vsz(sx(hi)) : 0) + (lo ? 1 + vsz(sx(lo)) : 0); }
+
+struct AlertFields {
+    uint8_t st;
+    int64_t cfg, hi, lo;
+};
+// AlertMessage content as MembershipService builds it: edgeSrc, edgeDst, edgeStatus (omitted when UP), configurationId (omitted
+// when 0), ringNumber packed and ascending; an UP alert also sets nodeId (:250) and metadata (:252, empty: the device holds none)
+__device__ int32_t alert_size(const AlertIn& a, const EpTab& t, int32_t i, AlertFields* f) {
+    const int32_t c = a.cpos[i];
+    f->st = a.status[c];
+    f->cfg = a.cfg[c];
+    f->hi = f->lo = 0;
+    const int32_t nr = __popc((uint32_t)a.mask[i]);
+    int32_t s = msg_field(ep_size(t, a.obs[i])) + msg_field(ep_size(t, a.subj[i])) + (f->st ? 2 : 0) +
+                (f->cfg ? 1 + vsz(sx(f->cfg)) : 0) + 1 + vsz((uint64_t)nr) + nr;   // ring numbers < RAPID_MAX_K: one byte each
+    if (f->st == RAPID_EDGE_UP) {
+        if (a.nid_hi) { f->hi = a.nid_hi[a.subj[i]]; f->lo = a.nid_lo[a.subj[i]]; }
+        s += msg_field(nid_size(f->hi, f->lo)) + 2;
+    }
+    return s;
+}
+
+__global__ void k_enc_popc(int32_t n, const uint16_t* __restrict__ mask, int32_t* __restrict__ cnt) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) cnt[i] = __popc((uint32_t)mask[i]);
+}
+// per alert: the size of its entry in BatchedAlertMessage.messages, and whether it opens a sender's batch
+__global__ void k_enc_alert_sizes(AlertIn a, EpTab t, int32_t* __restrict__ esz, int32_t* __restrict__ head, EncScal* __restrict__ sc) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n) return;
+    AlertFields f;
+    const int32_t e = msg_field(alert_size(a, t, i, &f));
+    esz[i] = e;
+    head[i] = (i == 0 || a.obs[i] != a.obs[i - 1]) ? 1 : 0;
+    atomicAdd(&sc->bytes64, (unsigned long long)e);
+}
+// per batch (the thread of the alert that opens it): its first alert, its header size and the whole message's size
+__global__ void k_enc_batch_sizes(int32_t n, const int32_t* __restrict__ obs, const int32_t* __restrict__ head,
+                                  const int32_t* __restrict__ bpos, const int32_t* __restrict__ epos, const EncScal* __restrict__ sc,
+                                  EpTab t, int wrap, int32_t* __restrict__ start, int32_t* __restrict__ hlen, int32_t* __restrict__ msz) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || !head[i]) return;
+    const int32_t b = bpos[i];
+    int32_t j = i + 1;                                                       // the next batch's first alert: a batch is <= ~2K alerts
+    while (j < n && !head[j]) ++j;
+    const int32_t body = (j < n ? epos[j] : sc->alert_bytes) - epos[i];
+    const int32_t content = msg_field(ep_size(t, obs[i])) + body;
+    const int32_t h = (wrap ? 1 + vsz((uint64_t)content) : 0) + content - body;
+    start[b] = i; hlen[b] = h; msz[b] = h + body;
+}
+// the batch's header: [RapidRequest tag 3, length] BatchedAlertMessage.sender
+__global__ void k_enc_batch_emit(int32_t nb, const int32_t* __restrict__ start, const int32_t* __restrict__ hlen,
+                                 const int32_t* __restrict__ msz, const int32_t* __restrict__ hpos, const int32_t* __restrict__ obs,
+                                 EpTab t, int wrap, int32_t* __restrict__ m_snd, uint8_t* __restrict__ out) {
+    const int32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nb) return;
+    uint8_t* p = out + hpos[b];
+    const int32_t s = obs[start[b]];
+    m_snd[b] = s;
+    if (wrap) {
+        const int32_t content = msz[b] - hlen[b] + msg_field(ep_size(t, s));
+        *p++ = 0x1A;
+        p = put_varint(p, (uint64_t)content);
+    }
+    put_ep_field(p, 0x0A, t, s);
+}
+// per alert: its entry (tag 3, length, AlertMessage) at its place in its sender's message
+__global__ void k_enc_alert_emit(AlertIn a, EpTab t, const int32_t* __restrict__ head, const int32_t* __restrict__ bpos,
+                                 const int32_t* __restrict__ epos, const int32_t* __restrict__ start, const int32_t* __restrict__ hlen,
+                                 const int32_t* __restrict__ hpos, uint8_t* __restrict__ out) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n) return;
+    const int32_t b = bpos[i] + head[i] - 1;                                 // bpos: exclusive count of batch openers
+    uint8_t* p = out + hpos[b] + hlen[b] + (epos[i] - epos[start[b]]);
+    AlertFields f;
+    const int32_t sz = alert_size(a, t, i, &f);
+    *p++ = 0x1A;
+    p = put_varint(p, (uint64_t)sz);
+    p = put_ep_field(p, 0x0A, t, a.obs[i]);
+    p = put_ep_field(p, 0x12, t, a.subj[i]);
+    if (f.st) { *p++ = 0x18; *p++ = f.st; }
+    if (f.cfg) { *p++ = 0x20; p = put_varint(p, sx(f.cfg)); }
+    const uint32_t m = a.mask[i];
+    *p++ = 0x2A;
+    *p++ = (uint8_t)__popc(m);
+    for (uint32_t r = 0; r < 16; ++r) if ((m >> r) & 1u) *p++ = (uint8_t)r;
+    if (f.st == RAPID_EDGE_UP) {
+        *p++ = 0x32;
+        p = put_varint(p, (uint64_t)nid_size(f.hi, f.lo));
+        if (f.hi) { *p++ = 0x08; p = put_varint(p, sx(f.hi)); }
+        if (f.lo) { *p++ = 0x10; p = put_varint(p, sx(f.lo)); }
+        *p++ = 0x3A; *p++ = 0x00;
+    }
+}
+
+// ------------------------------------------------------------------ list-carrying messages (rapid.proto:124-169)
+// One slot per candidate message: a detector receiver (FastRoundPhase2bMessage: it sends iff it announced in the last call) or a
+// pending acceptor answer (Phase1bMessage, Phase2bMessage: every slot sends).  Each kind ends with its endpoint list.
+struct ListIn {
+    int32_t n;
+    int32_t kind;                       // RAPID_WIRE_FAST_ROUND_PHASE2B, RAPID_WIRE_PHASE1B or RAPID_WIRE_PHASE2B
+    int wrap;
+    int64_t cfg;
+    const uint32_t* rflags;             // votes; NULL: every slot sends
+    const int32_t* acc;                 // answers: the sender's acceptor index, a ring-0 position; NULL: rbegin + slot
+    int64_t rbegin;
+    const int32_t* ring0;
+    const uint64_t* h1;                 // the slot's list fingerprint; NULL: the constant (c1, c2, clen) of a Phase2a value
+    const uint64_t* h2;
+    const int32_t* len;
+    uint64_t c1, c2;
+    int32_t clen;
+    const int64_t* vrnd;                // Phase1b: per slot
+    int64_t rank;                       // Phase1b / Phase2b: rnd (packed, see pack_rank)
+};
+__device__ __forceinline__ void list_fp(const ListIn& L, int32_t s, uint64_t* a, uint64_t* b, int32_t* l) {
+    if (L.h1) { *a = L.h1[s]; *b = L.h2[s]; *l = L.len[s]; } else { *a = L.c1; *b = L.c2; *l = L.clen; }
+}
+__device__ __forceinline__ bool list_sends(const ListIn& L, int32_t s) { return !L.rflags || (L.rflags[s] & RF_ANN_NOW); }
+__device__ __forceinline__ int32_t list_sender(const ListIn& L, int32_t s) { return L.ring0[L.acc ? L.acc[s] : L.rbegin + s]; }
+// Rank {round = 1, nodeIndex = 2}, int32 fields
+__device__ __forceinline__ int32_t rank_size(int64_t p) {
+    const int32_t r = rank_round(p), q = rank_node(p);
+    return (r ? 1 + vsz(sx(r)) : 0) + (q ? 1 + vsz(sx(q)) : 0);
+}
+__device__ uint8_t* put_rank_field(uint8_t* p, uint8_t tag, int64_t rk) {        // a SET Rank: written even when (0, 0)
+    const int32_t r = rank_round(rk), q = rank_node(rk);
+    *p++ = tag;
+    p = put_varint(p, (uint64_t)rank_size(rk));
+    if (r) { *p++ = 0x08; p = put_varint(p, sx(r)); }
+    if (q) { *p++ = 0x10; p = put_varint(p, sx(q)); }
+    return p;
+}
+RAPID_HD uint8_t list_tag(int32_t kind) {                                  // endpoints = 3 / vval = 5 / endpoints = 4
+    return kind == RAPID_WIRE_FAST_ROUND_PHASE2B ? 0x1A : kind == RAPID_WIRE_PHASE1B ? 0x2A : 0x22;
+}
+
+// every slot with a non-empty list claims the table slot of the list's fingerprint; the slot keeps the LOWEST such slot (the
+// body's representative)
+__global__ void k_enc_list_claim(ListIn L, uint32_t T, int32_t* __restrict__ table, int32_t* __restrict__ slot, int32_t* __restrict__ send) {
+    const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= L.n) return;
+    const bool v = list_sends(L, s);
+    send[s] = v ? 1 : 0;
+    uint64_t a, b; int32_t l;
+    list_fp(L, s, &a, &b, &l);
+    if (!v || l <= 0) { slot[s] = -1; return; }
+    uint32_t pos = (uint32_t)(splitmix64(a ^ (b * 0x9E3779B97F4A7C15ULL) ^ (uint64_t)l) >> 32) & (T - 1);
+    for (;;) {
+        int32_t cur = table[pos];
+        if (cur < 0) {
+            cur = atomicCAS(&table[pos], -1, s);
+            if (cur < 0) break;
+        }
+        uint64_t ca, cb; int32_t cl;
+        list_fp(L, cur, &ca, &cb, &cl);
+        if (ca == a && cb == b && cl == l) { atomicMin(&table[pos], s); break; }
+        pos = (pos + 1) & (T - 1);
+    }
+    slot[s] = (int32_t)pos;
+}
+__global__ void k_enc_list_rep(int32_t n, const int32_t* __restrict__ slot, const int32_t* __restrict__ table, int32_t* __restrict__ rep) {
+    const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < n) rep[s] = (slot[s] >= 0 && table[slot[s]] == s) ? 1 : 0;
+}
+// body id of every slot (bodies numbered by ascending representative, -1: no list), and the representatives in body order
+__global__ void k_enc_list_bodies(int32_t n, const int32_t* __restrict__ slot, const int32_t* __restrict__ table,
+                                  const int32_t* __restrict__ rep, const int32_t* __restrict__ rpos, int32_t* __restrict__ bid_s,
+                                  int32_t* __restrict__ reps) {
+    const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    bid_s[s] = slot[s] >= 0 ? rpos[table[slot[s]]] : -1;
+    if (rep[s]) reps[rpos[s]] = s;
+}
+__global__ void k_enc_gather_fp(int32_t nb, ListIn L, const int32_t* __restrict__ reps, uint64_t* __restrict__ g1, uint64_t* __restrict__ g2,
+                                int32_t* __restrict__ gl, int32_t* __restrict__ gacc) {
+    const int32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nb) return;
+    const int32_t s = reps[b];
+    list_fp(L, s, &g1[b], &g2[b], &gl[b]);
+    gacc[b] = L.acc ? L.acc[s] : (int32_t)(L.rbegin + s);
+}
+// one thread per list entry: its size as a repeated Endpoint field
+__global__ void k_enc_entry_sizes(int32_t n, const int32_t* __restrict__ ids, EpTab t, int32_t* __restrict__ sz, EncScal* __restrict__ sc) {
+    const int32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const int32_t s = msg_field(ep_size(t, ids[j]));
+    sz[j] = s;
+    atomicAdd(&sc->bytes64, (unsigned long long)s);
+}
+__global__ void k_enc_entry_emit(int32_t n, const int32_t* __restrict__ ids, EpTab t, uint8_t tag, const int32_t* __restrict__ pos,
+                                 uint8_t* __restrict__ out) {
+    const int32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < n) put_ep_field(out + pos[j], tag, t, ids[j]);
+}
+// body b = entries [first[b], first[b + 1]): its byte range
+__global__ void k_enc_body_off(int32_t nb, int32_t n_entries, const int32_t* __restrict__ first, const int32_t* __restrict__ pos,
+                               const EncScal* __restrict__ sc, int64_t* __restrict__ boff) {
+    const int32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b > nb) return;
+    const int32_t e = first[b];
+    boff[b] = e < n_entries ? pos[e] : sc->body_bytes;
+}
+// per sending slot: header = [RapidRequest tag, length] sender, configurationId (omitted when 0), and the kind's ranks (Phase1b:
+// rnd, vrnd; Phase2b: rnd; both set, so written even when (0, 0))
+__device__ __forceinline__ int32_t list_header(const ListIn& L, const EpTab& t, const int32_t* bid, const int64_t* boff, int32_t s,
+                                               int32_t* content) {
+    const int32_t b = bid[s];
+    const int32_t body = b >= 0 ? (int32_t)(boff[b + 1] - boff[b]) : 0;
+    int32_t own = msg_field(ep_size(t, list_sender(L, s))) + (L.cfg ? 1 + vsz(sx(L.cfg)) : 0);
+    if (L.kind != RAPID_WIRE_FAST_ROUND_PHASE2B) own += msg_field(rank_size(L.rank));
+    if (L.kind == RAPID_WIRE_PHASE1B) own += msg_field(rank_size(L.vrnd[s]));
+    *content = own + body;
+    return (L.wrap ? 1 + vsz((uint64_t)*content) : 0) + own;
+}
+__global__ void k_enc_list_sizes(ListIn L, EpTab t, const int32_t* __restrict__ send, const int32_t* __restrict__ mpos,
+                                 const int32_t* __restrict__ bid, const int64_t* __restrict__ boff, int32_t* __restrict__ hsz) {
+    const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= L.n || !send[s]) return;
+    int32_t content;
+    hsz[mpos[s]] = list_header(L, t, bid, boff, s, &content);
+}
+__global__ void k_enc_list_emit(ListIn L, EpTab t, const int32_t* __restrict__ send, const int32_t* __restrict__ mpos,
+                                const int32_t* __restrict__ bid, const int64_t* __restrict__ boff, const int32_t* __restrict__ hpos,
+                                int32_t* __restrict__ m_bid, int32_t* __restrict__ m_snd, uint8_t* __restrict__ out) {
+    const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= L.n || !send[s]) return;
+    const int32_t m = mpos[s];
+    int32_t content;
+    list_header(L, t, bid, boff, s, &content);
+    uint8_t* p = out + hpos[m];
+    if (L.wrap) { *p++ = (uint8_t)((L.kind << 3) | 2); p = put_varint(p, (uint64_t)content); }
+    const int32_t snd = list_sender(L, s);
+    p = put_ep_field(p, 0x0A, t, snd);
+    if (L.cfg) { *p++ = 0x10; p = put_varint(p, sx(L.cfg)); }
+    if (L.kind != RAPID_WIRE_FAST_ROUND_PHASE2B) p = put_rank_field(p, 0x1A, L.rank);
+    if (L.kind == RAPID_WIRE_PHASE1B) p = put_rank_field(p, 0x22, L.vrnd[s]);
+    m_bid[m] = bid[s];
+    m_snd[m] = snd;
+}
+
+// ------------------------------------------------------------------ offsets, sizes
+__global__ void k_enc_off64(int32_t n, const int32_t* __restrict__ pos, const int32_t* __restrict__ total, int64_t* __restrict__ off) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) off[i] = pos[i];
+    if (i == n) off[i] = *total;
+}
+__global__ void k_enc_fill(int32_t n, int32_t v, int32_t* __restrict__ a) {
+    const int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) a[i] = v;
+}
+__global__ void k_enc_sizes(int64_t n, const int64_t* __restrict__ hoff, const int32_t* __restrict__ bid, const int64_t* __restrict__ boff,
+                            int64_t* __restrict__ out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int32_t b = bid[i];
+    out[i] = hoff[i + 1] - hoff[i] + (b >= 0 ? boff[b + 1] - boff[b] : 0);
+}
+
+// ------------------------------------------------------------------ state
+struct EncOut {
+    int64_t n = 0, n_bodies = 0, hdr_bytes = 0, body_bytes = 0;
+    DevBuf<uint8_t> hdr, bodies;
+    DevBuf<int64_t> hoff, boff;        // [n + 1], [n_bodies + 1]
+    DevBuf<int32_t> bid;               // [n]: body of each message, -1 for none
+    DevBuf<int32_t> snd;               // [n]: view id of each message's sender
+};
+
+struct WireEnc {
+    EncOut out[2];
+    int cur = 0;                       // out[cur] holds the last successful encode
+    DevBuf<int32_t> a, b, c, d, e, f, g, scan_sums;
+    DevBuf<int32_t> table, ids, ids2, epos, gl, gacc;
+    DevBuf<uint64_t> g1, g2;
+    DevBuf<int64_t> sizes;
+    DevBuf<EncScal> sc;
+    PinnedBuf<EncScal> h_sc;
+    // the lists already fetched as ids, by (h1, h2, len), for the view's member_epoch `lists_epoch`: a vval or Phase2a value is
+    // looked up here first (the votes encoded earlier hold every proposal the acceptors can have registered)
+    std::map<std::tuple<uint64_t, uint64_t, int32_t>, std::vector<int32_t>> lists;
+    uint64_t lists_epoch = 0;
+};
+
+static const int TB = 256;
+static inline unsigned grid_for(int64_t n) { return (unsigned)ceil_div<int64_t>(n > 0 ? n : 1, TB); }
+
+void wire_enc_free(WireEnc* e) { delete e; }
+
+static int32_t enc_get(rapid_wire* w, WireEncCtx* ctx, WireEnc** out) {
+    wire_enc_ctx(w, ctx);
+    if (!*ctx->enc) {
+        WireEnc* e = new WireEnc();
+        int32_t rc;
+        if ((rc = e->sc.reserve(1)) || (rc = e->h_sc.reserve(1))) { delete e; return rc; }
+        for (EncOut& o : e->out) {                                   // an empty encode: offsets {0}
+            if ((rc = o.hoff.reserve(1)) || (rc = o.boff.reserve(1))) { delete e; return rc; }
+            RAPID_CUDA(cudaMemsetAsync(o.hoff.p, 0, sizeof(int64_t), ctx->stream));
+            RAPID_CUDA(cudaMemsetAsync(o.boff.p, 0, sizeof(int64_t), ctx->stream));
+        }
+        *ctx->enc = e;
+    }
+    *out = *ctx->enc;
+    return RAPID_OK;
+}
+
+static int32_t enc_read_scal(WireEnc* e, cudaStream_t s) {
+    RAPID_CUDA(cudaMemcpyAsync(e->h_sc.p, e->sc.p, sizeof(EncScal), cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    return RAPID_OK;
+}
+
+static EpTab ep_tab(const View* v) { return EpTab{v->host_bytes.p, v->host_off.p, v->port.p}; }
+
+static const int64_t ENC_LIMIT = 0x7ff00000LL;   // bytes of one encode's headers or bodies (int32 offsets in the scans)
+
+static int32_t too_big() { set_error("the encoded messages would exceed 2^31 bytes"); return RAPID_ENOMEM; }
+
+// BatchedAlertMessage of every sender of the fdet's last interval
+static int32_t encode_alerts(WireEnc* e, const WireEncCtx& ctx, const FdetInterval& in, uint32_t flags) {
+    cudaStream_t s = ctx.stream;
+    EncOut& o = e->out[1 - e->cur];
+    const int32_t n = (int32_t)in.n_alerts;
+    const int wrap = (flags & RAPID_WIRE_REQUEST) ? 1 : 0;
+    const EpTab t = ep_tab(ctx.view);
+    RAPID_CUDA(cudaMemsetAsync(e->sc.p, 0, sizeof(EncScal), s));
+    int64_t nb = 0, hbytes = 0;
+    if (n > 0) {
+        const size_t N = (size_t)n;
+        RAPID_CHECK(e->a.reserve(N)); RAPID_CHECK(e->b.reserve(N)); RAPID_CHECK(e->c.reserve(N)); RAPID_CHECK(e->d.reserve(N));
+        RAPID_CHECK(e->f.reserve(N)); RAPID_CHECK(e->g.reserve(N)); RAPID_CHECK(e->e.reserve(N + 1));
+        int32_t *cpos = e->a.p, *esz = e->b.p, *epos = e->b.p, *head = e->c.p, *bpos = e->d.p;
+        int32_t *start = e->e.p, *hlen = e->f.p, *msz = e->g.p;
+        k_enc_popc<<<grid_for(n), TB, 0, s>>>(n, in.mask, cpos);
+        RAPID_KERNEL_CHECK();
+        RAPID_CHECK(exclusive_scan_i32(cpos, n, e->scan_sums, nullptr, s, nullptr));
+        const bool nid = ctx.view->has_node_ids;
+        const AlertIn a{n, in.obs, in.subj, in.mask, in.cell_status, in.cell_cfg, cpos, nid ? ctx.view->node_hi.p : nullptr,
+                        nid ? ctx.view->node_lo.p : nullptr};
+        k_enc_alert_sizes<<<grid_for(n), TB, 0, s>>>(a, t, esz, head, e->sc.p);
+        RAPID_KERNEL_CHECK();
+        RAPID_CHECK(enc_read_scal(e, s));
+        // + one sender field per alert at most: a bound on the headers too
+        if ((int64_t)e->h_sc.p->bytes64 > ENC_LIMIT / 2) return too_big();
+        RAPID_CHECK(exclusive_scan_i32(epos, n, e->scan_sums, &e->sc.p->alert_bytes, s, nullptr));      // in place: esz -> epos
+        RAPID_CHECK(exclusive_scan_i32_to(head, bpos, n, e->scan_sums, s));
+        k_enc_batch_sizes<<<grid_for(n), TB, 0, s>>>(n, in.obs, head, bpos, epos, e->sc.p, t, wrap, start, hlen, msz);
+        RAPID_KERNEL_CHECK();
+        // one batch per sender: the exclusive count of openers at the last alert, plus whether it opens one
+        int32_t last[2] = {0, 0};
+        RAPID_CUDA(cudaMemcpyAsync(&last[0], bpos + n - 1, 4, cudaMemcpyDeviceToHost, s));
+        RAPID_CUDA(cudaMemcpyAsync(&last[1], head + n - 1, 4, cudaMemcpyDeviceToHost, s));
+        RAPID_CUDA(cudaStreamSynchronize(s));
+        nb = last[0] + last[1];
+        RAPID_CHECK(o.hoff.reserve((size_t)nb + 1)); RAPID_CHECK(o.bid.reserve((size_t)nb)); RAPID_CHECK(o.snd.reserve((size_t)nb));
+        RAPID_CHECK(e->ids.reserve((size_t)nb));
+        int32_t* hpos = e->ids.p;
+        RAPID_CHECK(exclusive_scan_i32(hpos, nb, e->scan_sums, &e->sc.p->hdr_bytes, s, nullptr, msz));
+        RAPID_CHECK(enc_read_scal(e, s));
+        hbytes = e->h_sc.p->hdr_bytes;
+        RAPID_CHECK(o.hdr.reserve((size_t)std::max<int64_t>(hbytes, 1)));
+        k_enc_batch_emit<<<grid_for(nb), TB, 0, s>>>((int32_t)nb, start, hlen, msz, hpos, in.obs, t, wrap, o.snd.p, o.hdr.p);
+        k_enc_alert_emit<<<grid_for(n), TB, 0, s>>>(a, t, head, bpos, epos, start, hlen, hpos, o.hdr.p);
+        k_enc_off64<<<grid_for(nb + 1), TB, 0, s>>>((int32_t)nb, hpos, &e->sc.p->hdr_bytes, o.hoff.p);
+        k_enc_fill<<<grid_for(nb), TB, 0, s>>>((int32_t)nb, -1, o.bid.p);
+        RAPID_KERNEL_CHECK();
+    } else {
+        RAPID_CUDA(cudaMemsetAsync(o.hoff.p, 0, sizeof(int64_t), s));
+    }
+    RAPID_CUDA(cudaMemsetAsync(o.boff.p, 0, sizeof(int64_t), s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    o.n = nb; o.n_bodies = 0; o.hdr_bytes = hbytes; o.body_bytes = 0;
+    e->cur = 1 - e->cur;
+    return RAPID_OK;
+}
+
+
+// The list of every distinct body: fetch(representative's acceptor / receiver index, fingerprint, ids) -> RAPID_OK with the ids.
+using ListFetch = std::function<int32_t(int64_t, uint64_t, uint64_t, int32_t, std::vector<int32_t>&)>;
+
+// The messages of the sending slots of L, in slot order: bodies first (distinct fingerprints on the device, each list fetched
+// once on the host and encoded one thread per entry), then one header per message.
+static int32_t encode_lists(WireEnc* e, const WireEncCtx& ctx, const ListIn& L0, const ListFetch& fetch) {
+    cudaStream_t s = ctx.stream;
+    EncOut& o = e->out[1 - e->cur];
+    ListIn L = L0;
+    const int32_t n = L.n;
+    const EpTab t = ep_tab(ctx.view);
+    RAPID_CUDA(cudaMemsetAsync(e->sc.p, 0, sizeof(EncScal), s));
+    int64_t nm = 0, nb = 0, hbytes = 0, bbytes = 0;
+    if (n > 0) {
+        const size_t N = (size_t)n;
+        uint32_t T = 1024;
+        while ((int64_t)T < 2 * (int64_t)n) T <<= 1;
+        RAPID_CHECK(e->table.reserve(T));
+        RAPID_CHECK(e->a.reserve(N)); RAPID_CHECK(e->b.reserve(N)); RAPID_CHECK(e->c.reserve(N)); RAPID_CHECK(e->d.reserve(N));
+        RAPID_CHECK(e->f.reserve(N)); RAPID_CHECK(e->g.reserve(N));
+        int32_t *slot = e->a.p, *send = e->b.p, *rep = e->c.p, *rpos = e->d.p, *bid_s = e->f.p, *reps = e->g.p;
+        RAPID_CUDA(cudaMemsetAsync(e->table.p, 0xff, (size_t)T * sizeof(int32_t), s));
+        k_enc_list_claim<<<grid_for(n), TB, 0, s>>>(L, T, e->table.p, slot, send);
+        k_enc_list_rep<<<grid_for(n), TB, 0, s>>>(n, slot, e->table.p, rep);
+        RAPID_KERNEL_CHECK();
+        RAPID_CHECK(exclusive_scan_i32(rpos, n, e->scan_sums, &e->sc.p->n_bodies, s, nullptr, rep));
+        k_enc_list_bodies<<<grid_for(n), TB, 0, s>>>(n, slot, e->table.p, rep, rpos, bid_s, reps);
+        RAPID_KERNEL_CHECK();
+        int32_t* mpos = rep;                                                 // rep and rpos are consumed: reuse them
+        int32_t* hsz = rpos;
+        RAPID_CHECK(exclusive_scan_i32(mpos, n, e->scan_sums, &e->sc.p->n_msgs, s, nullptr, send));
+        RAPID_CHECK(enc_read_scal(e, s));
+        nm = e->h_sc.p->n_msgs; nb = e->h_sc.p->n_bodies;
+        if (nb > 0) {
+            const size_t B = (size_t)nb;
+            RAPID_CHECK(e->g1.reserve(B)); RAPID_CHECK(e->g2.reserve(B)); RAPID_CHECK(e->gl.reserve(B)); RAPID_CHECK(e->gacc.reserve(B));
+            k_enc_gather_fp<<<grid_for(nb), TB, 0, s>>>((int32_t)nb, L, reps, e->g1.p, e->g2.p, e->gl.p, e->gacc.p);
+            RAPID_KERNEL_CHECK();
+            std::vector<uint64_t> f1(B), f2(B);
+            std::vector<int32_t> fl(B), facc(B), first(B + 1, 0), ids;
+            RAPID_CUDA(cudaMemcpyAsync(f1.data(), e->g1.p, B * 8, cudaMemcpyDeviceToHost, s));
+            RAPID_CUDA(cudaMemcpyAsync(f2.data(), e->g2.p, B * 8, cudaMemcpyDeviceToHost, s));
+            RAPID_CUDA(cudaMemcpyAsync(fl.data(), e->gl.p, B * 4, cudaMemcpyDeviceToHost, s));
+            RAPID_CUDA(cudaMemcpyAsync(facc.data(), e->gacc.p, B * 4, cudaMemcpyDeviceToHost, s));
+            RAPID_CUDA(cudaStreamSynchronize(s));
+            int64_t tot = 0;
+            for (size_t b = 0; b < B; ++b) tot += fl[b];
+            if (tot > ENC_LIMIT / 2) return too_big();                      // every entry is >= 2 bytes
+            ids.reserve((size_t)tot);
+            std::vector<int32_t> one;
+            for (size_t b = 0; b < B; ++b) {
+                RAPID_CHECK(fetch(facc[b], f1[b], f2[b], fl[b], one));
+                ids.insert(ids.end(), one.begin(), one.end());
+                first[b + 1] = (int32_t)ids.size();
+            }
+            const int32_t nE = first[B];
+            RAPID_CHECK(e->ids.reserve((size_t)std::max(nE, 1))); RAPID_CHECK(e->e.reserve(B + 1));
+            RAPID_CHECK(e->epos.reserve((size_t)std::max(nE, 1)));
+            RAPID_CUDA(cudaMemcpyAsync(e->ids.p, ids.data(), (size_t)nE * 4, cudaMemcpyHostToDevice, s));
+            RAPID_CUDA(cudaMemcpyAsync(e->e.p, first.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
+            k_enc_entry_sizes<<<grid_for(nE), TB, 0, s>>>(nE, e->ids.p, t, e->epos.p, e->sc.p);
+            RAPID_KERNEL_CHECK();
+            RAPID_CHECK(enc_read_scal(e, s));
+            if ((int64_t)e->h_sc.p->bytes64 > ENC_LIMIT) return too_big();
+            RAPID_CHECK(exclusive_scan_i32(e->epos.p, nE, e->scan_sums, &e->sc.p->body_bytes, s, nullptr));
+            bbytes = (int64_t)e->h_sc.p->bytes64;
+            RAPID_CHECK(o.bodies.reserve((size_t)std::max<int64_t>(bbytes, 1))); RAPID_CHECK(o.boff.reserve(B + 1));
+            k_enc_entry_emit<<<grid_for(nE), TB, 0, s>>>(nE, e->ids.p, t, list_tag(L.kind), e->epos.p, o.bodies.p);
+            k_enc_body_off<<<grid_for(nb + 1), TB, 0, s>>>((int32_t)nb, nE, e->e.p, e->epos.p, e->sc.p, o.boff.p);
+            RAPID_KERNEL_CHECK();
+        } else {
+            RAPID_CUDA(cudaMemsetAsync(o.boff.p, 0, sizeof(int64_t), s));
+        }
+        if (nm > 0) {
+            RAPID_CHECK(o.hoff.reserve((size_t)nm + 1)); RAPID_CHECK(o.bid.reserve((size_t)nm)); RAPID_CHECK(o.snd.reserve((size_t)nm));
+            RAPID_CHECK(e->ids2.reserve((size_t)nm));
+            k_enc_list_sizes<<<grid_for(n), TB, 0, s>>>(L, t, send, mpos, bid_s, o.boff.p, hsz);
+            RAPID_KERNEL_CHECK();
+            int32_t* hpos = e->ids2.p;
+            RAPID_CHECK(exclusive_scan_i32(hpos, nm, e->scan_sums, &e->sc.p->hdr_bytes, s, nullptr, hsz));
+            RAPID_CHECK(enc_read_scal(e, s));
+            hbytes = e->h_sc.p->hdr_bytes;
+            RAPID_CHECK(o.hdr.reserve((size_t)std::max<int64_t>(hbytes, 1)));
+            k_enc_list_emit<<<grid_for(n), TB, 0, s>>>(L, t, send, mpos, bid_s, o.boff.p, hpos, o.bid.p, o.snd.p, o.hdr.p);
+            k_enc_off64<<<grid_for(nm + 1), TB, 0, s>>>((int32_t)nm, hpos, &e->sc.p->hdr_bytes, o.hoff.p);
+            RAPID_KERNEL_CHECK();
+        } else {
+            RAPID_CUDA(cudaMemsetAsync(o.hoff.p, 0, sizeof(int64_t), s));
+        }
+    } else {
+        RAPID_CUDA(cudaMemsetAsync(o.hoff.p, 0, sizeof(int64_t), s));
+        RAPID_CUDA(cudaMemsetAsync(o.boff.p, 0, sizeof(int64_t), s));
+    }
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    o.n = nm; o.n_bodies = nb; o.hdr_bytes = hbytes; o.body_bytes = bbytes;
+    e->cur = 1 - e->cur;
+    return RAPID_OK;
+}
+
+// the list cache follows the view's members: ids are renumbered by a cut
+static void lists_sync(WireEnc* e, const View* v) {
+    if (e->lists_epoch != v->member_epoch) { e->lists.clear(); e->lists_epoch = v->member_epoch; }
+}
+
+// a detector receiver's announced proposal in canonical order, checked against the fingerprint it must have
+static int32_t cd_list(const rapid_cd* cd, int64_t receiver, uint64_t h1, uint64_t h2, int32_t len, std::vector<int32_t>& ids) {
+    ids.assign((size_t)std::max(len, 1), 0);
+    int32_t got = 0;
+    RAPID_CHECK(rapid_cd_get_proposal(cd, receiver, ids.data(), len, &got));
+    uint64_t a = 0, b = 0;
+    if (got == len) RAPID_CHECK(rapid_proposal_fingerprint(ids.data(), got, &a, &b));
+    if (got != len || a != h1 || b != h2) return -1;
+    ids.resize((size_t)len);
+    return RAPID_OK;
+}
+
+static int32_t check_cd(const WireEncCtx& ctx, const rapid_cd* cd) {
+    if (cd->view != ctx.view || cd->device != ctx.device) { set_error("the detector was created on another view or device"); return RAPID_EINVAL; }
+    if (cd->raw) { set_error("RAW detectors do not announce proposals"); return RAPID_EINVAL; }
+    if (cd->member_epoch != ctx.view->member_epoch) { set_error("the view's members changed since the detector was created"); return RAPID_EINVAL; }
+    return RAPID_OK;
+}
+
+// Phase1b (want = 1) / Phase2b (want = 2) answers of the acceptors; each distinct list from the cache, else from the detector
+// receiver with the representative's index
+static int32_t encode_answers(rapid_wire* w, const rapid_pxa* pxa, const rapid_cd* cd, uint32_t flags, int want, int64_t* n_messages,
+                              int64_t* n_bodies) {
+    if (!w || !pxa || (flags & ~RAPID_WIRE_REQUEST)) { set_error("bad arguments"); return RAPID_EINVAL; }
+    WireEncCtx ctx;
+    wire_enc_ctx(w, &ctx);
+    PxaAnswers in;
+    pxa_answers_dev(pxa, &in);
+    if (in.device != ctx.device) { set_error("the acceptors live on another device"); return RAPID_EINVAL; }
+    if (in.kind != want) {
+        set_error(want == 1 ? "no Phase1b answers pending (call rapid_pxa_phase1a first)" : "no Phase2b answers pending (call rapid_pxa_phase2a first)");
+        return RAPID_EINVAL;
+    }
+    if (in.begin + in.R > ctx.view->n) { set_error("the acceptors' ring-0 positions exceed the view"); return RAPID_EINVAL; }
+    if (cd) RAPID_CHECK(check_cd(ctx, cd));
+    DeviceGuard g(ctx.device);
+    if (cd) RAPID_CHECK(cd_wait(cd, false));
+    WireEnc* e = nullptr;
+    RAPID_CHECK(enc_get(w, &ctx, &e));
+    lists_sync(e, ctx.view);
+    ListIn L{};
+    L.n = (int32_t)in.n; L.kind = want == 1 ? RAPID_WIRE_PHASE1B : RAPID_WIRE_PHASE2B; L.wrap = (flags & RAPID_WIRE_REQUEST) ? 1 : 0;
+    L.cfg = in.cfg; L.acc = in.sender; L.ring0 = ctx.view->ring.p; L.rank = in.rank;
+    if (want == 1) { L.h1 = in.h1; L.h2 = in.h2; L.len = in.len; L.vrnd = in.vrnd; }
+    else { L.c1 = in.v_h1; L.c2 = in.v_h2; L.clen = in.v_len; }
+    const ListFetch fetch = [&](int64_t acc, uint64_t h1, uint64_t h2, int32_t len, std::vector<int32_t>& ids) -> int32_t {
+        const auto key = std::make_tuple(h1, h2, len);
+        auto it = e->lists.find(key);
+        if (it != e->lists.end()) { ids = it->second; return RAPID_OK; }
+        const int64_t r = cd ? acc - cd->rbegin : -1;
+        if (cd && r >= 0 && r < cd->R && cd_list(cd, r, h1, h2, len, ids) == RAPID_OK) { e->lists[key] = ids; return RAPID_OK; }
+        set_error("the %d-endpoint list held by acceptor %lld is not known: encode the votes that carried it first, or pass the "
+                  "detector whose receiver announced it", len, (long long)acc);
+        return RAPID_EINVAL;
+    };
+    RAPID_CHECK(encode_lists(e, ctx, L, fetch));
+    const EncOut& o = e->out[e->cur];
+    if (n_messages) *n_messages = o.n;
+    if (n_bodies) *n_bodies = o.n_bodies;
+    return RAPID_OK;
+}
+
+}  // namespace rapid
+
+using namespace rapid;
+
+extern "C" {
+
+int32_t rapid_wire_encode_alert_batches(rapid_wire* w, const rapid_fdet* fd, uint32_t flags, int64_t* n_messages, int64_t* n_bytes) {
+    if (!w || !fd || (flags & ~RAPID_WIRE_REQUEST)) { set_error("bad arguments"); return RAPID_EINVAL; }
+    WireEncCtx ctx;
+    wire_enc_ctx(w, &ctx);
+    FdetInterval in;
+    fdet_interval_dev(fd, &in);
+    if (in.view != ctx.view || in.device != ctx.device) { set_error("the failure detectors were created on another view or device"); return RAPID_EINVAL; }
+    if (!in.have) { set_error("no failure-detector interval since the last reset (call rapid_fdet_tick first)"); return RAPID_EINVAL; }
+    DeviceGuard g(ctx.device);
+    WireEnc* e = nullptr;
+    RAPID_CHECK(enc_get(w, &ctx, &e));
+    RAPID_CHECK(encode_alerts(e, ctx, in, flags));
+    const EncOut& o = e->out[e->cur];
+    if (n_messages) *n_messages = o.n;
+    if (n_bytes) *n_bytes = o.hdr_bytes + o.body_bytes;
+    return RAPID_OK;
+}
+
+int32_t rapid_wire_encode_votes(rapid_wire* w, const rapid_cd* cd, int64_t cfg_id, uint32_t flags, int64_t* n_messages, int64_t* n_bodies) {
+    if (!w || !cd || (flags & ~RAPID_WIRE_REQUEST)) { set_error("bad arguments"); return RAPID_EINVAL; }
+    WireEncCtx ctx;
+    wire_enc_ctx(w, &ctx);
+    RAPID_CHECK(check_cd(ctx, cd));
+    if (cd->batch_serial == 0) { set_error("the detector has applied no batch: it has no outputs to encode"); return RAPID_EINVAL; }
+    DeviceGuard g(ctx.device);
+    RAPID_CHECK(cd_wait(cd, false));                                         // asynchronous batches still in flight on its stream
+    WireEnc* e = nullptr;
+    RAPID_CHECK(enc_get(w, &ctx, &e));
+    lists_sync(e, ctx.view);
+    ListIn L{};
+    L.n = (int32_t)cd->R; L.kind = RAPID_WIRE_FAST_ROUND_PHASE2B; L.wrap = (flags & RAPID_WIRE_REQUEST) ? 1 : 0; L.cfg = cfg_id;
+    L.rflags = cd->rflags.p; L.rbegin = cd->rbegin; L.ring0 = ctx.view->ring.p;
+    L.h1 = cd->out_h1.p; L.h2 = cd->out_h2.p; L.len = cd->out_len.p;
+    const ListFetch fetch = [&](int64_t pos, uint64_t h1, uint64_t h2, int32_t len, std::vector<int32_t>& ids) -> int32_t {
+        if (cd_list(cd, pos - cd->rbegin, h1, h2, len, ids) != RAPID_OK) {
+            set_error("receiver %lld's proposal does not match its fingerprint", (long long)(pos - cd->rbegin)); return RAPID_EINVAL;
+        }
+        e->lists[std::make_tuple(h1, h2, len)] = ids;
+        return RAPID_OK;
+    };
+    RAPID_CHECK(encode_lists(e, ctx, L, fetch));
+    const EncOut& o = e->out[e->cur];
+    if (n_messages) *n_messages = o.n;
+    if (n_bodies) *n_bodies = o.n_bodies;
+    return RAPID_OK;
+}
+
+int32_t rapid_wire_encode_phase1b(rapid_wire* w, const rapid_pxa* pxa, const rapid_cd* cd, uint32_t flags, int64_t* n_messages,
+                                  int64_t* n_bodies) {
+    return encode_answers(w, pxa, cd, flags, 1, n_messages, n_bodies);
+}
+
+int32_t rapid_wire_encode_phase2b(rapid_wire* w, const rapid_pxa* pxa, const rapid_cd* cd, uint32_t flags, int64_t* n_messages,
+                                  int64_t* n_bodies) {
+    return encode_answers(w, pxa, cd, flags, 2, n_messages, n_bodies);
+}
+
+int32_t rapid_wire_encoded_counts(const rapid_wire* cw, int64_t* n_messages, int64_t* header_bytes, int64_t* n_bodies, int64_t* body_bytes) {
+    if (!cw) { set_error("NULL handle"); return RAPID_EINVAL; }
+    WireEncCtx ctx;
+    wire_enc_ctx(const_cast<rapid_wire*>(cw), &ctx);
+    const EncOut* o = *ctx.enc ? &(*ctx.enc)->out[(*ctx.enc)->cur] : nullptr;
+    if (n_messages) *n_messages = o ? o->n : 0;
+    if (header_bytes) *header_bytes = o ? o->hdr_bytes : 0;
+    if (n_bodies) *n_bodies = o ? o->n_bodies : 0;
+    if (body_bytes) *body_bytes = o ? o->body_bytes : 0;
+    return RAPID_OK;
+}
+
+int32_t rapid_wire_encoded_dev(const rapid_wire* cw, const uint8_t** headers, const int64_t** header_off, const int32_t** body_id,
+                               const uint8_t** bodies, const int64_t** body_off) {
+    if (!cw) { set_error("NULL handle"); return RAPID_EINVAL; }
+    WireEncCtx ctx;
+    wire_enc_ctx(const_cast<rapid_wire*>(cw), &ctx);
+    if (!*ctx.enc) { set_error("nothing was encoded on this handle"); return RAPID_EINVAL; }
+    const EncOut& o = (*ctx.enc)->out[(*ctx.enc)->cur];
+    if (headers) *headers = o.hdr.p;
+    if (header_off) *header_off = o.hoff.p;
+    if (body_id) *body_id = o.bid.p;
+    if (bodies) *bodies = o.bodies.p;
+    if (body_off) *body_off = o.boff.p;
+    return RAPID_OK;
+}
+
+int32_t rapid_wire_read_encoded(const rapid_wire* cw, uint8_t* headers, int64_t* header_off, int32_t* body_id, uint8_t* bodies,
+                                int64_t* body_off) {
+    if (!cw) { set_error("NULL handle"); return RAPID_EINVAL; }
+    WireEncCtx ctx;
+    wire_enc_ctx(const_cast<rapid_wire*>(cw), &ctx);
+    if (!*ctx.enc) { set_error("nothing was encoded on this handle"); return RAPID_EINVAL; }
+    const EncOut& o = (*ctx.enc)->out[(*ctx.enc)->cur];
+    DeviceGuard g(ctx.device);
+    cudaStream_t s = ctx.stream;
+    if (headers && o.hdr_bytes) RAPID_CUDA(cudaMemcpyAsync(headers, o.hdr.p, (size_t)o.hdr_bytes, cudaMemcpyDeviceToHost, s));
+    if (header_off) RAPID_CUDA(cudaMemcpyAsync(header_off, o.hoff.p, ((size_t)o.n + 1) * 8, cudaMemcpyDeviceToHost, s));
+    if (body_id && o.n) RAPID_CUDA(cudaMemcpyAsync(body_id, o.bid.p, (size_t)o.n * 4, cudaMemcpyDeviceToHost, s));
+    if (bodies && o.body_bytes) RAPID_CUDA(cudaMemcpyAsync(bodies, o.bodies.p, (size_t)o.body_bytes, cudaMemcpyDeviceToHost, s));
+    if (body_off) RAPID_CUDA(cudaMemcpyAsync(body_off, o.boff.p, ((size_t)o.n_bodies + 1) * 8, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    return RAPID_OK;
+}
+
+int32_t rapid_wire_read_encoded_sizes(const rapid_wire* cw, int64_t* sizes) {
+    if (!cw) { set_error("NULL handle"); return RAPID_EINVAL; }
+    WireEncCtx ctx;
+    wire_enc_ctx(const_cast<rapid_wire*>(cw), &ctx);
+    if (!*ctx.enc) { set_error("nothing was encoded on this handle"); return RAPID_EINVAL; }
+    WireEnc* e = *ctx.enc;
+    const EncOut& o = e->out[e->cur];
+    if (o.n == 0) return RAPID_OK;
+    if (!sizes) { set_error("NULL sizes"); return RAPID_EINVAL; }
+    DeviceGuard g(ctx.device);
+    cudaStream_t s = ctx.stream;
+    RAPID_CHECK(e->sizes.reserve((size_t)o.n));
+    k_enc_sizes<<<grid_for(o.n), TB, 0, s>>>(o.n, o.hoff.p, o.bid.p, o.boff.p, e->sizes.p);
+    RAPID_KERNEL_CHECK();
+    RAPID_CUDA(cudaMemcpyAsync(sizes, e->sizes.p, (size_t)o.n * 8, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    return RAPID_OK;
+}
+
+int32_t rapid_wire_read_encoded_senders(const rapid_wire* cw, int32_t* sender) {
+    if (!cw) { set_error("NULL handle"); return RAPID_EINVAL; }
+    WireEncCtx ctx;
+    wire_enc_ctx(const_cast<rapid_wire*>(cw), &ctx);
+    if (!*ctx.enc) { set_error("nothing was encoded on this handle"); return RAPID_EINVAL; }
+    const EncOut& o = (*ctx.enc)->out[(*ctx.enc)->cur];
+    if (o.n == 0) return RAPID_OK;
+    if (!sender) { set_error("NULL sender"); return RAPID_EINVAL; }
+    DeviceGuard g(ctx.device);
+    RAPID_CUDA(cudaMemcpyAsync(sender, o.snd.p, (size_t)o.n * 4, cudaMemcpyDeviceToHost, ctx.stream));
+    RAPID_CUDA(cudaStreamSynchronize(ctx.stream));
+    return RAPID_OK;
+}
+
+}  // extern "C"

@@ -48,6 +48,12 @@ ClusterSimulation rules (tests/simref.py restates them independently; DESIGN.md 
   meet the batches in different orders can announce different proposals; the records count them: intervals[i]["proposals"]
   is the number of distinct proposals announced in the interval, history[c]["distinct_proposals"] the number over the
   configuration.  Every node sees every vote, so one tally stands for every node's.
+* Wire traffic (wire_traffic=True; off by default, and then no record changes): every interval record gains wire_bytes, the
+  bytes of the interval's alert batches, fast-round votes and (when a classic round ran) Phase1b / Phase2b answers, each wrapped
+  as a RapidRequest, encoded on the device and counted once per member (a broadcast is one unicast per member,
+  UnicastToAllBroadcaster.java:46-52); wire_tx_max / wire_tx_mean over the members' transmitted bytes and wire_rx_max /
+  wire_rx_mean (every member receives every broadcast, so they are equal).  Probes, join messages and LeaveMessage are not
+  encoded: these are not the traffic figures of the Rapid paper.
 * Overlay quality (overlay_quality=True; off by default, and then no record changes): every configuration record gains
   overlay_ratio and overlay_residual, MembershipView.overlaySpectrum() (default seed, tolerance and step limit) of the view
   AFTER that view change: lambda / 2K of its monitoring overlay and the bound on the error of lambda (DESIGN.md §4.13);
@@ -58,11 +64,13 @@ import time
 
 import numpy as np
 
+from . import _native as N
 from .classic_paxos import Paxos, PaxosAcceptors
 from .cut_detector import VirtualCluster
 from .failure_detector import CRASHED, EdgeFailureDetectors, FAILURE_THRESHOLD
 from .fast_paxos import FastPaxos
 from .membership_view import MembershipView
+from .wire import WireDecoder
 from .workloads import splitmix64
 
 _M64 = 0xFFFFFFFFFFFFFFFF
@@ -98,7 +106,7 @@ class ClusterSimulation:
     configuration, intervals one per interval."""
 
     def __init__(self, endpoints, node_ids, K=10, H=9, L=4, seed=0, failure_threshold=FAILURE_THRESHOLD, fallback_intervals=1,
-                 device=0, batch_order="sender", overlay_quality=False):
+                 device=0, batch_order="sender", overlay_quality=False, wire_traffic=False):
         if batch_order not in ("sender", "shuffled"):
             raise ValueError("batch_order is 'sender' or 'shuffled', not %r" % (batch_order,))
         self.batch_order = batch_order
@@ -127,6 +135,8 @@ class ClusterSimulation:
         self._new_handles()
         self.overlay_quality = bool(overlay_quality)
         self.initial_overlay = self._overlay() if self.overlay_quality else None
+        self.wire = WireDecoder(self.view) if wire_traffic else None     # sizes of the interval's messages, encoded on the device
+        self._wire_tx = None
 
     # ---- scenario ------------------------------------------------------------------------------------------------------------
     def setFlags(self, node, flags):
@@ -277,6 +287,11 @@ class ClusterSimulation:
         rec = {"cfg": cfg, "interval": i, "alerts": na, "cells": nc, "announced": 0, "event": "quiet", "leavers": len(leavers),
                "proposals": 0}
         decided = None
+        n_members = self.N
+        if self.wire is not None:
+            self._wire_tx = np.zeros(n_members, np.float64)
+            if na:
+                self._wire_count(lambda: N.check(N.lib().rapid_wire_encode_alert_batches(self.wire._h, self.fd._h, N.WIRE_REQUEST, None, None)))
         if nc:
             rec["event"] = "alerts"
             p = self.fd.cellsDevice()
@@ -285,6 +300,9 @@ class ClusterSimulation:
                                         blocked_dev=self.d_blocked.data_ptr(), **order)
             dev_ms += self.cl.lastDeviceMs()[0]
             self.acc.registerFastRoundVotesFrom(self.cl)
+            if self.wire is not None:
+                self._wire_count(lambda: N.check(N.lib().rapid_wire_encode_votes(self.wire._h, self.cl._h, cfg, N.WIRE_REQUEST, None,
+                                                                                 None)))
             t = self.fp.tallyCluster(self.cl)
             dev_ms += self.fp.lastDeviceMs()
             # votes are counted up to the decision (FastPaxos.java:138): in a deciding interval the announcers are counted instead,
@@ -313,6 +331,13 @@ class ClusterSimulation:
                 rec["event"] = "stalled"
             else:
                 decided = ("classic", value)
+        if self.wire is not None:
+            # a broadcast is one unicast per member (UnicastToAllBroadcaster.java:46-52): every member receives every message
+            tx = self._wire_tx
+            rec["wire_bytes"] = int(tx.sum())
+            rec["wire_tx_max"], rec["wire_tx_mean"] = int(tx.max()), float(tx.mean())
+            rx = rec["wire_bytes"] // n_members
+            rec["wire_rx_max"], rec["wire_rx_mean"] = rx, float(rx)
         self._cfg_t["device_ms"] += dev_ms
         rec["device_ms"] = dev_ms
         rec["host_ms"] = (time.perf_counter() - t0) * 1e3               # host clock of the whole interval, view change excluded
@@ -346,15 +371,29 @@ class ClusterSimulation:
         px.startPhase1a(2, coord)
         self.acc.setSilent(self.crashed_r)
         self.acc.handlePhase1aMessage((2, coord))
+        if self.wire is not None:
+            self._wire_count(lambda: N.check(N.lib().rapid_wire_encode_phase1b(self.wire._h, self.acc._h, self.cl._h, N.WIRE_REQUEST,
+                                                                               None, None)))
         r1 = px.handlePhase1bFromAcceptors(self.acc, perm_seed=s1)
         ms = px.lastDeviceMs()
         if not r1.proposed:
             return None, ms
         self._proposer = self.acc.findValue(r1.cval)                # before Phase2a overwrites the vvals
         self.acc.handlePhase2aMessage((2, coord), r1.cval)
+        if self.wire is not None:
+            self._wire_count(lambda: N.check(N.lib().rapid_wire_encode_phase2b(self.wire._h, self.acc._h, self.cl._h, N.WIRE_REQUEST,
+                                                                               None, None)))
         r2 = px.handlePhase2bFromAcceptors(self.acc, perm_seed=s2)
         ms += px.lastDeviceMs()
         return (r2.decision if r2.decided else None), ms
+
+    def _wire_count(self, encode):
+        """encode one kind of the interval's messages on the device (wrapped as RapidRequests) and add size x members to each
+        sender's transmitted bytes; only the sizes and senders leave the device"""
+        encode()
+        sizes, senders = self.wire.encodedSizes(), self.wire.encodedSenders()
+        if len(sizes):
+            self._wire_tx += np.bincount(senders, weights=sizes.astype(np.float64) * self.N, minlength=self.N)[: self.N]
 
     def _announced_flags(self):
         if self._ann is None:

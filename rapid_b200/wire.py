@@ -19,6 +19,36 @@ class DecodedAlerts:
             self.n_messages, self.n_cells, self.n_dropped, self.n_new_joiners, self.sender)
 
 
+class EncodedMessages:
+    """The outputs of one encode, copied to the host: message i = headers[header_off[i]:header_off[i+1]] ++ body body_ids[i]
+    (none when -1).  Messages that carry the same list share one body."""
+
+    def __init__(self, headers, header_off, body_ids, bodies, body_off, sizes, senders):
+        self.headers, self.header_off, self.body_ids, self.bodies, self.body_off = headers, header_off, body_ids, bodies, body_off
+        self._sizes = sizes
+        self.senders = senders                 # view id of each message's sender
+
+    def __len__(self):
+        return len(self.body_ids)
+
+    def header(self, i):
+        return self.headers[self.header_off[i]:self.header_off[i + 1]].tobytes()
+
+    def body(self, b):
+        return self.bodies[self.body_off[b]:self.body_off[b + 1]].tobytes()
+
+    def message(self, i):
+        b = int(self.body_ids[i])
+        return self.header(i) + (self.body(b) if b >= 0 else b"")
+
+    def sizes(self):
+        """bytes of every message, header + body, as the device computed them"""
+        return self._sizes
+
+    def __repr__(self):
+        return "EncodedMessages(messages=%d, bodies=%d, bytes=%d)" % (len(self), len(self.body_off) - 1, int(self._sizes.sum()))
+
+
 class WireDecoder:
     """Owns the Endpoint{hostname, port} -> id table of a MembershipView on the device."""
 
@@ -134,3 +164,55 @@ class WireDecoder:
         out = C.c_float(0)
         N.check(N.lib().rapid_wire_last_device_ms(self._h, C.byref(out)))
         return out.value
+
+    # ---- egress: the messages the virtual nodes send, encoded on the device (csrc/wire_encode.cu) ----
+    def encodeAlertBatches(self, detectors, as_request=False):
+        """one BatchedAlertMessage per sender of the last interval of an EdgeFailureDetectors -> EncodedMessages"""
+        N.check(N.lib().rapid_wire_encode_alert_batches(self._h, detectors._h, N.WIRE_REQUEST if as_request else 0, None, None))
+        return self.encoded()
+
+    def encodeVotes(self, detector, cfg_id, as_request=False):
+        """one FastRoundPhase2bMessage per receiver of a MembershipServiceCutDetector that announced in its last call"""
+        N.check(N.lib().rapid_wire_encode_votes(self._h, detector._h, int(cfg_id), N.WIRE_REQUEST if as_request else 0, None, None))
+        return self.encoded()
+
+    def encodePhase1b(self, acceptors, detector=None, as_request=False):
+        """one Phase1bMessage per answer of a PaxosAcceptors' last handlePhase1aMessage; vval lists from the votes this handle
+        encoded, else from the detector whose receivers are the acceptors"""
+        N.check(N.lib().rapid_wire_encode_phase1b(self._h, acceptors._h, detector._h if detector is not None else None,
+                                                  N.WIRE_REQUEST if as_request else 0, None, None))
+        return self.encoded()
+
+    def encodePhase2b(self, acceptors, detector=None, as_request=False):
+        """one Phase2bMessage per answer of a PaxosAcceptors' last handlePhase2aMessage"""
+        N.check(N.lib().rapid_wire_encode_phase2b(self._h, acceptors._h, detector._h if detector is not None else None,
+                                                  N.WIRE_REQUEST if as_request else 0, None, None))
+        return self.encoded()
+
+    def encodedSenders(self):
+        """view id of the sender of every message of the last encode"""
+        n = self.encodedCounts()[0]
+        out = np.zeros(n, np.int32)
+        N.check(N.lib().rapid_wire_read_encoded_senders(self._h, N.ptr(out) if n else None))
+        return out
+
+    def encodedCounts(self):
+        """(messages, header bytes, bodies, body bytes) of the last encode"""
+        v = [C.c_int64(0) for _ in range(4)]
+        N.check(N.lib().rapid_wire_encoded_counts(self._h, *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
+
+    def encodedSizes(self):
+        """bytes of every message of the last encode, header + body, computed on the device"""
+        n = self.encodedCounts()[0]
+        out = np.zeros(n, np.int64)
+        N.check(N.lib().rapid_wire_read_encoded_sizes(self._h, N.ptr(out) if n else None))
+        return out
+
+    def encoded(self):
+        """host copies of the last encode -> EncodedMessages"""
+        n, hb, nb, bb = self.encodedCounts()
+        hdr, hoff, bid = np.zeros(max(hb, 1), np.uint8), np.zeros(n + 1, np.int64), np.zeros(max(n, 1), np.int32)
+        bodies, boff = np.zeros(max(bb, 1), np.uint8), np.zeros(nb + 1, np.int64)
+        N.check(N.lib().rapid_wire_read_encoded(self._h, N.ptr(hdr), N.ptr(hoff), N.ptr(bid), N.ptr(bodies), N.ptr(boff)))
+        return EncodedMessages(hdr[:hb], hoff, bid[:n], bodies[:bb], boff, self.encodedSizes(), self.encodedSenders())
