@@ -186,7 +186,7 @@ def lib():
     global _LIB
     if _LIB is not None:
         return _LIB
-    path = os.environ.get("RAPID_B200_LIB") or _build.LIB      # (A/B builds of the library: profiles/ab_build.sh)
+    path = _build.LIB
     if not os.path.exists(path):
         _build.build_native()
     L = C.CDLL(path)

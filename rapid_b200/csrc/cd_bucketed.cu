@@ -47,32 +47,14 @@ namespace cg = cooperative_groups;
 
 namespace rapid {
 
-// tuning switches (A/B builds: profiles/ab_build.sh)
+// Tuning choices (why each was made: DESIGN.md §4.2 and §4.3):
 // k_apply_uniform: resident blocks/SM its register budget is sized for.  5 = 96 registers; at 8 (64) every instantiation spills
 // on sm_90a and the kernel is slower (A/B in DESIGN.md §4.2).
-#ifndef RAPID_UNI_MINBLOCKS
-#define RAPID_UNI_MINBLOCKS 5
-#endif
-#ifndef RAPID_SPLIT_LOOP
-#define RAPID_SPLIT_LOOP 0
-#endif
-#ifndef RAPID_PF
-#define RAPID_PF 2                    // carried subjects: L2 prefetch distance (in staged subjects) of the row loads, 0 = off
-#endif
-#ifndef RAPID_INVAL_SPLIT
-#define RAPID_INVAL_SPLIT 1           // k_inval_finalize2 splits the work list of a tile over several blocks (small clusters); 0 = one block per tile
-#endif
-#ifndef RAPID_PF_L1
-#define RAPID_PF_L1 0                 // 1: prefetch into L1 instead of L2
-#endif
-#if RAPID_PF_L1
-#define RAPID_PF_ASM "prefetch.global.L1 [%0];"
-#else
-#define RAPID_PF_ASM "prefetch.global.L2 [%0];"
-#endif
-#ifndef RAPID_MEMO
-#define RAPID_MEMO 1                  // carried subjects: the visit of the tile's sample state is computed once per block (see k_apply_uniform)
-#endif
+constexpr int UNI_MINBLOCKS = 5;
+// k_apply_uniform, carried subjects: the rows of the next PF_DIST staged subjects are prefetched into L2 (DESIGN.md §4.2).
+constexpr int PF_DIST = 2;
+// k_apply_uniform, carried subjects: the visit of the tile's sample state is computed once per block (memo, DESIGN.md §4.2).
+// k_inval_finalize2: below 64 tiles a tile's work list is split over several blocks (DESIGN.md §4.3).
 
 constexpr int TILE_R = 1024;          // receivers per tile (uniform kernel: 128 threads x 8 receivers)
 constexpr int UNI_THREADS = 128;
@@ -151,10 +133,8 @@ struct Bucketed {
     DevBuf<int32_t> mx_changed;               // [4] rotating "the component grew" counters of the fixpoint loop
     DevBuf<uint32_t> mx_dev;                  // [Rpad / 32]
     DevBuf<int32_t> batch_index;              // [slot] -> index of the subject in the batch in flight
-#if RAPID_INVAL_SPLIT
     DevBuf<int32_t> inv_res, inv_ticket;      // [Rpad] / [n_tiles] hand-over of k_inval_finalize2's blocks (all zero between launches)
     DevBuf<unsigned long long> inv_h1, inv_h2;
-#endif
     // invalidation work list (WorkList)
     DevBuf<int32_t> wl_slots, wl_count, wl_listed, wl_so_tab;
     DevBuf<uint8_t> wl_in_tile;               // [slot][n_tiles]
@@ -500,7 +480,7 @@ __device__ __forceinline__ uint32_t seq_state(const ApplyArgs& a, const SubjDesc
 }
 
 template <bool PERM, bool SEQ, int HB>
-__global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_uniform(const ApplyArgs a) {
+__global__ void __launch_bounds__(UNI_THREADS, UNI_MINBLOCKS) k_apply_uniform(const ApplyArgs a) {
     __shared__ SubjDesc sd[STAGE];
     __shared__ SubjWalk sw[PERM ? 1 : STAGE];
     __shared__ SubjWalk spw[SEQ ? STAGE : 1];
@@ -516,7 +496,7 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
     __shared__ uint8_t s_ek[SEQ ? STAGE : 1][MAXK];
     __shared__ const uint8_t* s_erow[SEQ ? STAGE : 1][MAXK];
     __shared__ int32_t s_eob[SEQ ? STAGE : 1][MAXK];
-    // Memo of the carried subjects (RAPID_MEMO): receivers of a tile have almost always seen the same history, so warp 0 computes
+    // Memo of the carried subjects: receivers of a tile have almost always seen the same history, so warp 0 computes
     // the visit ONCE per (block, subject) for the state the tile's first active receiver holds; a thread whose active receivers
     // all hold exactly that state only merges the precomputed new word, and takes the stage's summed contribution at the end of the
     // stage.  (The visit itself — the walk over the first-occurrence rings — was what kept the read-modify-write path issue-bound.)
@@ -528,7 +508,7 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
     __shared__ uint32_t s_mall;               // which staged subjects have a memo
     __shared__ int s_wfirst[UNI_THREADS / 32];
 
-    constexpr bool MEMO = RAPID_MEMO && !SEQ; // (the sequence kernels keep the plain path: their visit depends on the observers' rows too)
+    constexpr bool MEMO = !SEQ;               // (the sequence kernels keep the plain path: their visit depends on the observers' rows too)
     if (a.bc->overflow) return;               // the batch was rolled back by k_prepare
     // the number of batch subjects / the first fresh slot are only known on the device
     const int Sb = a.bc->n_batch_subj, S_before = a.bc->S_before;
@@ -648,52 +628,34 @@ __global__ void __launch_bounds__(UNI_THREADS, RAPID_UNI_MINBLOCKS) k_apply_unif
         }
         __syncthreads();
         uint32_t hit = 0;                                  // staged subjects for which this thread took the memo
-#if RAPID_PF > 0
         // The read-modify-write path has ONE group load (both planes) in flight per thread (the loop body branches on the loaded
-        // words), far below what the HBM latency-bandwidth product needs.  The rows of the next RAPID_PF staged subjects are
+        // words), far below what the HBM latency-bandwidth product needs.  The rows of the next PF_DIST staged subjects are
         // therefore pulled into L2 ahead of their loads.
         const bool pf_on = !SEQ && s_heavy != 0;          // (the sequence kernels keep their measured code: no memo, no prefetch)
         if (pf_on) {
 #pragma unroll
-            for (int j = 0; j < RAPID_PF; ++j)
+            for (int j = 0; j < PF_DIST; ++j)
                 if (j < n && s_src[j]) {
-                    asm volatile(RAPID_PF_ASM ::"l"(s_src[j] + r0));
-                    asm volatile(RAPID_PF_ASM ::"l"(group8_hi<HB>(rows, s_src[j], r0)));
+                    asm volatile("prefetch.global.L2 [%0];" ::"l"(s_src[j] + r0));
+                    asm volatile("prefetch.global.L2 [%0];" ::"l"(group8_hi<HB>(rows, s_src[j], r0)));
                 }
         }
-#endif
-#if RAPID_SPLIT_LOOP
-        // fresh subjects of the stage first: write-only, in a loop of their own
-#pragma unroll 4
-        for (int i = 0; i < n; ++i) {
-            if (s_src[i] == nullptr && (!SEQ || s_ne[i] == 0)) group8_store<HB>(rows, s_dst[i], r0, group8_fill<HB>(s_nrep[i], am));
-        }
-        const int n_heavy = s_heavy ? n : 0;               // (uniform) nothing but plain fresh subjects in this stage: skip the visit loop
-        for (int i = 0; i < n_heavy; ++i) {
-            const uint8_t* src = s_src[i];
-            uint8_t* dst = s_dst[i];
-            const int ne = SEQ ? (int)s_ne[i] : 0;
-            if (src == nullptr && ne == 0) continue;       // (done above)
-#else
 #pragma unroll 4
         for (int i = 0; i < n; ++i) {
             const uint8_t* src = s_src[i];
             uint8_t* dst = s_dst[i];
             const int ne = SEQ ? (int)s_ne[i] : 0;
-#if RAPID_PF > 0
-            if (pf_on && i + RAPID_PF < n) {
-                const uint8_t* nx = s_src[i + RAPID_PF];
+            if (pf_on && i + PF_DIST < n) {
+                const uint8_t* nx = s_src[i + PF_DIST];
                 if (nx) {
-                    asm volatile(RAPID_PF_ASM ::"l"(nx + r0));
-                    asm volatile(RAPID_PF_ASM ::"l"(group8_hi<HB>(rows, nx, r0)));
+                    asm volatile("prefetch.global.L2 [%0];" ::"l"(nx + r0));
+                    asm volatile("prefetch.global.L2 [%0];" ::"l"(group8_hi<HB>(rows, nx, r0)));
                 }
             }
-#endif
             if (src == nullptr && ne == 0) {               // fresh subject: write-only, full width (zeros for inactive receivers)
                 group8_store<HB>(rows, dst, r0, group8_fill<HB>(s_nrep[i], am));
                 continue;
             }
-#endif
             Group8<HB> w;
             if (src) w = group8_load<HB>(rows, src, r0);
             else { w.lo = 0; w.hi = 0; }
@@ -1011,13 +973,11 @@ struct ResolveArgs {
     const int32_t* touch;
     const int32_t* batch_index;
     int32_t serial;
-#if RAPID_INVAL_SPLIT
     int inv_split;                // blocks per 1024-receiver tile in k_inval_finalize2 (1: a block walks the whole work list)
     int32_t* inv_res;             // [Rpad] subjects raised to >= H by the pass, summed over the blocks of a tile
     unsigned long long* inv_h1;   // [Rpad] their fingerprint sums
     unsigned long long* inv_h2;
     int32_t* inv_ticket;          // [n_tiles] blocks of the tile that have handed their part over
-#endif
 };
 
 __device__ __forceinline__ int32_t block_sum_i32(int32_t v, int32_t* s_red) {      // every thread gets the block total
@@ -1375,16 +1335,12 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
     const int t = threadIdx.x;
     const int n_list = min(*(volatile int32_t*)a.wl.count, a.wl.cap);
     int32_t my_inval = 0;
-#if RAPID_INVAL_SPLIT
     // Small clusters have few tiles and one block per tile would walk the whole list alone (C3: 10 blocks x ~125 dependent
     // iterations).  The pass is independent per subject — an observer's membership in proposal U preProposal does not
     // change while it runs (implicit reports only move subjects from the band to >= H) — so P blocks share a tile: each takes a
     // contiguous part of the list, adds what it raised to per-receiver accumulators, and the last one to finish closes the receivers.
     const int P = MX ? 1 : max(1, e.inv_split);
     __shared__ int s_fin;
-#else
-    constexpr int P = 1;
-#endif
     for (int tb = blockIdx.x; tb < a.n_tiles * P; tb += gridDim.x) {
         const int tile = P > 1 ? tb % a.n_tiles : tb;
         int lo = 0, hi = n_list;
@@ -1507,7 +1463,6 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
                 }
             }
         }
-#if RAPID_INVAL_SPLIT
         if (P > 1) {
 #pragma unroll
             for (int j = 0; j < 4; ++j)
@@ -1526,7 +1481,6 @@ __device__ void phase_inval_finalize2(const ResolveArgs& e, int mixed, InvSmem& 
             }
             if (t == 0) e.inv_ticket[tile] = 0;
         }
-#endif
         // ---- finalize2: emissions of the invalidation pass, announced flags --------------------------------------------------
         uint32_t ann = 0;
         bool touched = false;
@@ -2078,7 +2032,7 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
             eff -= 0.001 * cc;                                                     // per-chunk prologue (fresh subjects cost no partials)
             if (eff > best) { best = eff; n_chunks = cc; }
         }
-        if (const char* ov = getenv("RAPID_B200_CHUNKS")) n_chunks = std::max(1, std::min(Sb, atoi(ov)));   // tuning aid
+        if (const char* ov = getenv("RAPID_B200_CHUNKS")) n_chunks = std::max(1, std::min(Sb, atoi(ov)));   // test hook: forced chunk counts
     }
     cd->last_chunks = n_chunks;
     const size_t pn = (size_t)n_chunks * cd->Rpad;
@@ -2140,7 +2094,6 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
     ra.mx_e1 = b->mx_e1.p; ra.mx_e2 = b->mx_e2.p; ra.mx_ec = b->mx_ec.p; ra.mx_changed = b->mx_changed.p; ra.mx_dev = b->mx_dev.p;
     ra.slot_of = cd->slot_of.p; ra.obs = cd->view->obs.p; ra.touch = cd->touch.p; ra.batch_index = b->batch_index.p;
     ra.serial = cd->batch_serial;
-#if RAPID_INVAL_SPLIT
     // blocks per tile of the invalidation pass: enough to fill the device twice over when the tiles alone are far from it.
     // A few tiles walked by one block each leave most SMs idle (BASELINE config 3: 10 tiles); from 64 tiles on the tiles alone
     // spread over the device and extra blocks per tile only add their fixed cost.
@@ -2154,7 +2107,6 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
         RAPID_CUDA(cudaMemsetAsync(b->inv_ticket.p, 0, (size_t)std::max(b->n_tiles, 1) * sizeof(int32_t), s));
     }
     ra.inv_split = inv_split; ra.inv_res = b->inv_res.p; ra.inv_h1 = b->inv_h1.p; ra.inv_h2 = b->inv_h2.p; ra.inv_ticket = b->inv_ticket.p;
-#endif
     const unsigned rblocks = (unsigned)(cd->Rpad / GEN_THREADS);
     const int cgrid = std::max(1, std::min(b->resolve_grid, std::max(32, 4 * (int)rblocks)));      // co-resident (cooperative) grids
     RAPID_CHECK(b->ra_dev.reserve(sizeof(ResolveArgs)));
@@ -2172,11 +2124,7 @@ int32_t bucketed_apply(CD* cd, int64_t A, const DeliveryDev& dl, bool seq) {
     k_finalize1<<<rblocks, GEN_THREADS, 0, s>>>(ga);
     RAPID_KERNEL_CHECK();
     RAPID_CUDA(cudaLaunchCooperativeKernel((void*)k_mixed_flip, dim3((unsigned)cgrid), dim3(GEN_THREADS), args, 0, s));
-#if RAPID_INVAL_SPLIT
     k_inval_finalize2<<<(unsigned)(std::max(b->n_tiles, 1) * inv_split), GEN_THREADS, 0, s>>>(ga);
-#else
-    k_inval_finalize2<<<(unsigned)std::max(b->n_tiles, 1), GEN_THREADS, 0, s>>>(ga);
-#endif
     RAPID_KERNEL_CHECK();
     RAPID_CUDA(cudaLaunchCooperativeKernel((void*)k_marks, dim3((unsigned)cgrid), dim3(GEN_THREADS), args, 0, s));
     cd->last_launches += 5;

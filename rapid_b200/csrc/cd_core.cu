@@ -11,7 +11,6 @@
 // receiver is one CUDA thread (sweep kernel) or a SWAR lane of the subject-bucketed kernels (cd_bucketed.cu).
 #include <algorithm>
 #include <climits>
-#include <cstdio>
 #include <cstdlib>
 
 #include "cd_internal.cuh"
@@ -354,17 +353,6 @@ static void collect(CD* cd) {
     cudaEventElapsedTime(&cd->last_ms, cd->ev0, cd->ev1);
     cudaEventElapsedTime(&cd->last_main_ms, cd->evk0, cd->evk1);
     cudaGetLastError();
-    if (cd->prep_stamps.p && getenv("RAPID_B200_PREP_STAMPS")) {           // profiling aid: phase boundaries of the last k_prepare
-        unsigned long long st[16];
-        if (cudaMemcpy(st, cd->prep_stamps.p, sizeof(st), cudaMemcpyDeviceToHost) == cudaSuccess) {
-            fprintf(stderr, "[k_prepare phases, us]");
-            // stamps 1, 2, 15: after the grid barriers / at the end; 8-11: block 0's progress inside phases 2 and 3
-            static const int order[] = {1, 8, 9, 2, 10, 11, 15};
-            int prev = 0;
-            for (int q = 0; q < 7; ++q) { const int i = order[q]; if (st[i]) { fprintf(stderr, " S%d:+%.1f", i, (double)(st[i] - st[prev]) / 1e3); prev = i; } }
-            fprintf(stderr, " total:%.1f\n", (double)(st[prev] - st[0]) / 1e3);
-        }
-    }
     if (c.sticky_overflow || c.sticky_bad_ring || c.sticky_bad_dst) {
         if (c.sticky_overflow) {
             cd->log_complete = false;                       // a logged batch was not applied after all
@@ -441,19 +429,23 @@ static int32_t check_shuffled(const CD* cd, const rapid_delivery* d, bool sequen
     return RAPID_OK;
 }
 
-static int32_t upload_delivery(CD* cd, int64_t A, const rapid_delivery* d, bool on_device, DeliveryDev* out) {
-    *out = DeliveryDev();
+static int32_t check_delivery(int64_t A, const rapid_delivery* d) {
     if (!d || d->flags == 0) return RAPID_OK;
     if (d->flags & ~(RAPID_DELIVERY_BLOCKED | RAPID_DELIVERY_BITMAP | RAPID_DELIVERY_PERMUTED | RAPID_DELIVERY_SHUFFLED_BATCHES)) { set_error("unknown delivery flags"); return RAPID_EINVAL; }
+    if ((d->flags & RAPID_DELIVERY_BLOCKED) && !d->blocked) { set_error("delivery.blocked is NULL"); return RAPID_EINVAL; }
+    if ((d->flags & RAPID_DELIVERY_BITMAP) && !d->bitmap && A) { set_error("delivery.bitmap is NULL"); return RAPID_EINVAL; }
+    return RAPID_OK;
+}
+
+// a delivery that passed check_delivery; `blocked` is its receiver array in device memory (host arrays travel in the staging blob)
+static int32_t upload_delivery(CD* cd, int64_t A, const rapid_delivery* d, bool on_device, const uint8_t* blocked, DeliveryDev* out) {
+    *out = DeliveryDev();
+    if (!d || d->flags == 0) return RAPID_OK;
     out->flags = d->flags;
     out->perm_seed = d->perm_seed;
     out->words = (cd->R + 31) / 32;
-    if (d->flags & RAPID_DELIVERY_BLOCKED) {
-        if (!d->blocked) { set_error("delivery.blocked is NULL"); return RAPID_EINVAL; }
-        if (on_device) out->blocked = d->blocked;      // host arrays: the caller puts it in the staging blob
-    }
+    if (d->flags & RAPID_DELIVERY_BLOCKED) out->blocked = blocked;
     if (d->flags & RAPID_DELIVERY_BITMAP) {
-        if (!d->bitmap && A) { set_error("delivery.bitmap is NULL"); return RAPID_EINVAL; }
         if (on_device) out->bitmap = d->bitmap;
         else {
             const size_t n = (size_t)A * (size_t)out->words;
@@ -707,7 +699,7 @@ static int32_t bucketed_sequence(CD* cd, int64_t cfg, int64_t A, const int32_t* 
         if (first_rc != RAPID_OK) { set_error("%s", first_msg.c_str()); return first_rc; }
         return RAPID_OK;
     }
-    const bool mergeable = !(dl.flags & RAPID_DELIVERY_BITMAP) && getenv("RAPID_B200_NO_SEQ_MERGE") == nullptr;
+    const bool mergeable = !(dl.flags & RAPID_DELIVERY_BITMAP);
     if (mergeable) {
         DeliveryDev d = dl;
         d.perm_seed = dl.perm_seed + (uint64_t)last;             // the moments that matter are those of the last batch
@@ -754,7 +746,6 @@ static int32_t apply_common(CD* cd, int64_t cfg, int64_t A, const int32_t* dst_d
     RAPID_CUDA(cudaEventRecord(cd->ev0, cd->stream));
     BatchCounts bc;
     RAPID_CHECK(preprocess(cd, cfg, A, dst_dev, ring_dev, status_dev, cfg_dev, &bc));
-    if (dl.flags & RAPID_DELIVERY_PERMUTED) { set_error("the sweep kernel applies cells in array order; RAPID_DELIVERY_PERMUTED needs a bucketed handle"); return RAPID_EUNSUPPORTED; }
     RAPID_CHECK(launch_sweep(cd, A, ring_dev, status_dev, dl, true, !cd->raw, batch_off_dev, n_batches, out_batch_dev));
     RAPID_CUDA(cudaEventRecord(cd->ev1, cd->stream));
     RAPID_CUDA(cudaEventRecord(cd->ev_done, cd->stream));
@@ -763,6 +754,68 @@ static int32_t apply_common(CD* cd, int64_t cfg, int64_t A, const int32_t* dst_d
     cudaEventElapsedTime(&cd->last_main_ms, cd->evk0, cd->evk1);
     cd->last = bc;
     return bad_cell_status(cd, bc);
+}
+
+// Host arrays -> one pinned blob -> ONE host-to-device copy.  Layout: [cfg int64 x n]? [dst int32 x n] [ring u8 x n]
+// [status u8 x n] [blocked u8 x R]?  (8-byte things first so every section is naturally aligned)
+struct Staged { const int32_t* dst; const uint8_t* ring; const uint8_t* status; const int64_t* cfg; const uint8_t* blocked; };
+
+static int32_t stage_cells(rapid_cd* cd, int64_t n, const int32_t* dst, const uint8_t* ring, const uint8_t* status, const int64_t* cfg,
+                           const uint8_t* blocked, Staged* out) {
+    const size_t un = (size_t)n, R = (size_t)cd->R;
+    const size_t o_cfg = 0, o_dst = o_cfg + (cfg ? 8 * un : 0), o_ring = o_dst + 4 * un, o_status = o_ring + un;
+    const size_t o_blk = (o_status + un + 7) & ~(size_t)7, total = o_blk + (blocked ? R : 0);
+    RAPID_CHECK(cd->h_stage.reserve(std::max<size_t>(total, 8)));
+    RAPID_CHECK(cd->d_stage.reserve(std::max<size_t>(total, 8)));
+    uint8_t* h = cd->h_stage.p;
+    if (cfg) memcpy(h + o_cfg, cfg, 8 * un);
+    if (un) { memcpy(h + o_dst, dst, 4 * un); memcpy(h + o_ring, ring, un); memcpy(h + o_status, status, un); }
+    if (blocked) memcpy(h + o_blk, blocked, R);
+    if (total) RAPID_CUDA(cudaMemcpyAsync(cd->d_stage.p, h, total, cudaMemcpyHostToDevice, cd->stream));
+    const uint8_t* d = cd->d_stage.p;
+    out->cfg = cfg ? (const int64_t*)(d + o_cfg) : nullptr;
+    out->dst = (const int32_t*)(d + o_dst);
+    out->ring = d + o_ring;
+    out->status = d + o_status;
+    out->blocked = blocked ? d + o_blk : nullptr;
+    return RAPID_OK;
+}
+
+// The one front door of the rapid_cd_apply_batch* entry points.  Every argument is checked before anything is enqueued, so a
+// refused call leaves the handle exactly as it was; then host arrays are staged, the delivery and a sequence's batch offsets
+// uploaded, and the batch applied.  *applied: apply_common ran (its RAPID_EINVAL means bad cells were dropped, the rest applied).
+static int32_t apply_entry(rapid_cd* cd, int64_t cfg, int64_t n, const int32_t* dst, const uint8_t* ring, const uint8_t* status,
+                           const int64_t* cell_cfg, const rapid_delivery* d, bool on_device, bool async, bool sequence = false,
+                           int64_t n_batches = 0, const int64_t* batch_off = nullptr, bool* applied = nullptr) {
+    if (!cd || n < 0 || (n && (!dst || !ring || !status)) ||
+        (sequence && (n_batches < 0 || n_batches > 0x7ffffff0LL || !batch_off))) { set_error("bad arguments"); return RAPID_EINVAL; }
+    RAPID_CHECK(check_delivery(n, d));
+    RAPID_CHECK(check_shuffled(cd, d, sequence));
+    if (async && !cd->bucketed) { set_error("asynchronous batches run on the subject-bucketed kernels (SERVICE / BUCKETED handles)"); return RAPID_EUNSUPPORTED; }
+    if (cd->raw) { set_error("RAW handles take rapid_cd_aggregate / rapid_cd_invalidate"); return RAPID_EINVAL; }
+    if (!cd->bucketed && d && (d->flags & RAPID_DELIVERY_PERMUTED)) { set_error("the sweep kernel applies cells in array order; RAPID_DELIVERY_PERMUTED needs a bucketed handle"); return RAPID_EUNSUPPORTED; }
+    if (sequence) {
+        if (batch_off[0] != 0 || batch_off[n_batches] != n) { set_error("batch_off must run from 0 to n_cells"); return RAPID_EINVAL; }
+        for (int64_t b = 0; b < n_batches; ++b)
+            if (batch_off[b + 1] < batch_off[b]) { set_error("batch_off must be non-decreasing"); return RAPID_EINVAL; }
+    }
+    DeviceGuard g(cd->device);
+    const uint8_t* blocked = (d && (d->flags & RAPID_DELIVERY_BLOCKED)) ? d->blocked : nullptr;
+    if (!on_device) {
+        Staged st;
+        RAPID_CHECK(stage_cells(cd, n, dst, ring, status, cell_cfg, blocked, &st));
+        dst = st.dst; ring = st.ring; status = st.status; cell_cfg = st.cfg; blocked = st.blocked;
+    }
+    DeliveryDev dl;
+    RAPID_CHECK(upload_delivery(cd, n, d, on_device, blocked, &dl));
+    if (sequence) {
+        RAPID_CHECK(cd->batch_off.reserve((size_t)n_batches + 1));
+        RAPID_CHECK(cd->out_batch.reserve((size_t)cd->Rpad));
+        RAPID_CUDA(cudaMemcpyAsync(cd->batch_off.p, batch_off, (size_t)(n_batches + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, cd->stream));
+    }
+    if (applied) *applied = true;
+    return apply_common(cd, cfg, n, dst, ring, status, cell_cfg, dl, sequence ? cd->batch_off.p : nullptr, (int32_t)n_batches,
+                        sequence ? cd->out_batch.p : nullptr, async, sequence ? batch_off : nullptr);
 }
 
 // getNumProposals of ONE receiver of a bucketed handle: replay its epoch through the literal per-cell rule (the bucketed kernels
@@ -975,51 +1028,14 @@ int32_t rapid_cd_apply_batch_dev(rapid_cd* cd, int64_t cfg_id, int64_t n_cells, 
                                  const uint8_t* ring_dev, const uint8_t* status_dev, const int64_t* cell_cfg_dev,
                                  const rapid_delivery* delivery_dev) {
     (void)src_dev;   // edgeSrc is stored by the Java but never read back (MultiNodeCutDetector.java:101)
-    if (!cd || n_cells < 0 || (n_cells && (!dst_dev || !ring_dev || !status_dev))) { set_error("bad arguments"); return RAPID_EINVAL; }
-    RAPID_CHECK(check_shuffled(cd, delivery_dev, false));
-    if (cd->raw) { set_error("RAW handles take rapid_cd_aggregate / rapid_cd_invalidate"); return RAPID_EINVAL; }
-    DeviceGuard g(cd->device);
-    DeliveryDev dl;
-    RAPID_CHECK(upload_delivery(cd, n_cells, delivery_dev, true, &dl));
-    return apply_common(cd, cfg_id, n_cells, dst_dev, ring_dev, status_dev, cell_cfg_dev, dl);
+    return apply_entry(cd, cfg_id, n_cells, dst_dev, ring_dev, status_dev, cell_cfg_dev, delivery_dev, /*on_device=*/true, /*async=*/false);
 }
 
 int32_t rapid_cd_apply_batch_dev_async(rapid_cd* cd, int64_t cfg_id, int64_t n_cells, const int32_t* src_dev, const int32_t* dst_dev,
                                        const uint8_t* ring_dev, const uint8_t* status_dev, const int64_t* cell_cfg_dev,
                                        const rapid_delivery* delivery_dev) {
     (void)src_dev;
-    if (!cd || n_cells < 0 || (n_cells && (!dst_dev || !ring_dev || !status_dev))) { set_error("bad arguments"); return RAPID_EINVAL; }
-    RAPID_CHECK(check_shuffled(cd, delivery_dev, false));
-    if (!cd->bucketed) { set_error("asynchronous batches run on the subject-bucketed kernels (SERVICE / BUCKETED handles)"); return RAPID_EUNSUPPORTED; }
-    DeviceGuard g(cd->device);
-    DeliveryDev dl;
-    RAPID_CHECK(upload_delivery(cd, n_cells, delivery_dev, true, &dl));
-    return apply_common(cd, cfg_id, n_cells, dst_dev, ring_dev, status_dev, cell_cfg_dev, dl, nullptr, 0, nullptr, true);
-}
-
-// Host arrays -> one pinned blob -> ONE host-to-device copy.  Layout: [cfg int64 x n]? [dst int32 x n] [ring u8 x n]
-// [status u8 x n] [blocked u8 x R]?  (8-byte things first so every section is naturally aligned)
-struct Staged { const int32_t* dst; const uint8_t* ring; const uint8_t* status; const int64_t* cfg; const uint8_t* blocked; };
-
-static int32_t stage_cells(rapid_cd* cd, int64_t n, const int32_t* dst, const uint8_t* ring, const uint8_t* status, const int64_t* cfg,
-                           const uint8_t* blocked, Staged* out) {
-    const size_t un = (size_t)n, R = (size_t)cd->R;
-    const size_t o_cfg = 0, o_dst = o_cfg + (cfg ? 8 * un : 0), o_ring = o_dst + 4 * un, o_status = o_ring + un;
-    const size_t o_blk = (o_status + un + 7) & ~(size_t)7, total = o_blk + (blocked ? R : 0);
-    RAPID_CHECK(cd->h_stage.reserve(std::max<size_t>(total, 8)));
-    RAPID_CHECK(cd->d_stage.reserve(std::max<size_t>(total, 8)));
-    uint8_t* h = cd->h_stage.p;
-    if (cfg) memcpy(h + o_cfg, cfg, 8 * un);
-    if (un) { memcpy(h + o_dst, dst, 4 * un); memcpy(h + o_ring, ring, un); memcpy(h + o_status, status, un); }
-    if (blocked) memcpy(h + o_blk, blocked, R);
-    if (total) RAPID_CUDA(cudaMemcpyAsync(cd->d_stage.p, h, total, cudaMemcpyHostToDevice, cd->stream));
-    const uint8_t* d = cd->d_stage.p;
-    out->cfg = cfg ? (const int64_t*)(d + o_cfg) : nullptr;
-    out->dst = (const int32_t*)(d + o_dst);
-    out->ring = d + o_ring;
-    out->status = d + o_status;
-    out->blocked = blocked ? d + o_blk : nullptr;
-    return RAPID_OK;
+    return apply_entry(cd, cfg_id, n_cells, dst_dev, ring_dev, status_dev, cell_cfg_dev, delivery_dev, /*on_device=*/true, /*async=*/true);
 }
 
 int32_t rapid_cd_apply_batch(rapid_cd* cd, int64_t cfg_id, int64_t n_cells, const int32_t* src, const int32_t* dst,
@@ -1027,18 +1043,7 @@ int32_t rapid_cd_apply_batch(rapid_cd* cd, int64_t cfg_id, int64_t n_cells, cons
                              const rapid_delivery* delivery, uint64_t* proposal_hash, uint64_t* proposal_hash2,
                              int32_t* proposal_len, uint8_t* announced) {
     (void)src;
-    if (!cd || n_cells < 0 || (n_cells && (!dst || !ring || !status))) { set_error("bad arguments"); return RAPID_EINVAL; }
-    RAPID_CHECK(check_shuffled(cd, delivery, false));
-    if (cd->raw) { set_error("RAW handles take rapid_cd_aggregate / rapid_cd_invalidate"); return RAPID_EINVAL; }
-    DeviceGuard g(cd->device);
-    Staged st;
-    const bool has_blocked = delivery && (delivery->flags & RAPID_DELIVERY_BLOCKED);
-    if (has_blocked && !delivery->blocked) { set_error("delivery.blocked is NULL"); return RAPID_EINVAL; }
-    RAPID_CHECK(stage_cells(cd, n_cells, dst, ring, status, cell_cfg, has_blocked ? delivery->blocked : nullptr, &st));
-    DeliveryDev dl;
-    RAPID_CHECK(upload_delivery(cd, n_cells, delivery, false, &dl));
-    if (has_blocked) dl.blocked = st.blocked;          // travelled in the staging blob
-    RAPID_CHECK(apply_common(cd, cfg_id, n_cells, st.dst, st.ring, st.status, st.cfg, dl));
+    RAPID_CHECK(apply_entry(cd, cfg_id, n_cells, dst, ring, status, cell_cfg, delivery, /*on_device=*/false, /*async=*/false));
     if (proposal_hash || proposal_hash2 || proposal_len || announced)
         return rapid_cd_read_outputs(cd, proposal_hash, proposal_hash2, proposal_len, announced);
     return RAPID_OK;
@@ -1051,26 +1056,11 @@ int32_t rapid_cd_apply_batches(rapid_cd* cd, int64_t cfg_id, int64_t n_cells, co
                                const rapid_delivery* delivery, uint64_t* proposal_hash, uint64_t* proposal_hash2, int32_t* proposal_len,
                                uint8_t* announced, int32_t* announced_in) {
     (void)src;
-    if (!cd || n_cells < 0 || (n_cells && (!dst || !ring || !status)) || n_batches < 0 || n_batches > 0x7ffffff0LL || !batch_off) { set_error("bad arguments"); return RAPID_EINVAL; }
-    RAPID_CHECK(check_shuffled(cd, delivery, true));
-    if (cd->raw) { set_error("RAW handles take rapid_cd_aggregate / rapid_cd_invalidate"); return RAPID_EINVAL; }
-    if (batch_off[0] != 0 || batch_off[n_batches] != n_cells) { set_error("batch_off must run from 0 to n_cells"); return RAPID_EINVAL; }
-    for (int64_t b = 0; b < n_batches; ++b)
-        if (batch_off[b + 1] < batch_off[b]) { set_error("batch_off must be non-decreasing"); return RAPID_EINVAL; }
+    bool applied = false;
+    const int32_t rc = apply_entry(cd, cfg_id, n_cells, dst, ring, status, cell_cfg, delivery, /*on_device=*/false, /*async=*/false,
+                                   /*sequence=*/true, n_batches, batch_off, &applied);
+    if (!applied || (rc != RAPID_OK && rc != RAPID_EINVAL)) return rc;   // RAPID_EINVAL: bad cells were dropped, the rest was applied
     DeviceGuard g(cd->device);
-    Staged st;
-    const bool has_blocked = delivery && (delivery->flags & RAPID_DELIVERY_BLOCKED);
-    if (has_blocked && !delivery->blocked) { set_error("delivery.blocked is NULL"); return RAPID_EINVAL; }
-    RAPID_CHECK(stage_cells(cd, n_cells, dst, ring, status, cell_cfg, has_blocked ? delivery->blocked : nullptr, &st));
-    DeliveryDev dl;
-    RAPID_CHECK(upload_delivery(cd, n_cells, delivery, false, &dl));
-    if (has_blocked) dl.blocked = st.blocked;
-    RAPID_CHECK(cd->batch_off.reserve((size_t)n_batches + 1));
-    RAPID_CHECK(cd->out_batch.reserve((size_t)cd->Rpad));
-    RAPID_CUDA(cudaMemcpyAsync(cd->batch_off.p, batch_off, (size_t)(n_batches + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, cd->stream));
-    if (!cd->bucketed && (dl.flags & RAPID_DELIVERY_PERMUTED)) { set_error("the sweep kernel applies cells in array order; RAPID_DELIVERY_PERMUTED needs a bucketed handle"); return RAPID_EUNSUPPORTED; }
-    const int32_t rc = apply_common(cd, cfg_id, n_cells, st.dst, st.ring, st.status, st.cfg, dl, cd->batch_off.p, (int32_t)n_batches, cd->out_batch.p, false, batch_off);
-    if (rc != RAPID_OK && rc != RAPID_EINVAL) return rc;         // RAPID_EINVAL: bad cells were dropped, the rest was applied
     char msg[512];
     if (rc != RAPID_OK) rapid_last_error(msg, sizeof(msg));
     RAPID_CHECK(cd_wait(cd, false));
@@ -1087,20 +1077,8 @@ int32_t rapid_cd_apply_batches_dev(rapid_cd* cd, int64_t cfg_id, int64_t n_cells
                                    const uint8_t* ring_dev, const uint8_t* status_dev, const int64_t* cell_cfg_dev, int64_t n_batches,
                                    const int64_t* batch_off, const rapid_delivery* delivery_dev) {
     (void)src_dev;
-    if (!cd || n_cells < 0 || (n_cells && (!dst_dev || !ring_dev || !status_dev)) || n_batches < 0 || n_batches > 0x7ffffff0LL || !batch_off) { set_error("bad arguments"); return RAPID_EINVAL; }
-    RAPID_CHECK(check_shuffled(cd, delivery_dev, true));
-    if (cd->raw) { set_error("RAW handles take rapid_cd_aggregate / rapid_cd_invalidate"); return RAPID_EINVAL; }
-    if (batch_off[0] != 0 || batch_off[n_batches] != n_cells) { set_error("batch_off must run from 0 to n_cells"); return RAPID_EINVAL; }
-    for (int64_t b = 0; b < n_batches; ++b)
-        if (batch_off[b + 1] < batch_off[b]) { set_error("batch_off must be non-decreasing"); return RAPID_EINVAL; }
-    DeviceGuard g(cd->device);
-    DeliveryDev dl;
-    RAPID_CHECK(upload_delivery(cd, n_cells, delivery_dev, true, &dl));
-    if (!cd->bucketed && (dl.flags & RAPID_DELIVERY_PERMUTED)) { set_error("the sweep kernel applies cells in array order; RAPID_DELIVERY_PERMUTED needs a bucketed handle"); return RAPID_EUNSUPPORTED; }
-    RAPID_CHECK(cd->batch_off.reserve((size_t)n_batches + 1));
-    RAPID_CHECK(cd->out_batch.reserve((size_t)cd->Rpad));
-    RAPID_CUDA(cudaMemcpyAsync(cd->batch_off.p, batch_off, (size_t)(n_batches + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, cd->stream));
-    return apply_common(cd, cfg_id, n_cells, dst_dev, ring_dev, status_dev, cell_cfg_dev, dl, cd->batch_off.p, (int32_t)n_batches, cd->out_batch.p, false, batch_off);
+    return apply_entry(cd, cfg_id, n_cells, dst_dev, ring_dev, status_dev, cell_cfg_dev, delivery_dev, /*on_device=*/true, /*async=*/false,
+                       /*sequence=*/true, n_batches, batch_off);
 }
 
 int32_t rapid_cd_read_announced_in(const rapid_cd* cd, int32_t* announced_in) {

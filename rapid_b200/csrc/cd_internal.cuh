@@ -132,7 +132,6 @@ struct CD {
     int64_t est_A = 0;
     BatchCounts last;                 // counters of the last collected batch
     int32_t retries = 0;              // batches replayed after growing the subject capacity
-    DevBuf<unsigned long long> prep_stamps;   // RAPID_B200_PREP_STAMPS profiling aid
     // bucketed scratch lives in cd_bucketed.cu's own struct hung off here
     void* bucketed_state = nullptr;
 

@@ -52,7 +52,6 @@ struct PrepArgs {
     PrepOut po;
     const int64_t* batch_off;     // sequences of batches: [n_batches + 1] cell offsets (device), else nullptr
     int32_t n_batches, seq_last;
-    unsigned long long* stamps;   // profiling aid (RAPID_B200_PREP_STAMPS): %globaltimer of block 0 at every phase boundary
 };
 
 // exclusive scan of one int per thread across the block; returns the thread's offset, *total = block sum
@@ -104,20 +103,11 @@ constexpr int PREP_BIN = 64;          // cells of one subject kept in its bin; t
 constexpr int PREP_REG = 32;          // ... of which this many are sorted in registers (~K cells per subject and batch; a few more with
                                      // re-sent duplicates or when a whole sequence of batches is prepared at once)
 
-__device__ __forceinline__ void prep_stamp(const PrepArgs& a, int i) {
-    if (a.stamps && blockIdx.x == 0 && threadIdx.x == 0) {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        a.stamps[i] = t;
-    }
-}
-
 __global__ void __launch_bounds__(PREP_THREADS) k_prepare(PrepArgs a) {
     cg::grid_group grid = cg::this_grid();
     __shared__ int32_t warp_sums[PREP_THREADS / 32];
     __shared__ int32_t s_base;
     const int t = threadIdx.x, G = gridDim.x, bid = blockIdx.x;
-    prep_stamp(a, 0);
     // slots in use before this batch: the host's number (sweep handles) or the device's (bucketed handles keep it on the
     // device: bc->S_before == bc->n_slots between batches — nobody writes S_before while this kernel runs)
     if (a.S_old < 0) a.S_old = a.bc->S_before;
@@ -169,7 +159,6 @@ __global__ void __launch_bounds__(PREP_THREADS) k_prepare(PrepArgs a) {
         }
     }
     grid.sync();
-    prep_stamp(a, 1);
     const int32_t S_new = *(volatile int32_t*)&a.bc->n_slots;
     if (S_new > a.S_cap) {
         // More subjects than the handle has rows for: undo the slot assignment of this batch and apply NOTHING (the host
@@ -211,7 +200,6 @@ __global__ void __launch_bounds__(PREP_THREADS) k_prepare(PrepArgs a) {
         if (t == 0 && total) atomicAdd(&a.bc->n_valid, total);
     }
     if (!a.regroup) return;
-    prep_stamp(a, 8);                                   // (sub-stamps: block 0's own progress inside a phase)
     if (a.wl.has_so && S_new > a.S_old) {
         // Some subject got a slot: refresh "which observers of this subject are subjects themselves" for every slot.  Only
         // subjects with such an observer can ever receive an implicit report (MultiNodeCutDetector.java:147-158), so only
@@ -240,9 +228,7 @@ __global__ void __launch_bounds__(PREP_THREADS) k_prepare(PrepArgs a) {
             }
         }
     }
-    prep_stamp(a, 9);
     grid.sync();
-    prep_stamp(a, 2);
     // ---- P3: per subject: arrival order, segment, descriptor -------------------------------------------------------------------
     const int32_t Sb = *(volatile int32_t*)&a.bc->n_batch_subj;
     const int32_t n_ovf = *(volatile int32_t*)&a.ctr[1];
@@ -261,7 +247,6 @@ __global__ void __launch_bounds__(PREP_THREADS) k_prepare(PrepArgs a) {
         __syncthreads();
         if (!on) continue;
         const int32_t seg_begin = s_base + off;
-        prep_stamp(a, 10);
         int32_t* seg = a.po.sidx + seg_begin;
         SubjDesc d;
         d.slot = slot; d.bmask = 0; d.nr = 0; d.any_down = 0; d.tLf = 0; d.tHf = 0;
@@ -361,7 +346,6 @@ __global__ void __launch_bounds__(PREP_THREADS) k_prepare(PrepArgs a) {
                 }
             for (int32_t e = 0; e < len; ++e) { const int32_t ci = seg[e]; take(e, ci, a.ring[ci], a.status[ci], a.batch_off ? a.po.cell_batch[ci] : 0); }
         }
-        prep_stamp(a, 11);
         for (int q = d.nr; q < 16; ++q) { w.ring[q] = 0; w.time[q] = 0; }
         const int32_t id = a.slot_subject[slot];
         d.mix1 = fp_mix1(id);
@@ -375,7 +359,6 @@ __global__ void __launch_bounds__(PREP_THREADS) k_prepare(PrepArgs a) {
             a.po.pwalk[b] = pw;
         }
     }
-    prep_stamp(a, 15);
 }
 
 int32_t prepare_batch(CD* cd, int64_t cfg, int64_t A, const int32_t* dst_dev, const uint8_t* ring_dev, const uint8_t* status_dev,
@@ -391,7 +374,7 @@ int32_t prepare_batch(CD* cd, int64_t cfg, int64_t A, const int32_t* dst_dev, co
         cd->prep_grid_max = std::max(1, sms * std::max(per, 1));
     }
     int G = (int)std::max<int64_t>(1, std::min<int64_t>(cd->prep_grid_max, ceil_div<int64_t>(A, PREP_THREADS * 2)));
-    if (const char* ov = getenv("RAPID_B200_PREP_GRID")) G = std::max(1, std::min(cd->prep_grid_max, atoi(ov)));   // tuning aid
+    if (const char* ov = getenv("RAPID_B200_PREP_GRID")) G = std::max(1, std::min(cd->prep_grid_max, atoi(ov)));   // test hook: forced grids
     cd->last_prep_grid = G;
     RAPID_CHECK(cd->scan_sums.reserve(8));
     PrepArgs a;
@@ -409,12 +392,6 @@ int32_t prepare_batch(CD* cd, int64_t cfg, int64_t A, const int32_t* dst_dev, co
     a.regroup = po ? 1 : 0;
     a.batch_off = (po && cd->bucketed) ? batch_off_dev : nullptr; a.n_batches = n_batches; a.seq_last = a.batch_off ? seq_last : 0;
     if (po) a.po = *po; else memset(&a.po, 0, sizeof(a.po));
-    a.stamps = nullptr;
-    if (getenv("RAPID_B200_PREP_STAMPS")) {
-        RAPID_CHECK(cd->prep_stamps.reserve(16));
-        RAPID_CUDA(cudaMemsetAsync(cd->prep_stamps.p, 0, 16 * sizeof(unsigned long long), s));
-        a.stamps = cd->prep_stamps.p;
-    }
     void* args[] = {(void*)&a};
     RAPID_CUDA(cudaLaunchCooperativeKernel((void*)k_prepare, dim3((unsigned)G), dim3(PREP_THREADS), args, 0, s));
     cd->last_launches += 1;

@@ -787,7 +787,7 @@ static int32_t tally_cd_collect(rapid_fp* fp, int32_t* decided, uint64_t* decide
     rapid_comm* comm = fp->pending_comm;
     if (comm == nullptr)
         return take_result(fp, decided, decided_hash, decided_hash2, decided_len, decided_count, votes_received, decided_in_call);
-    if (getenv("RAPID_B200_FORCE_REFINE") == nullptr) {
+    if (getenv("RAPID_B200_FORCE_REFINE") == nullptr) {              // (test hook, see above)
         const FPSumResult res = *(const FPSumResult*)fp->h_res_raw.p;
         if (!res.ambiguous) {
             if (res.r.decided) fp->decided_host = true;

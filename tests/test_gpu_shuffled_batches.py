@@ -119,19 +119,21 @@ def test_refusals_change_nothing(rb, world):
     for kernel in ("sweep", "bucketed"):
         cl = rb.VirtualCluster(world["v"], H, L, kernel=kernel)
         cl.handleBatch(cfg, src[: off[3]], dst[: off[3]], ring[: off[3]], st[: off[3]])   # some state to keep
-        before = (_state(cl, rs), cl.readOutputs().proposal_len.copy())
+        before = (_state(cl, rs), cl.readOutputs().proposal_len.copy(), cl.lastPath())
         calls = [lambda: cl.handleBatches(cfg, src, dst, ring, st, off, batch_order_seed=1, perm_seed=2),
                  lambda: cl.handleBatches(cfg, src, dst, ring, st, off, batch_order_seed=1,
                                           bitmap=np.full((len(dst), (N + 31) // 32), 0xFFFFFFFF, np.uint32))]
         if kernel == "bucketed":
             calls.append(lambda: cl.handleBatches(cfg, src, dst, ring, st, off, batch_order_seed=1))
+        else:                                                     # PERMUTED needs a bucketed handle: refused before k_prepare runs
+            calls.append(lambda: cl.handleBatch(cfg, src, dst, ring, st, perm_seed=3))
         for i, call in enumerate(calls):
             with pytest.raises(N_.RapidError) as e:
                 call()
             want = N_.EUNSUPPORTED if i == 2 else N_.EINVAL
             assert e.value.code == want, (kernel, i, str(e.value))
             if i == 2:
-                assert "RAPID_CD_SWEEP" in str(e.value)
+                assert ("RAPID_CD_SWEEP" if kernel == "bucketed" else "needs a bucketed handle") in str(e.value)
         d = N_.Delivery()
         d.flags, d.perm_seed = N_.DELIVERY_SHUFFLED_BATCHES, 1
         rc = N_.lib().rapid_cd_apply_batch(cl._h, int(cfg), len(dst), N_.ptr(src), N_.ptr(dst), N_.ptr(ring), N_.ptr(st), None,
@@ -139,6 +141,7 @@ def test_refusals_change_nothing(rb, world):
         assert rc == N_.EINVAL
         assert _state(cl, rs) == before[0]
         np.testing.assert_array_equal(cl.readOutputs().proposal_len, before[1])
+        assert cl.lastPath() == before[2], kernel
     raw = rb.MultiNodeCutDetector(world["v"], H, L, n_detectors=4)
     for i in range(0, 40, 7):
         raw.aggregateForProposal(int(src[i]), int(dst[i]), int(st[i]), [int(ring[i])], detector=i % 4)
