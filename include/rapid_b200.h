@@ -258,6 +258,23 @@ int32_t rapid_cd_read_outputs(const rapid_cd* cd, uint64_t* proposal_hash, uint6
 /* The proposal receiver r announced, in canonical order = sorted by the ring-0 comparator
  * (MembershipService.java:346-348). */
 int32_t rapid_cd_get_proposal(const rapid_cd* cd, int64_t receiver, int32_t* out_ids, int32_t cap, int32_t* out_len);
+/* Census of the receivers that announced in cd's last call (those rapid_fp_tally_cd counts): *n_classes distinct proposals,
+ * *n_entries ids over all their lists.  Class c is the c-th lowest receiver of a distinct (hash, hash2, len) in receiver order (the
+ * wire encoder's body numbering); its list is rapid_cd_get_proposal(its representative), each entry with a status,
+ * RAPID_EDGE_DOWN for a member and RAPID_EDGE_UP for a registered joiner (VIEW_CHANGE_PROPOSAL's NodeStatusChange list,
+ * MembershipService.java:336-345, :586-593).  cut_ids may be NULL (then in_cut reads -1); else in_cut[c] = entries of class c in
+ * the cut.  Results stay on the handle until the next census; a refused call leaves the previous census bit-identical.
+ * RAPID_EINVAL: a RAW handle, a handle that has applied no batch or was created before the view's members last changed, cut ids
+ * outside [0, members + registered joiners) or repeated.  On a sharded handle representatives are local receiver indices.
+ * Waits for the handle's asynchronous batches; synchronises once, for the counts. */
+int32_t rapid_cd_proposal_census(rapid_cd* cd, const int32_t* cut_ids, int32_t cut_len, int64_t* n_classes, int64_t* n_entries);
+/* any pointer may be NULL; arrays sized by the counts above (list_off: n_classes + 1; class c's entries are
+ * ids[list_off[c] .. list_off[c + 1])) */
+int32_t rapid_cd_read_census(const rapid_cd* cd, uint64_t* hash, uint64_t* hash2, int32_t* len, int32_t* voters,
+                             int32_t* representative, int32_t* in_cut, int64_t* list_off, int32_t* ids, uint8_t* status);
+/* class of every receiver, [R], -1 = did not announce: device memory of the handle, valid until the next census */
+int32_t rapid_cd_census_classes_dev(const rapid_cd* cd, const int32_t** cls_dev);
+int32_t rapid_cd_read_census_classes(const rapid_cd* cd, int32_t* cls);
 /* getNumProposals :62-66 (the reference's tests are its only caller).  Sweep handles count while they walk the cells.
  * Subject-bucketed handles never see a receiver's cells in order, so they answer by REPLAYING that one receiver through the
  * literal per-cell rule over the epoch's cell log — exact; needs RAPID_CD_LOG at creation (RAPID_EUNSUPPORTED otherwise, or once

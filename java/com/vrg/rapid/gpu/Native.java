@@ -50,6 +50,16 @@ public final class Native {
                                           ByteBuffer bitmap, long permSeed, ByteBuffer outHash, ByteBuffer outHash2,
                                           ByteBuffer outLen, ByteBuffer outAnnounced);
     public static native int cdGetProposal(long cd, long receiver, int[] outIds);      // returns length or <0
+    /** rapid_cd_proposal_census: the distinct proposals announced in the detector's last call (VIEW_CHANGE_PROPOSAL's payload,
+     *  one NodeStatusChange list per class).  cutIds may be null; out2 = {classes, entries}. */
+    public static native int cdProposalCensus(long cd, int[] cutIds, long[] out2);
+    /** rapid_cd_read_census into direct buffers (any may be null): hash, hash2 uint64[classes], len, voters, representative,
+     *  inCut int32[classes], listOff int64[classes + 1], ids int32[entries], status uint8[entries] (0 = UP, 1 = DOWN) */
+    public static native int cdReadCensus(long cd, ByteBuffer hash, ByteBuffer hash2, ByteBuffer len, ByteBuffer voters,
+                                          ByteBuffer representative, ByteBuffer inCut, ByteBuffer listOff, ByteBuffer ids,
+                                          ByteBuffer status);
+    /** class of every receiver of the last census, -1 = did not announce */
+    public static native int cdReadCensusClasses(long cd, int[] cls);
     public static native int cdAggregate(long cd, int[] dst, byte[] ring, byte[] status, long receiver, int[] outIds);
     public static native int cdInvalidate(long cd, long receiver, int[] outIds);
     public static native int cdNumProposals(long cd, long receiver);

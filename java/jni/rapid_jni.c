@@ -201,6 +201,32 @@ JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_cdGetProposal(JNIEnv* env, 
     return rc == RAPID_OK ? len : rc;
 }
 
+/* cutIds == NULL: no cut (in_cut reads -1); out2 = {n_classes, n_entries} */
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_cdProposalCensus(JNIEnv* env, jclass c, jlong cd, jintArray cutIds, jlongArray out2) {
+    const jsize n = cutIds ? (*env)->GetArrayLength(env, cutIds) : 0;
+    jint* ids = cutIds ? (*env)->GetIntArrayElements(env, cutIds, NULL) : NULL;
+    int64_t counts[2] = {0, 0};
+    const int32_t rc = rapid_cd_proposal_census(H(rapid_cd, cd), (const int32_t*)ids, n, &counts[0], &counts[1]);
+    if (ids) (*env)->ReleaseIntArrayElements(env, cutIds, ids, JNI_ABORT);
+    if (rc == RAPID_OK) (*env)->SetLongArrayRegion(env, out2, 0, 2, (const jlong*)counts);
+    return rc;
+}
+
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_cdReadCensus(JNIEnv* env, jclass c, jlong cd, jobject hash, jobject hash2, jobject len,
+                                                                  jobject voters, jobject representative, jobject inCut, jobject listOff,
+                                                                  jobject ids, jobject status) {
+    return rapid_cd_read_census(H(rapid_cd, cd), (uint64_t*)BUF(env, hash), (uint64_t*)BUF(env, hash2), (int32_t*)BUF(env, len),
+                                (int32_t*)BUF(env, voters), (int32_t*)BUF(env, representative), (int32_t*)BUF(env, inCut),
+                                (int64_t*)BUF(env, listOff), (int32_t*)BUF(env, ids), (uint8_t*)BUF(env, status));
+}
+
+JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_cdReadCensusClasses(JNIEnv* env, jclass c, jlong cd, jintArray cls) {
+    jint* o = (*env)->GetIntArrayElements(env, cls, NULL);
+    const int32_t rc = rapid_cd_read_census_classes(H(rapid_cd, cd), (int32_t*)o);
+    (*env)->ReleaseIntArrayElements(env, cls, o, 0);
+    return rc;
+}
+
 JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_cdAggregate(JNIEnv* env, jclass c, jlong cd, jintArray dst, jbyteArray ring,
                                                                  jbyteArray status, jlong receiver, jintArray out) {
     const jsize n = (*env)->GetArrayLength(env, dst), cap = (*env)->GetArrayLength(env, out);

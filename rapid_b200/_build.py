@@ -8,7 +8,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librapid_b200.so")
-SOURCES = ["api.cu", "view.cu", "overlay.cu", "cd_core.cu", "cd_prepare.cu", "cd_bucketed.cu", "fast_paxos.cu", "classic_paxos.cu", "wire.cu", "wire_encode.cu", "fd.cu"]
+SOURCES = ["api.cu", "view.cu", "overlay.cu", "cd_core.cu", "cd_census.cu", "cd_prepare.cu", "cd_bucketed.cu", "fast_paxos.cu", "classic_paxos.cu", "wire.cu", "wire_encode.cu", "fd.cu"]
 HEADERS = ["common.cuh", "cd_internal.cuh", "nccl_api.cuh", "scan.cuh", "radix.cuh", "wire_internal.cuh", os.path.join("..", "..", "include", "rapid_b200.h")]
 ARCH = "sm_90a"
 GENCODE = ["-gencode", "arch=compute_90a,code=" + ARCH]

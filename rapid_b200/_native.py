@@ -91,6 +91,10 @@ SIGNATURES = {
     "rapid_cd_read_outputs": [_vp, _p, _p, _p, _p],
     "rapid_cd_get_proposal": [_vp, _i64, _p, _i32, _p],
     "rapid_cd_num_proposals": [_vp, _i64, _p],
+    "rapid_cd_proposal_census": [_vp, _p, _i32, _p, _p],
+    "rapid_cd_read_census": [_vp, _p, _p, _p, _p, _p, _p, _p, _p, _p],
+    "rapid_cd_census_classes_dev": [_vp, _p],
+    "rapid_cd_read_census_classes": [_vp, _p],
     "rapid_cd_clear": [_vp],
     "rapid_cd_debug_masks": [_vp, _i64, _p, _p, _i32, _p],
     "rapid_cd_debug_counters": [_vp, _i64, _p, _p],

@@ -195,20 +195,14 @@ __global__ void k_clear_call(RowRef rows, int32_t S, int64_t R) {
     if (w & CD_BIT_CALL) *p = (uint16_t)(w & ~CD_BIT_CALL);
 }
 
-// the announced proposal of one receiver: (id, ring-0 key) pairs.  Bucketed handles (emit.p != nullptr) keep bit 15 in the emit
-// plane.  That plane is written for every slot < S when the receiver announces, and never cleared: slots assigned later may carry
-// marks of an earlier configuration epoch.  A mark always comes with >= H, and a receiver that has announced is frozen, so its
-// word in a slot assigned later stays zero.  Requiring both therefore lists exactly the marked subjects of this epoch.
+// the announced proposal of one receiver: (id, ring-0 key) pairs (in_announced_proposal, cd_internal.cuh)
 __global__ void k_gather_proposal(RowRef rows, MarkPlane emit, int32_t S, int64_t r, int H, uint32_t RM, int rule_ge_h,
                                   const int32_t* __restrict__ slot_subject, const int64_t* __restrict__ key0,
                                   int32_t* __restrict__ out_ids, int64_t* __restrict__ out_keys, int32_t cap,
                                   int32_t* __restrict__ count) {
     const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= S) return;
-    const uint32_t w = rows.get(s, r);
-    const bool ge_h = __popc(w & RM) >= H;
-    const bool in = rule_ge_h ? ge_h : emit.p ? (ge_h && emit.test(s, r)) : ((w & CD_BIT_EMIT) != 0);
-    if (in) {
+    if (in_announced_proposal(rows, emit, s, r, H, RM, rule_ge_h)) {
         const int32_t at = atomicAdd(count, 1);
         if (at < cap) { const int32_t id = slot_subject[s]; out_ids[at] = id; out_keys[at] = key0[id]; }
     }
@@ -245,9 +239,6 @@ __global__ void k_clear_receivers(int64_t R, int32_t* __restrict__ n_pre, int32_
 // =====================================================================================================
 // host side
 // =====================================================================================================
-static RowRef rowref(const CD* cd) { return RowRef{cd->masks.p, cd->cur.p, cd->Rpad, cd->row_stride, cd->nbuf, cd->hb}; }
-static MarkPlane emit_plane(const CD* cd) { return MarkPlane{cd->bucketed ? cd->emit_marks.p : nullptr, cd->Rpad / 32}; }
-
 static int32_t ensure_id_capacity(CD* cd) {
     const int64_t ntot = cd->view->n + cd->view->nj;
     if (ntot <= cd->ntot_cap) return RAPID_OK;
@@ -948,6 +939,7 @@ int32_t rapid_cd_destroy(rapid_cd* cd) {
     DeviceGuard g(cd->device);
     if (cd->stream) cudaStreamSynchronize(cd->stream);
     bucketed_destroy(cd);
+    census_destroy(cd);
     if (cd->ev0) cudaEventDestroy(cd->ev0);
     if (cd->ev1) cudaEventDestroy(cd->ev1);
     if (cd->evk0) cudaEventDestroy(cd->evk0);

@@ -139,6 +139,8 @@ struct CD {
     int32_t last_chunks = 0, last_prep_grid = 0;   // grid of the last batch: subject chunks of the apply kernel, k_prepare blocks
     float last_ms = 0.f, last_main_ms = 0.f;
     int64_t last_A = 0;
+    // the proposal census (cd_census.cu): scratch and its two output sets, created by the first census
+    struct Census* census = nullptr;
 };
 
 // ---- state rows: the only code that knows how a row stores the logical words ---------------------------------------------
@@ -327,6 +329,21 @@ struct MarkPlane {
     __device__ __forceinline__ bool test(int32_t slot, int64_t r) const { return (*word(slot, r) >> (r & 31)) & 1u; }
 };
 
+inline RowRef rowref(const CD* cd) { return RowRef{cd->masks.p, cd->cur.p, cd->Rpad, cd->row_stride, cd->nbuf, cd->hb}; }
+inline MarkPlane emit_plane(const CD* cd) { return MarkPlane{cd->bucketed ? cd->emit_marks.p : nullptr, cd->Rpad / 32}; }
+
+// Is subject slot s in the proposal receiver r announced?  rule_ge_h: r's RF_RULE_GE_H flag.  Bucketed handles (emit.p != nullptr)
+// keep bit 15 in the emit plane.  That plane is written for every slot < S when the receiver announces, and never cleared: slots
+// assigned later may carry marks of an earlier configuration epoch.  A mark always comes with >= H, and a receiver that has
+// announced is frozen, so its word in a slot assigned later stays zero.  Requiring both therefore lists exactly the marked
+// subjects of this epoch.  (rapid_cd_get_proposal and the proposal census both list proposals by this rule.)
+__device__ __forceinline__ bool in_announced_proposal(const RowRef& rows, const MarkPlane& emit, int32_t s, int64_t r, int H, uint32_t RM,
+                                                      int rule_ge_h) {
+    const uint32_t w = rows.get(s, r);
+    const bool ge_h = __popc(w & RM) >= H;
+    return rule_ge_h ? ge_h : emit.p ? (ge_h && emit.test(s, r)) : ((w & CD_BIT_EMIT) != 0);
+}
+
 struct DeliveryDev {
     uint32_t flags = 0;
     const uint8_t* blocked = nullptr;
@@ -413,6 +430,8 @@ int32_t bucketed_clear_sticky(CD* cd);
 // Wait for everything enqueued on the handle and collect the outcome of asynchronous batches (host mirrors of the slot count,
 // timings, latched errors).  Returns the latched status (and clears it) when take_status is set.
 int32_t cd_wait(const CD* cd, bool take_status);
+// implemented in cd_census.cu
+void census_destroy(CD* cd);
 
 }  // namespace rapid
 

@@ -149,6 +149,28 @@ RAPID_HD int64_t batch_order_at(const BatchOrder& o, int64_t j) {
 RAPID_HD uint64_t fp_mix1(int32_t id) { return splitmix64((uint64_t)(uint32_t)id ^ 0x52415049445F4831ULL); }
 RAPID_HD uint64_t fp_mix2(int32_t id) { return splitmix64(((uint64_t)(uint32_t)id * 0xD6E8FEB86659FD93ULL) ^ 0x52415049445F4832ULL); }
 
+#ifdef __CUDACC__
+// Open addressing over proposal fingerprints (a, b, l) = (h1, h2, len) in a table of T (a power of two) slots, empty slots -1:
+// item s claims the slot of its fingerprint, and the slot keeps the LOWEST item holding it (atomicCAS, then atomicMin).
+// fp(i, &a, &b, &l) reads item i's fingerprint.  Returns the slot.  The wire encoder numbers its bodies and the proposal census
+// its classes this way.
+template <typename FP>
+__device__ __forceinline__ uint32_t fp_table_claim(int32_t* table, uint32_t T, int32_t s, uint64_t a, uint64_t b, int32_t l, const FP& fp) {
+    uint32_t pos = (uint32_t)(splitmix64(a ^ (b * 0x9E3779B97F4A7C15ULL) ^ (uint64_t)l) >> 32) & (T - 1);
+    for (;;) {
+        int32_t cur = table[pos];
+        if (cur < 0) {
+            cur = atomicCAS(&table[pos], -1, s);
+            if (cur < 0) return pos;
+        }
+        uint64_t ca, cb; int32_t cl;
+        fp(cur, &ca, &cb, &cl);
+        if (ca == a && cb == b && cl == l) { atomicMin(&table[pos], s); return pos; }
+        pos = (pos + 1) & (T - 1);
+    }
+}
+#endif
+
 #define XXP1 0x9E3779B185EBCA87ULL
 #define XXP2 0xC2B2AE3D27D4EB4FULL
 #define XXP3 0x165667B19E3779F9ULL

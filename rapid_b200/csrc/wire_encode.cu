@@ -223,8 +223,8 @@ RAPID_HD uint8_t list_tag(int32_t kind) {                                  // en
     return kind == RAPID_WIRE_FAST_ROUND_PHASE2B ? 0x1A : kind == RAPID_WIRE_PHASE1B ? 0x2A : 0x22;
 }
 
-// every slot with a non-empty list claims the table slot of the list's fingerprint; the slot keeps the LOWEST such slot (the
-// body's representative)
+// every slot with a non-empty list claims the table slot of the list's fingerprint (fp_table_claim); the slot keeps the LOWEST
+// such slot (the body's representative)
 __global__ void k_enc_list_claim(ListIn L, uint32_t T, int32_t* __restrict__ table, int32_t* __restrict__ slot, int32_t* __restrict__ send) {
     const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= L.n) return;
@@ -233,19 +233,8 @@ __global__ void k_enc_list_claim(ListIn L, uint32_t T, int32_t* __restrict__ tab
     uint64_t a, b; int32_t l;
     list_fp(L, s, &a, &b, &l);
     if (!v || l <= 0) { slot[s] = -1; return; }
-    uint32_t pos = (uint32_t)(splitmix64(a ^ (b * 0x9E3779B97F4A7C15ULL) ^ (uint64_t)l) >> 32) & (T - 1);
-    for (;;) {
-        int32_t cur = table[pos];
-        if (cur < 0) {
-            cur = atomicCAS(&table[pos], -1, s);
-            if (cur < 0) break;
-        }
-        uint64_t ca, cb; int32_t cl;
-        list_fp(L, cur, &ca, &cb, &cl);
-        if (ca == a && cb == b && cl == l) { atomicMin(&table[pos], s); break; }
-        pos = (pos + 1) & (T - 1);
-    }
-    slot[s] = (int32_t)pos;
+    const auto fp = [&](int32_t i, uint64_t* ca, uint64_t* cb, int32_t* cl) { list_fp(L, i, ca, cb, cl); };
+    slot[s] = (int32_t)fp_table_claim(table, T, s, a, b, l, fp);
 }
 __global__ void k_enc_list_rep(int32_t n, const int32_t* __restrict__ slot, const int32_t* __restrict__ table, int32_t* __restrict__ rep) {
     const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;

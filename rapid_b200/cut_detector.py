@@ -82,6 +82,52 @@ class AlertBatchResult:
         self.proposal_hash, self.proposal_hash2, self.proposal_len, self.announced = h1, h2, ln, ann
 
 
+class ProposalCensus:
+    """The distinct proposals announced in a VirtualCluster's last call (rapid_cd_proposal_census).
+
+    Class i is the i-th distinct (hash, hash2, length) in order of its lowest announcing receiver (representative[i]); voters[i]
+    receivers announced it.  entries(i) is its list in canonical ring-0 order (getProposal(representative[i])), statuses(i) the
+    NodeStatusChange status of each entry (DOWN: a member, UP: a registered joiner) as VIEW_CHANGE_PROPOSAL hands them out.
+    With a cut: in_cut[i] entries of the class are in it, missing[i] = |cut| - in_cut[i], extra[i] = length[i] - in_cut[i];
+    without one the three read -1.  classes() is the class of every receiver (-1: did not announce), classes_dev the same array
+    in device memory (valid until the next census of the cluster)."""
+
+    def __init__(self, cluster, n_classes, n_entries, cut_len):
+        nc, ne = int(n_classes), int(n_entries)
+        self._cluster = cluster
+        self.hash, self.hash2 = np.zeros(nc, np.uint64), np.zeros(nc, np.uint64)
+        self.length, self.voters, self.representative = (np.zeros(nc, np.int32) for _ in range(3))
+        self.in_cut = np.zeros(nc, np.int32)
+        self.list_off = np.zeros(nc + 1, np.int64)
+        self.ids, self.status = np.zeros(ne, np.int32), np.zeros(ne, np.uint8)
+        N.check(N.lib().rapid_cd_read_census(cluster._h, N.ptr(self.hash), N.ptr(self.hash2), N.ptr(self.length), N.ptr(self.voters),
+                                             N.ptr(self.representative), N.ptr(self.in_cut), N.ptr(self.list_off), N.ptr(self.ids),
+                                             N.ptr(self.status)))
+        if cut_len is None:
+            self.missing = np.full(nc, -1, np.int32)
+            self.extra = np.full(nc, -1, np.int32)
+        else:
+            self.missing = (cut_len - self.in_cut).astype(np.int32)
+            self.extra = (self.length - self.in_cut).astype(np.int32)
+        p = C.c_void_p()
+        N.check(N.lib().rapid_cd_census_classes_dev(cluster._h, C.byref(p)))
+        self.classes_dev = p.value or 0
+
+    def __len__(self):
+        return len(self.hash)
+
+    def entries(self, i):
+        return self.ids[self.list_off[i]: self.list_off[i + 1]]
+
+    def statuses(self, i):
+        return self.status[self.list_off[i]: self.list_off[i + 1]]
+
+    def classes(self):
+        out = np.zeros(self._cluster.R, np.int32)
+        N.check(N.lib().rapid_cd_read_census_classes(self._cluster._h, N.ptr(out)))
+        return out
+
+
 class VirtualCluster:
     """The cut detectors + announcedProposal flags of R virtual nodes (MembershipService.java:300-354 for each).
 
@@ -272,6 +318,16 @@ class VirtualCluster:
         if cnt.value > cap:
             return self.getProposal(receiver, cnt.value)
         return out[: cnt.value].tolist()
+
+    def proposalCensus(self, cut=None):
+        """The distinct proposals announced in the last call, counted and listed on the device -> ProposalCensus.  cut: node
+        ids to measure each proposal against (missing / extra), e.g. the decided cut."""
+        c = None if cut is None else N.as_i32(cut)
+        n = 0 if c is None else len(c)
+        buf = None if c is None else (c if n else np.zeros(1, np.int32))    # an empty cut is a cut: a non-NULL pointer
+        nc, ne = C.c_int64(0), C.c_int64(0)
+        N.check(N.lib().rapid_cd_proposal_census(self._h, N.ptr(buf), n, C.byref(nc), C.byref(ne)))
+        return ProposalCensus(self, nc.value, ne.value, None if c is None else n)
 
     def getNumProposals(self, receiver):
         out = C.c_int32(0)

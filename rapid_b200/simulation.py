@@ -59,6 +59,14 @@ ClusterSimulation rules (tests/simref.py restates them independently; DESIGN.md 
   AFTER that view change: lambda / 2K of its monitoring overlay and the bound on the error of lambda (DESIGN.md §4.13);
   initial_overlay holds the same pair for the view the simulation started with.  Both are None for a view of fewer than 3
   members, which has no such figure.
+* Proposal census (proposal_census=True; off by default, and then no record changes): every interval record with announcers
+  gains census, the distinct proposals announced in that interval (VirtualCluster.proposalCensus, counted on the device) in
+  order of their lowest announcing receiver, each {"size", "down", "up", "voters", "representative"}: its length, its
+  entries that are members (DOWN) and registered joiners (UP) as VIEW_CHANGE_PROPOSAL lists them, how many receivers announced
+  it, and the tag of the lowest of them.  Every configuration record gains census, the interval censuses merged by proposal
+  in order of first appearance, each {"size", "down", "up", "voters", "decided", "missing", "extra"}: decided marks the
+  decided cut, missing / extra count the cut's nodes the proposal lacks and the nodes it names outside the cut; and agreement,
+  the decided proposal's voters over the configuration's announcers.
 """
 import time
 
@@ -106,7 +114,7 @@ class ClusterSimulation:
     configuration, intervals one per interval."""
 
     def __init__(self, endpoints, node_ids, K=10, H=9, L=4, seed=0, failure_threshold=FAILURE_THRESHOLD, fallback_intervals=1,
-                 device=0, batch_order="sender", overlay_quality=False, wire_traffic=False):
+                 device=0, batch_order="sender", overlay_quality=False, wire_traffic=False, proposal_census=False):
         if batch_order not in ("sender", "shuffled"):
             raise ValueError("batch_order is 'sender' or 'shuffled', not %r" % (batch_order,))
         self.batch_order = batch_order
@@ -114,6 +122,7 @@ class ClusterSimulation:
         self._torch = torch
         self.K, self.H, self.L, self.seed, self.device = int(K), int(H), int(L), int(seed), device
         self.fallback_intervals = int(fallback_intervals)
+        self.proposal_census = bool(proposal_census)
         hb, off, ports = endpoints
         self.view = MembershipView.from_packed(self.K, hb, off, ports, device=device)
         self.view.setNodeIds(*node_ids)
@@ -245,6 +254,8 @@ class ClusterSimulation:
         self.votes = 0
         self.announced = 0
         self.proposal_fps = set()                                 # (h1, h2, len) of every proposal announced in the configuration
+        self.census = {}                                          # proposal_census: (h1, h2, len) -> the configuration's class
+        self._census_interval = None                              # ... and the interval of the cluster's last census
         self._ann = None                                          # announcedProposal flags, read at most once per interval
         self._dirty = True
         self._cfg_t = {"detect_ms": 0.0, "classic_ms": 0.0, "view_change_ms": 0.0, "handles_ms": 0.0, "device_ms": 0.0}
@@ -316,6 +327,8 @@ class ClusterSimulation:
                 rec["proposals"] = len(fps)
                 self.proposal_fps |= fps
                 rec["event"] = "proposals"
+                if self.proposal_census:
+                    rec["census"] = self._interval_census(i)
                 self.announced += rec["announced"]
                 if self.first_proposal is None:
                     self.first_proposal = i
@@ -395,6 +408,41 @@ class ClusterSimulation:
         if len(sizes):
             self._wire_tx += np.bincount(senders, weights=sizes.astype(np.float64) * self.N, minlength=self.N)[: self.N]
 
+    def _interval_census(self, i):
+        """the interval's census record; its classes are merged into the configuration's by fingerprint"""
+        c = self.cl.proposalCensus()
+        self._census_interval = i
+        out = []
+        for k in range(len(c)):
+            st = c.statuses(k)
+            down = int((st == N.EDGE_DOWN).sum())
+            cls = {"size": int(c.length[k]), "down": down, "up": int(len(st)) - down, "voters": int(c.voters[k])}
+            out.append(dict(cls, representative=int(self.tags[self.ring0[c.representative[k]]])))
+            fp = (int(c.hash[k]), int(c.hash2[k]), int(c.length[k]))
+            if fp in self.census:
+                self.census[fp]["voters"] += cls["voters"]
+            else:
+                self.census[fp] = dict(cls, ids=frozenset(c.entries(k).tolist()))
+        return out
+
+    def _config_census(self, cut, i):
+        """the configuration's classes against the decided cut (device ids) -> (census, agreement).  The deciding interval's
+        classes are measured by a census with cut= on the device, those of earlier intervals from their lists."""
+        cut_set = frozenset(int(x) for x in cut)
+        dist = {}
+        if self._census_interval == i:
+            d = self.cl.proposalCensus(cut=cut)
+            for k in range(len(d)):
+                dist[(int(d.hash[k]), int(d.hash2[k]), int(d.length[k]))] = (int(d.missing[k]), int(d.extra[k]))
+        out = []
+        for fp, c in self.census.items():
+            missing, extra = dist.get(fp, (len(cut_set - c["ids"]), len(c["ids"] - cut_set)))
+            out.append({"size": c["size"], "down": c["down"], "up": c["up"], "voters": c["voters"], "decided": c["ids"] == cut_set,
+                        "missing": missing, "extra": extra})
+        total = sum(c["voters"] for c in out)
+        agreement = sum(c["voters"] for c in out if c["decided"]) / total if total else None
+        return out, agreement
+
     def _announced_flags(self):
         if self._ann is None:
             self._ann = self.cl.readAnnounced()
@@ -412,6 +460,7 @@ class ClusterSimulation:
         r = self._proposer if path == "classic" else self.acc.findValue(value)
         assert r >= 0, "a decided value is some acceptor's vote"
         cut = self.cl.getProposal(r)
+        census = self._config_census(cut, i) if self.proposal_census else None
         old_tags = np.concatenate([self.tags, np.zeros(self.view.numJoiners(), np.int64)])
         for t, j in self.joiner_id.items():
             old_tags[j] = t
@@ -440,6 +489,8 @@ class ClusterSimulation:
                              "votes": votes, "members": sorted(self.tags.tolist()), "distinct_proposals": distinct, **times})
         if self.overlay_quality:
             self.history[-1]["overlay_ratio"], self.history[-1]["overlay_residual"] = self._overlay()
+        if census is not None:
+            self.history[-1]["census"], self.history[-1]["agreement"] = census
 
     # ---- whole runs --------------------------------------------------------------------------------------------------------------
     def run(self, max_intervals):
