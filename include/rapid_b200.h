@@ -424,19 +424,11 @@ int32_t rapid_pxa_phase1a(rapid_pxa* a, int64_t msg_cfg, int32_t round, int32_t 
  * vrnd != msg.rnd accept (rnd = vrnd = msg.rnd, vval = msg.vval) and broadcast Phase2bMessage.  *n_accepted = how many. */
 int32_t rapid_pxa_phase2a(rapid_pxa* a, int64_t msg_cfg, int32_t round, int32_t node_index, uint64_t hash, uint64_t hash2,
                           int32_t len, int64_t* n_accepted);
-/* Deliver the device-resident answers of the last rapid_pxa_phase1a / rapid_pxa_phase2a to a coordinator / learner,
- * in acceptor order (perm_seed == 0) or in ascending splitmix64(perm_seed ^ sender) order.  Outputs as in
- * rapid_px_phase1b / rapid_px_phase2b; trigger_index / decided_index are positions in that arrival order. */
-int32_t rapid_px_phase1b_from_acceptors(rapid_px* px, const rapid_pxa* a, uint64_t perm_seed, int32_t* proposed,
-                                        int64_t* trigger_index, uint64_t* cval_hash, uint64_t* cval_hash2,
-                                        int32_t* cval_len, int64_t* n_messages);
-int32_t rapid_px_phase2b_from_acceptors(rapid_px* px, const rapid_pxa* a, uint64_t perm_seed, int32_t* decided,
-                                        int64_t* decided_index, uint64_t* decided_hash, uint64_t* decided_hash2,
-                                        int32_t* decided_len);
-/* The same over acceptor SHARDS: the answers of the n_shards handles listed (1..64 per rank, any order) and, with comm != NULL,
- * of every other rank's shards, delivered as if one handle held the union of their acceptors: in ascending sender
- * (perm_seed == 0) or in ascending splitmix64(perm_seed ^ sender) order.  Outputs, and the state the px keeps for later
- * calls, are bit-identical to rapid_px_phase1b_from_acceptors / rapid_px_phase2b_from_acceptors on that one handle.
+/* Deliver the device-resident answers of the last rapid_pxa_phase1a / rapid_pxa_phase2a to a coordinator / learner: the
+ * answers of the n_shards acceptor handles listed (1..64 per rank, any order) and, with comm != NULL, of every other rank's
+ * shards, delivered as one handle holding the union of their acceptors would: in ascending sender (perm_seed == 0) or in
+ * ascending splitmix64(perm_seed ^ sender) order.  Outputs as in rapid_px_phase1b / rapid_px_phase2b; trigger_index /
+ * decided_index are positions in that arrival order.  One handle without a comm is read in place, without the exchange.
  * comm == NULL: this process only.  comm != NULL: a collective call; every rank calls it with its own shards and every rank
  * gets the same outputs (each holds a replica of the coordinator's / learner's tallies; O(N) bytes cross ranks: 32 B per
  * Phase1b answer, 4 B per Phase2b answer).

@@ -105,9 +105,8 @@ public final class Native {
     public static native int pxaRegisterFastRoundVotesCd(long pxa, long cd);
     public static native long pxaPhase1a(long pxa, long msgCfg, int round, int nodeIndex);            // replies or <0
     public static native long pxaPhase2a(long pxa, long msgCfg, int round, int nodeIndex, long hash, long hash2, int len);
-    public static native int pxPhase1bFromAcceptors(long px, long pxa, long permSeed, long[] out6);
-    public static native int pxPhase2bFromAcceptors(long px, long pxa, long permSeed, long[] out5);
-    /** the same over this rank's acceptor shards (and, comm != 0, every rank's: a collective call); outputs as above */
+    /** the answers of the last pxaPhase1a / pxaPhase2a of this rank's acceptor shards (and, comm != 0, every rank's: a
+     *  collective call), delivered to the tallies; one shard, comm == 0: a single handle; out6 / out5 as pxPhase1b / pxPhase2b */
     public static native int pxPhase1bFromAcceptorShards(long px, long[] pxaShards, long comm, long permSeed, long[] out6);
     public static native int pxPhase2bFromAcceptorShards(long px, long[] pxaShards, long comm, long permSeed, long[] out5);
 

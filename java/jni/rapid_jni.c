@@ -461,24 +461,6 @@ JNIEXPORT jlong JNICALL Java_com_vrg_rapid_gpu_Native_pxaPhase2a(JNIEnv* env, jc
     const int32_t rc = rapid_pxa_phase2a(H(rapid_pxa, a), cfg, round, node, (uint64_t)h1, (uint64_t)h2, len, &n);
     return rc == RAPID_OK ? (jlong)n : (jlong)rc;
 }
-JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_pxPhase1bFromAcceptors(JNIEnv* env, jclass c, jlong px, jlong a, jlong seed, jlongArray out6) {
-    int32_t proposed = 0, clen = 0;
-    int64_t trigger = -1, total = 0;
-    uint64_t ca = 0, cb = 0;
-    const int32_t rc = rapid_px_phase1b_from_acceptors(H(rapid_px, px), H(rapid_pxa, a), (uint64_t)seed, &proposed, &trigger, &ca, &cb, &clen, &total);
-    const jlong v[6] = {proposed, (jlong)trigger, (jlong)ca, (jlong)cb, clen, (jlong)total};
-    (*env)->SetLongArrayRegion(env, out6, 0, 6, v);
-    return rc;
-}
-JNIEXPORT jint JNICALL Java_com_vrg_rapid_gpu_Native_pxPhase2bFromAcceptors(JNIEnv* env, jclass c, jlong px, jlong a, jlong seed, jlongArray out5) {
-    int32_t decided = 0, dlen = 0;
-    int64_t at = -1;
-    uint64_t da = 0, db = 0;
-    const int32_t rc = rapid_px_phase2b_from_acceptors(H(rapid_px, px), H(rapid_pxa, a), (uint64_t)seed, &decided, &at, &da, &db, &dlen);
-    const jlong v[5] = {decided, (jlong)at, (jlong)da, (jlong)db, dlen};
-    (*env)->SetLongArrayRegion(env, out5, 0, 5, v);
-    return rc;
-}
 /* jlong[] of handles -> rapid_pxa* array (malloc'ed; NULL if out of memory, which the entry point refuses as a NULL list) */
 static const rapid_pxa** shard_list(JNIEnv* env, jlongArray shards, jint* n) {
     *n = (*env)->GetArrayLength(env, shards);

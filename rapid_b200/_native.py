@@ -171,8 +171,6 @@ SIGNATURES = {
     "rapid_pxa_register_fast_round_votes_cd": [_vp, _vp],
     "rapid_pxa_phase1a": [_vp, _i64, _i32, _i32, _p],
     "rapid_pxa_phase2a": [_vp, _i64, _i32, _i32, _u64, _u64, _i32, _p],
-    "rapid_px_phase1b_from_acceptors": [_vp, _vp, _u64, _p, _p, _p, _p, _p, _p],
-    "rapid_px_phase2b_from_acceptors": [_vp, _vp, _u64, _p, _p, _p, _p, _p],
     "rapid_px_phase1b_from_acceptor_shards": [_vp, _p, _i32, _vp, _u64, _p, _p, _p, _p, _p, _p],
     "rapid_px_phase2b_from_acceptor_shards": [_vp, _p, _i32, _vp, _u64, _p, _p, _p, _p, _p],
     "rapid_pxa_read": [_vp, _i64, _p, _p, _p, _p],

@@ -113,9 +113,8 @@ class Paxos:
         return self._p1_result(o)
 
     def handlePhase1bFromAcceptors(self, acceptors, perm_seed=0):
-        o = self._p1_outs()
-        N.check(N.lib().rapid_px_phase1b_from_acceptors(self._h, acceptors._h, int(perm_seed), *[C.byref(x) for x in o]))
-        return self._p1_result(o)
+        """the Phase1b answers of one PaxosAcceptors, read on the device: handlePhase1bFromAcceptorShards([acceptors])"""
+        return self.handlePhase1bFromAcceptorShards([acceptors], perm_seed=perm_seed)
 
     def handlePhase1bFromWire(self, decoder):
         """:159-191 over the Phase1bMessages of decoder's last decode (WireDecoder.decodeConsensusMessages), on the device;
@@ -147,9 +146,8 @@ class Paxos:
         return self._p2_result(o)
 
     def handlePhase2bFromAcceptors(self, acceptors, perm_seed=0):
-        o = self._p2_outs()
-        N.check(N.lib().rapid_px_phase2b_from_acceptors(self._h, acceptors._h, int(perm_seed), *[C.byref(x) for x in o]))
-        return self._p2_result(o)
+        """the Phase2b broadcasts of one PaxosAcceptors: handlePhase2bFromAcceptorShards([acceptors])"""
+        return self.handlePhase2bFromAcceptorShards([acceptors], perm_seed=perm_seed)
 
     def handlePhase2bFromWire(self, decoder):
         """:223-236 over the Phase2bMessages of decoder's last decode, on the device.  Raises RapidError(EINVAL), nothing
@@ -163,8 +161,9 @@ class Paxos:
         return (C.c_void_p * max(len(shards), 1))(*[s._h.value for s in shards])
 
     def handlePhase1bFromAcceptorShards(self, shards, comm=None, perm_seed=0):
-        """handlePhase1bFromAcceptors over the union of several PaxosAcceptors shards (any order, disjoint ranges); with an
-        NcclComm, a collective call over every rank's shards that gives every rank the same result"""
+        """:159-191 over the Phase1b answers of the last handlePhase1aMessage of several PaxosAcceptors shards (any order,
+        disjoint ranges), as one handle over their union would deliver them: in acceptor order (perm_seed == 0) or in a
+        seeded permutation; with an NcclComm, a collective call over every rank's shards that gives every rank the same result"""
         o = self._p1_outs()
         N.check(N.lib().rapid_px_phase1b_from_acceptor_shards(self._h, self._shard_handles(shards), len(shards),
                                                               None if comm is None else comm._h, int(perm_seed),
@@ -172,7 +171,8 @@ class Paxos:
         return self._p1_result(o)
 
     def handlePhase2bFromAcceptorShards(self, shards, comm=None, perm_seed=0):
-        """handlePhase2bFromAcceptors over the union of several PaxosAcceptors shards, as handlePhase1bFromAcceptorShards"""
+        """:223-236 over the Phase2b broadcasts of the last handlePhase2aMessage of several PaxosAcceptors shards, as
+        handlePhase1bFromAcceptorShards"""
         o = self._p2_outs()
         N.check(N.lib().rapid_px_phase2b_from_acceptor_shards(self._h, self._shard_handles(shards), len(shards),
                                                               None if comm is None else comm._h, int(perm_seed),

@@ -419,9 +419,9 @@ struct PX {
     RadixScratch rs;
     DevBuf<PxScal> sc;
     PinnedBuf<PxScal> h_sc;
-    // staging of host message arrays
+    // staging of host message arrays (px_stage), and the packed ranks of every message batch
     DevBuf<int64_t> s_cfg, s_rnd, s_vr;
-    DevBuf<int32_t> s_i0, s_i1, s_len, s_sender;
+    DevBuf<int32_t> s_rnd_round, s_rnd_node, s_vrnd_round, s_vrnd_node, s_len, s_sender;
     DevBuf<uint64_t> s_h1, s_h2;
     // permuted deliveries
     DevBuf<uint64_t> pkey, spkey, g_h1, g_h2;
@@ -514,6 +514,17 @@ static int32_t px_read_scal(PX* px) {
     return RAPID_OK;
 }
 
+// Runs `body` on the px's device between ev0 and ev1.  Only a call that succeeds waits for ev1 and sets what
+// rapid_px_last_device_ms reports.
+template <class F>
+static int32_t px_timed(PX* px, F&& body) {
+    DeviceGuard g(px->device);
+    RAPID_CUDA(cudaEventRecord(px->ev0, px->stream));
+    const int32_t rc = body();
+    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, px->stream); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
+    return rc;
+}
+
 // handlePhase1bMessage over device arrays (rnd == NULL: every message carries rnd_const; mcfg == NULL: cfg)
 static int32_t px_phase1b_device(PX* px, int64_t n, const int64_t* mcfg, const int64_t* rnd, int64_t rnd_const, const int64_t* vr,
                                  const uint64_t* h1, const uint64_t* h2, const int32_t* len, int32_t* proposed,
@@ -603,10 +614,59 @@ static int32_t px_phase2b_device(PX* px, int64_t n, const int64_t* mcfg, const i
     return RAPID_OK;
 }
 
+// handlePhase1bMessage / handlePhase2bMessage over a batch of messages on the device, decoded from the wire or staged from host
+// arrays: the ranks are packed, then tallied
+static int32_t px_phase1b_msgs(PX* px, const WireMsgs& m, int32_t* proposed, int64_t* trigger_index, uint64_t* ch1, uint64_t* ch2,
+                               int32_t* clen, int64_t* n_messages) {
+    cudaStream_t s = px->stream;
+    if (m.n > 0) {
+        RAPID_CHECK(px->s_rnd.reserve((size_t)m.n)); RAPID_CHECK(px->s_vr.reserve((size_t)m.n));
+        k_px_pack<<<grid_for(m.n), TB, 0, s>>>(m.n, m.rnd_round, m.rnd_node, px->s_rnd.p);
+        k_px_pack<<<grid_for(m.n), TB, 0, s>>>(m.n, m.vrnd_round, m.vrnd_node, px->s_vr.p);
+        RAPID_KERNEL_CHECK();
+    }
+    return px_phase1b_device(px, m.n, m.cfg, px->s_rnd.p, 0, px->s_vr.p, m.h1, m.h2, m.len, proposed, trigger_index, ch1, ch2, clen,
+                             n_messages);
+}
+static int32_t px_phase2b_msgs(PX* px, const WireMsgs& m, int32_t* decided, int64_t* decided_index, uint64_t* dh1, uint64_t* dh2,
+                               int32_t* dlen) {
+    if (m.n > 0) {
+        RAPID_CHECK(px->s_rnd.reserve((size_t)m.n));
+        k_px_pack<<<grid_for(m.n), TB, 0, px->stream>>>(m.n, m.rnd_round, m.rnd_node, px->s_rnd.p);
+        RAPID_KERNEL_CHECK();
+    }
+    return px_phase2b_device(px, m.n, m.cfg, px->s_rnd.p, 0, m.sender, m.h1, m.h2, m.len, 0, 0, 0, decided, decided_index, dh1, dh2,
+                             dlen);
+}
+
 template <typename T>
 static int32_t upload(DevBuf<T>& d, const T* h, int64_t n, cudaStream_t s) {
     RAPID_CHECK(d.reserve((size_t)(n > 0 ? n : 1)));
     if (n > 0) RAPID_CUDA(cudaMemcpyAsync(d.p, h, (size_t)n * sizeof(T), cudaMemcpyHostToDevice, s));
+    return RAPID_OK;
+}
+
+// n messages of host arrays uploaded into the px's staging buffers, as a WireMsgs; an array passed as NULL stays NULL
+template <typename T>
+static int32_t stage(DevBuf<T>& d, const T* h, int64_t n, cudaStream_t s, const T** out) {
+    *out = nullptr;
+    if (h) { RAPID_CHECK(upload(d, h, n, s)); *out = d.p; }
+    return RAPID_OK;
+}
+static int32_t px_stage(PX* px, int64_t n, const int64_t* cfg, const int32_t* rnd_round, const int32_t* rnd_node,
+                        const int32_t* vrnd_round, const int32_t* vrnd_node, const int32_t* sender, const uint64_t* h1,
+                        const uint64_t* h2, const int32_t* len, WireMsgs* m) {
+    *m = WireMsgs{};
+    m->device = px->device; m->n = n;
+    if (n == 0) return RAPID_OK;
+    cudaStream_t s = px->stream;
+    RAPID_CHECK(stage(px->s_cfg, cfg, n, s, &m->cfg));
+    RAPID_CHECK(stage(px->s_rnd_round, rnd_round, n, s, &m->rnd_round)); RAPID_CHECK(stage(px->s_rnd_node, rnd_node, n, s, &m->rnd_node));
+    RAPID_CHECK(stage(px->s_vrnd_round, vrnd_round, n, s, &m->vrnd_round));
+    RAPID_CHECK(stage(px->s_vrnd_node, vrnd_node, n, s, &m->vrnd_node));
+    RAPID_CHECK(stage(px->s_sender, sender, n, s, &m->sender));
+    RAPID_CHECK(stage(px->s_h1, h1, n, s, &m->h1)); RAPID_CHECK(stage(px->s_h2, h2, n, s, &m->h2));
+    RAPID_CHECK(stage(px->s_len, len, n, s, &m->len));
     return RAPID_OK;
 }
 
@@ -633,43 +693,6 @@ static int32_t px_arrival_order(PX* px, const int32_t* sender, int64_t n, uint64
     RAPID_KERNEL_CHECK();
     *order = px->sidx.p;      // NOTE: valid until the next sort on this handle; callers gather before tallying
     return RAPID_OK;
-}
-
-// handlePhase1bMessage for n compacted Phase1b answers (sender ascending) to the broadcast of `rank`, delivered in acceptor
-// order or in the perm_seed order
-static int32_t px_answers_1b(PX* px, int64_t n, int64_t rank, const int32_t* sender, const int64_t* vr, const uint64_t* h1,
-                             const uint64_t* h2, const int32_t* len, uint64_t perm_seed, int32_t* proposed, int64_t* trigger_index,
-                             uint64_t* cval_hash, uint64_t* cval_hash2, int32_t* cval_len, int64_t* n_messages) {
-    cudaStream_t s = px->stream;
-    if (n > 0) {
-        const int32_t* order = nullptr;
-        RAPID_CHECK(px_arrival_order(px, sender, n, perm_seed, &order));
-        if (order) {
-            RAPID_CHECK(px->g_vr.reserve((size_t)n)); RAPID_CHECK(px->g_h1.reserve((size_t)n));
-            RAPID_CHECK(px->g_h2.reserve((size_t)n)); RAPID_CHECK(px->g_len.reserve((size_t)n));
-            k_px_gather<int64_t><<<grid_for(n), TB, 0, s>>>(n, order, vr, px->g_vr.p);
-            k_px_gather<uint64_t><<<grid_for(n), TB, 0, s>>>(n, order, h1, px->g_h1.p);
-            k_px_gather<uint64_t><<<grid_for(n), TB, 0, s>>>(n, order, h2, px->g_h2.p);
-            k_px_gather<int32_t><<<grid_for(n), TB, 0, s>>>(n, order, len, px->g_len.p);
-            RAPID_KERNEL_CHECK();
-            vr = px->g_vr.p; h1 = px->g_h1.p; h2 = px->g_h2.p; len = px->g_len.p;
-        }
-    }
-    return px_phase1b_device(px, n, nullptr, nullptr, rank, vr, h1, h2, len, proposed, trigger_index, cval_hash, cval_hash2, cval_len,
-                             n_messages);
-}
-
-// handlePhase2bMessage for n compacted Phase2b broadcasts (sender ascending) of the value (h1, h2, len) in round `rank`
-static int32_t px_answers_2b(PX* px, int64_t n, int64_t rank, const int32_t* sender, uint64_t h1, uint64_t h2, int32_t len,
-                             uint64_t perm_seed, int32_t* decided, int64_t* decided_index, uint64_t* decided_hash,
-                             uint64_t* decided_hash2, int32_t* decided_len) {
-    if (n > 0) {
-        const int32_t* order = nullptr;
-        RAPID_CHECK(px_arrival_order(px, sender, n, perm_seed, &order));
-        if (order) sender = px->g_sender.p;
-    }
-    return px_phase2b_device(px, n, nullptr, nullptr, rank, sender, nullptr, nullptr, nullptr, h1, h2, len, decided, decided_index,
-                             decided_hash, decided_hash2, decided_len);
 }
 
 // ------------------------------------------------------------------ answers of several acceptor shards
@@ -746,10 +769,11 @@ void rapid::pxa_answers_dev(const rapid_pxa* a, PxaAnswers* out) {
 
 // Gather the pending answers of `want` kind (1 Phase1b, 2 Phase2b) of this rank's shards and, with a comm, of every rank's into
 // px->sh_* in ascending sender.  Every refusal that depends on the shards is decided from the gathered header table, which is
-// the same on every rank, so either every rank returns it or every rank goes on to the data exchange.  Outputs: the number of
-// answers, the rank of the broadcast they answer and (Phase2b) its value.
+// the same on every rank, so either every rank returns it or every rank goes on to the data exchange.  One shard without a comm
+// is already in that order and is read in place.  *out: the answers as one handle would hold them (R and begin left 0 for
+// gathered ones), with the rank of the broadcast they answer and (Phase2b) its value.
 static int32_t px_gather_shards(rapid_px* px, const rapid_pxa* const* shards, int32_t n_shards, rapid_comm* comm, int want,
-                                int64_t* n_total, int64_t* rank, uint64_t* h1, uint64_t* h2, int32_t* len) {
+                                PxaAnswers* out) {
     cudaStream_t s = px->stream;
     const int world = comm ? comm->world : 1, me = comm ? comm->rank : 0;
     if (comm && !g_nccl.AllGather) { set_error("libnccl lacks ncclAllGather"); return RAPID_ENCCL; }
@@ -810,6 +834,10 @@ static int32_t px_gather_shards(rapid_px* px, const rapid_pxa* const* shards, in
                       (long long)(all[k - 1].begin + all[k - 1].R), (long long)all[k].begin, (long long)(all[k].begin + all[k].R));
             return RAPID_EINVAL;
         }
+    if (!comm && n_shards == 1) {
+        pxa_answers_dev(shards[0], out);
+        return RAPID_OK;
+    }
     const int64_t per_rank = *std::max_element(rank_total.begin(), rank_total.end());   // padded block of every rank
     int64_t n = 0;
     for (const Ent& e : all) n += e.n_out;
@@ -869,8 +897,10 @@ static int32_t px_gather_shards(rapid_px* px, const rapid_pxa* const* shards, in
             k_px_unpack2b<<<grid_for(n), TB, 0, s>>>(n, px->seg.p, k, (const int32_t*)in, px->sh_sender.p);
         RAPID_KERNEL_CHECK();
     }
-    *n_total = n;
-    *rank = ref->last_rank; *h1 = ref->h1; *h2 = ref->h2; *len = ref->len;
+    *out = PxaAnswers{};
+    out->device = px->device; out->kind = want; out->cfg = ref->cfg; out->n = n; out->rank = ref->last_rank;
+    out->sender = px->sh_sender.p; out->vrnd = px->sh_vr.p; out->h1 = px->sh_h1.p; out->h2 = px->sh_h2.p; out->len = px->sh_len.p;
+    out->v_h1 = ref->h1; out->v_h2 = ref->h2; out->v_len = ref->len;
     return RAPID_OK;
 }
 
@@ -937,15 +967,16 @@ int32_t rapid_px_coordinator_rule(rapid_px* px, int64_t n, const int32_t* vrnd_r
     if (!px || !chosen_index) { set_error("NULL argument"); return RAPID_EINVAL; }
     if (n <= 0) { set_error("phase1bMessages was empty"); return RAPID_EINVAL; }                   // :274
     if (n > 0x7ffffff0LL || !vrnd_round || !vrnd_node || !vval_hash || !vval_len) { set_error("bad arguments"); return RAPID_EINVAL; }
+    // timed apart from px_timed: ev1 is recorded before the readback, which goes out without waiting for it
     DeviceGuard g(px->device);
     cudaStream_t s = px->stream;
     RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    RAPID_CHECK(upload(px->s_i0, vrnd_round, n, s)); RAPID_CHECK(upload(px->s_i1, vrnd_node, n, s));
+    RAPID_CHECK(upload(px->s_vrnd_round, vrnd_round, n, s)); RAPID_CHECK(upload(px->s_vrnd_node, vrnd_node, n, s));
     RAPID_CHECK(upload(px->s_h1, vval_hash, n, s)); RAPID_CHECK(upload(px->s_len, vval_len, n, s));
     RAPID_CHECK(px->s_h2.reserve((size_t)n)); RAPID_CHECK(px->s_vr.reserve((size_t)n));
     if (vval_hash2) RAPID_CUDA(cudaMemcpyAsync(px->s_h2.p, vval_hash2, (size_t)n * 8, cudaMemcpyHostToDevice, s));
     else RAPID_CUDA(cudaMemsetAsync(px->s_h2.p, 0, (size_t)n * 8, s));
-    k_px_pack<<<grid_for(n), TB, 0, s>>>(n, px->s_i0.p, px->s_i1.p, px->s_vr.p);
+    k_px_pack<<<grid_for(n), TB, 0, s>>>(n, px->s_vrnd_round.p, px->s_vrnd_node.p, px->s_vr.p);
     RAPID_KERNEL_CHECK();
     RAPID_CHECK(px_rule_device(px, n, px->s_vr.p, px->s_h1.p, px->s_h2.p, px->s_len.p));
     RAPID_CUDA(cudaEventRecord(px->ev1, s));
@@ -962,27 +993,11 @@ int32_t rapid_px_phase1b(rapid_px* px, int64_t n, const int64_t* msg_cfg, const 
                          int32_t* cval_len, int64_t* n_messages) {
     if (!px) { set_error("NULL handle"); return RAPID_EINVAL; }
     if (n < 0 || n > 0x7ffffff0LL || (n && (!rnd_round || !rnd_node || !vrnd_round || !vrnd_node || !vval_hash || !vval_len))) { set_error("bad arguments"); return RAPID_EINVAL; }
-    DeviceGuard g(px->device);
-    cudaStream_t s = px->stream;
-    RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    const int64_t* dcfg = nullptr;
-    if (n > 0) {
-        if (msg_cfg) { RAPID_CHECK(upload(px->s_cfg, msg_cfg, n, s)); dcfg = px->s_cfg.p; }
-        RAPID_CHECK(px->s_rnd.reserve((size_t)n)); RAPID_CHECK(px->s_vr.reserve((size_t)n));
-        RAPID_CHECK(upload(px->s_i0, rnd_round, n, s)); RAPID_CHECK(upload(px->s_i1, rnd_node, n, s));
-        k_px_pack<<<grid_for(n), TB, 0, s>>>(n, px->s_i0.p, px->s_i1.p, px->s_rnd.p);
-        RAPID_KERNEL_CHECK();
-        // s_i0 / s_i1 are reused for vrnd: same stream, so the copies below are ordered after the pack above
-        RAPID_CHECK(upload(px->s_i0, vrnd_round, n, s)); RAPID_CHECK(upload(px->s_i1, vrnd_node, n, s));
-        k_px_pack<<<grid_for(n), TB, 0, s>>>(n, px->s_i0.p, px->s_i1.p, px->s_vr.p);
-        RAPID_KERNEL_CHECK();
-        RAPID_CHECK(upload(px->s_h1, vval_hash, n, s)); RAPID_CHECK(upload(px->s_len, vval_len, n, s));
-        if (vval_hash2) RAPID_CHECK(upload(px->s_h2, vval_hash2, n, s));
-    }
-    const int32_t rc = px_phase1b_device(px, n, dcfg, px->s_rnd.p, 0, px->s_vr.p, px->s_h1.p, vval_hash2 ? px->s_h2.p : nullptr, px->s_len.p,
-                                         proposed, trigger_index, cval_hash, cval_hash2, cval_len, n_messages);
-    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
-    return rc;
+    return px_timed(px, [&]() -> int32_t {
+        WireMsgs m;
+        RAPID_CHECK(px_stage(px, n, msg_cfg, rnd_round, rnd_node, vrnd_round, vrnd_node, nullptr, vval_hash, vval_hash2, vval_len, &m));
+        return px_phase1b_msgs(px, m, proposed, trigger_index, cval_hash, cval_hash2, cval_len, n_messages);
+    });
 }
 
 int32_t rapid_px_phase2b(rapid_px* px, int64_t n, const int64_t* msg_cfg, const int32_t* rnd_round, const int32_t* rnd_node,
@@ -990,27 +1005,14 @@ int32_t rapid_px_phase2b(rapid_px* px, int64_t n, const int64_t* msg_cfg, const 
                          int64_t* decided_index, uint64_t* decided_hash, uint64_t* decided_hash2, int32_t* decided_len) {
     if (!px) { set_error("NULL handle"); return RAPID_EINVAL; }
     if (n < 0 || n > 0x7ffffff0LL || (n && (!rnd_round || !rnd_node || !sender || !hash || !len))) { set_error("bad arguments"); return RAPID_EINVAL; }
-    DeviceGuard g(px->device);
-    cudaStream_t s = px->stream;
-    RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    const int64_t* dcfg = nullptr;
-    if (n > 0) {
-        if (msg_cfg) { RAPID_CHECK(upload(px->s_cfg, msg_cfg, n, s)); dcfg = px->s_cfg.p; }
-        RAPID_CHECK(px->s_rnd.reserve((size_t)n));
-        RAPID_CHECK(upload(px->s_i0, rnd_round, n, s)); RAPID_CHECK(upload(px->s_i1, rnd_node, n, s));
-        k_px_pack<<<grid_for(n), TB, 0, s>>>(n, px->s_i0.p, px->s_i1.p, px->s_rnd.p);
-        RAPID_KERNEL_CHECK();
-        RAPID_CHECK(upload(px->s_sender, sender, n, s));
-        RAPID_CHECK(upload(px->s_h1, hash, n, s)); RAPID_CHECK(upload(px->s_len, len, n, s));
-        if (hash2) RAPID_CHECK(upload(px->s_h2, hash2, n, s));
-    }
-    const int32_t rc = px_phase2b_device(px, n, dcfg, px->s_rnd.p, 0, px->s_sender.p, px->s_h1.p, hash2 ? px->s_h2.p : nullptr, px->s_len.p,
-                                         0, 0, 0, decided, decided_index, decided_hash, decided_hash2, decided_len);
-    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
-    return rc;
+    return px_timed(px, [&]() -> int32_t {
+        WireMsgs m;
+        RAPID_CHECK(px_stage(px, n, msg_cfg, rnd_round, rnd_node, nullptr, nullptr, sender, hash, hash2, len, &m));
+        return px_phase2b_msgs(px, m, decided, decided_index, decided_hash, decided_hash2, decided_len);
+    });
 }
 
-// the decoded messages of a wire handle (wire_internal.cuh): ranks packed on the device, nothing uploaded
+// the decoded messages of a wire handle (wire_internal.cuh): nothing uploaded
 static int32_t px_wire_msgs(rapid_px* px, const rapid_wire* w, int32_t kind, WireMsgs* m) {
     if (!px) { set_error("NULL handle"); return RAPID_EINVAL; }
     RAPID_CHECK(wire_consensus_dev(w, kind, m));
@@ -1022,49 +1024,30 @@ int32_t rapid_px_phase1b_wire(rapid_px* px, const rapid_wire* w, int32_t* propos
                               uint64_t* cval_hash2, int32_t* cval_len, int64_t* n_messages) {
     WireMsgs m;
     RAPID_CHECK(px_wire_msgs(px, w, RAPID_WIRE_PHASE1B, &m));
-    DeviceGuard g(px->device);
-    cudaStream_t s = px->stream;
-    const int64_t n = m.n;
-    RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    if (n > 0) {
-        RAPID_CHECK(px->s_rnd.reserve((size_t)n)); RAPID_CHECK(px->s_vr.reserve((size_t)n));
-        k_px_pack<<<grid_for(n), TB, 0, s>>>(n, m.rnd_round, m.rnd_node, px->s_rnd.p);
-        k_px_pack<<<grid_for(n), TB, 0, s>>>(n, m.vrnd_round, m.vrnd_node, px->s_vr.p);
-        RAPID_KERNEL_CHECK();
-    }
-    const int32_t rc = px_phase1b_device(px, n, m.cfg, px->s_rnd.p, 0, px->s_vr.p, m.h1, m.h2, m.len, proposed, trigger_index, cval_hash,
-                                         cval_hash2, cval_len, n_messages);
-    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
-    return rc;
+    return px_timed(px, [&]() -> int32_t {
+        return px_phase1b_msgs(px, m, proposed, trigger_index, cval_hash, cval_hash2, cval_len, n_messages);
+    });
 }
 
 int32_t rapid_px_phase2b_wire(rapid_px* px, const rapid_wire* w, int32_t* decided, int64_t* decided_index, uint64_t* decided_hash,
                               uint64_t* decided_hash2, int32_t* decided_len) {
     WireMsgs m;
     RAPID_CHECK(px_wire_msgs(px, w, RAPID_WIRE_PHASE2B, &m));
-    DeviceGuard g(px->device);
-    cudaStream_t s = px->stream;
-    const int64_t n = m.n;
-    RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    if (n > 0) {
-        // a message of another configuration is dropped whatever its sender (:224); one of this configuration from an endpoint
-        // outside the dictionary refuses the call before anything changes
-        k_px2b_unknown_begin<<<1, 1, 0, s>>>(px->sc.p);
-        k_px2b_unknown<<<grid_for(n), TB, 0, s>>>(n, m.cfg, px->cfg, m.sender, px->sc.p);
-        RAPID_KERNEL_CHECK();
-        RAPID_CHECK(px_read_scal(px));
-        if (px->h_sc.p->unknown_sender != INT_MAX) {
-            set_error("Phase2bMessage %d of the current configuration comes from an endpoint outside the dictionary", px->h_sc.p->unknown_sender);
-            return RAPID_EINVAL;
+    return px_timed(px, [&]() -> int32_t {
+        if (m.n > 0) {
+            // a message of another configuration is dropped whatever its sender (:224); one of this configuration from an
+            // endpoint outside the dictionary refuses the call before anything changes
+            k_px2b_unknown_begin<<<1, 1, 0, px->stream>>>(px->sc.p);
+            k_px2b_unknown<<<grid_for(m.n), TB, 0, px->stream>>>(m.n, m.cfg, px->cfg, m.sender, px->sc.p);
+            RAPID_KERNEL_CHECK();
+            RAPID_CHECK(px_read_scal(px));
+            if (px->h_sc.p->unknown_sender != INT_MAX) {
+                set_error("Phase2bMessage %d of the current configuration comes from an endpoint outside the dictionary", px->h_sc.p->unknown_sender);
+                return RAPID_EINVAL;
+            }
         }
-        RAPID_CHECK(px->s_rnd.reserve((size_t)n));
-        k_px_pack<<<grid_for(n), TB, 0, s>>>(n, m.rnd_round, m.rnd_node, px->s_rnd.p);
-        RAPID_KERNEL_CHECK();
-    }
-    const int32_t rc = px_phase2b_device(px, n, m.cfg, px->s_rnd.p, 0, m.sender, m.h1, m.h2, m.len, 0, 0, 0, decided, decided_index,
-                                         decided_hash, decided_hash2, decided_len);
-    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
-    return rc;
+        return px_phase2b_msgs(px, m, decided, decided_index, decided_hash, decided_hash2, decided_len);
+    });
 }
 
 int32_t rapid_px_last_device_ms(const rapid_px* px, float* total_ms) {
@@ -1199,50 +1182,31 @@ int32_t rapid_pxa_phase2a(rapid_pxa* a, int64_t msg_cfg, int32_t round, int32_t 
     return RAPID_OK;
 }
 
-int32_t rapid_px_phase1b_from_acceptors(rapid_px* px, const rapid_pxa* a, uint64_t perm_seed, int32_t* proposed, int64_t* trigger_index,
-                                        uint64_t* cval_hash, uint64_t* cval_hash2, int32_t* cval_len, int64_t* n_messages) {
-    if (!px || !a) { set_error("NULL handle"); return RAPID_EINVAL; }
-    if (px->device != a->device) { set_error("px and acceptors live on different devices"); return RAPID_EINVAL; }
-    if (a->last_kind != 1) { set_error("no Phase1b answers pending (call rapid_pxa_phase1a first)"); return RAPID_EINVAL; }
-    DeviceGuard g(px->device);
-    cudaStream_t s = px->stream;
-    RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    const int32_t rc = px_answers_1b(px, a->n_out, a->last_rank, a->o_sender.p, a->o_vr.p, a->o_h1.p, a->o_h2.p, a->o_len.p, perm_seed,
-                                     proposed, trigger_index, cval_hash, cval_hash2, cval_len, n_messages);
-    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
-    return rc;
-}
-
-int32_t rapid_px_phase2b_from_acceptors(rapid_px* px, const rapid_pxa* a, uint64_t perm_seed, int32_t* decided, int64_t* decided_index,
-                                        uint64_t* decided_hash, uint64_t* decided_hash2, int32_t* decided_len) {
-    if (!px || !a) { set_error("NULL handle"); return RAPID_EINVAL; }
-    if (px->device != a->device) { set_error("px and acceptors live on different devices"); return RAPID_EINVAL; }
-    if (a->last_kind != 2) { set_error("no Phase2b broadcasts pending (call rapid_pxa_phase2a first)"); return RAPID_EINVAL; }
-    DeviceGuard g(px->device);
-    cudaStream_t s = px->stream;
-    RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    const int32_t rc = px_answers_2b(px, a->n_out, a->last_rank, a->o_sender.p, a->last_h1, a->last_h2, a->last_len, perm_seed, decided,
-                                     decided_index, decided_hash, decided_hash2, decided_len);
-    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
-    return rc;
-}
-
 int32_t rapid_px_phase1b_from_acceptor_shards(rapid_px* px, const rapid_pxa* const* shards, int32_t n_shards, rapid_comm* comm,
                                               uint64_t perm_seed, int32_t* proposed, int64_t* trigger_index, uint64_t* cval_hash,
                                               uint64_t* cval_hash2, int32_t* cval_len, int64_t* n_messages) {
     if (!px) { set_error("NULL handle"); return RAPID_EINVAL; }
     if (comm && comm->device != px->device) { set_error("comm and px live on different devices"); return RAPID_EINVAL; }
-    DeviceGuard g(px->device);
-    cudaStream_t s = px->stream;
-    RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    int64_t n = 0, rank = 0;
-    uint64_t h1 = 0, h2 = 0;
-    int32_t len = 0;
-    RAPID_CHECK(px_gather_shards(px, shards, n_shards, comm, 1, &n, &rank, &h1, &h2, &len));
-    const int32_t rc = px_answers_1b(px, n, rank, px->sh_sender.p, px->sh_vr.p, px->sh_h1.p, px->sh_h2.p, px->sh_len.p, perm_seed, proposed,
-                                     trigger_index, cval_hash, cval_hash2, cval_len, n_messages);
-    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
-    return rc;
+    return px_timed(px, [&]() -> int32_t {
+        PxaAnswers a;
+        RAPID_CHECK(px_gather_shards(px, shards, n_shards, comm, 1, &a));
+        const int32_t* order = nullptr;
+        RAPID_CHECK(px_arrival_order(px, a.sender, a.n, perm_seed, &order));
+        if (order) {
+            cudaStream_t s = px->stream;
+            const int64_t n = a.n;
+            RAPID_CHECK(px->g_vr.reserve((size_t)n)); RAPID_CHECK(px->g_h1.reserve((size_t)n));
+            RAPID_CHECK(px->g_h2.reserve((size_t)n)); RAPID_CHECK(px->g_len.reserve((size_t)n));
+            k_px_gather<int64_t><<<grid_for(n), TB, 0, s>>>(n, order, a.vrnd, px->g_vr.p);
+            k_px_gather<uint64_t><<<grid_for(n), TB, 0, s>>>(n, order, a.h1, px->g_h1.p);
+            k_px_gather<uint64_t><<<grid_for(n), TB, 0, s>>>(n, order, a.h2, px->g_h2.p);
+            k_px_gather<int32_t><<<grid_for(n), TB, 0, s>>>(n, order, a.len, px->g_len.p);
+            RAPID_KERNEL_CHECK();
+            a.vrnd = px->g_vr.p; a.h1 = px->g_h1.p; a.h2 = px->g_h2.p; a.len = px->g_len.p;
+        }
+        return px_phase1b_device(px, a.n, nullptr, nullptr, a.rank, a.vrnd, a.h1, a.h2, a.len, proposed, trigger_index, cval_hash,
+                                 cval_hash2, cval_len, n_messages);
+    });
 }
 
 int32_t rapid_px_phase2b_from_acceptor_shards(rapid_px* px, const rapid_pxa* const* shards, int32_t n_shards, rapid_comm* comm,
@@ -1250,17 +1214,14 @@ int32_t rapid_px_phase2b_from_acceptor_shards(rapid_px* px, const rapid_pxa* con
                                               uint64_t* decided_hash2, int32_t* decided_len) {
     if (!px) { set_error("NULL handle"); return RAPID_EINVAL; }
     if (comm && comm->device != px->device) { set_error("comm and px live on different devices"); return RAPID_EINVAL; }
-    DeviceGuard g(px->device);
-    cudaStream_t s = px->stream;
-    RAPID_CUDA(cudaEventRecord(px->ev0, s));
-    int64_t n = 0, rank = 0;
-    uint64_t h1 = 0, h2 = 0;
-    int32_t len = 0;
-    RAPID_CHECK(px_gather_shards(px, shards, n_shards, comm, 2, &n, &rank, &h1, &h2, &len));
-    const int32_t rc = px_answers_2b(px, n, rank, px->sh_sender.p, h1, h2, len, perm_seed, decided, decided_index, decided_hash,
-                                     decided_hash2, decided_len);
-    if (rc == RAPID_OK) { cudaEventRecord(px->ev1, s); cudaEventSynchronize(px->ev1); cudaEventElapsedTime(&px->last_ms, px->ev0, px->ev1); }
-    return rc;
+    return px_timed(px, [&]() -> int32_t {
+        PxaAnswers a;
+        RAPID_CHECK(px_gather_shards(px, shards, n_shards, comm, 2, &a));
+        const int32_t* order = nullptr;
+        RAPID_CHECK(px_arrival_order(px, a.sender, a.n, perm_seed, &order));
+        return px_phase2b_device(px, a.n, nullptr, nullptr, a.rank, order ? px->g_sender.p : a.sender, nullptr, nullptr, nullptr, a.v_h1,
+                                 a.v_h2, a.v_len, decided, decided_index, decided_hash, decided_hash2, decided_len);
+    });
 }
 
 int32_t rapid_pxa_set_silent(rapid_pxa* a, const uint8_t* silent) {

@@ -6,7 +6,9 @@
 
 namespace rapid {
 
-// Device arrays of the last consensus decode, in message order (valid until the next decode on the handle).
+// Device arrays of the last consensus decode, in message order (valid until the next decode on the handle).  The classic-Paxos
+// tallies also stage batches of host arrays in this shape; there cfg == NULL means the tallying handle's configuration and
+// h2 == NULL means 0 for every message.
 struct WireMsgs {
     int device;
     int64_t n;
