@@ -5,7 +5,10 @@ subjects left in it) sum over every subject of a chunk, and the counters of the 
 batch that moves 70,000 subjects must count 70,000 of them.  The subjects are joiners (UP alerts): no DOWN alert is ever seen,
 so no invalidation pass adds reports and the expected counts are analytic — every receiver that gets the cells has 70,000
 subjects in progress after the L batch and announces all 70,000 after the H batch.  A 16-receiver window is also run through
-the literal oracle."""
+the literal oracle.
+
+Every case runs at K = 10 (two hi bits per receiver in the rows); the default grid and the one-chunk case also run at K = 14 (a
+hi byte per receiver, 2 B per (subject, receiver))."""
 import numpy as np
 import pytest
 
@@ -13,7 +16,7 @@ from helpers import OracleWorld, fingerprints_from_oracle
 from rapid_b200 import workloads as W
 
 pytestmark = pytest.mark.gpu
-K, H, L = 10, 9, 4
+KHL = {10: (9, 4), 14: (13, 5)}       # K -> (H, L)
 N_MEMBERS = 100_000
 N_WIDE = 70_000                       # subjects moved by one batch: more than 2^16
 R, BEGIN = 1003, 40_000 + 300         # the handle: R not a multiple of 8, starting mid-tile of the ring
@@ -22,9 +25,31 @@ W0 = R - WINDOW                       # the oracle's window ends with the tile's
 DUP_CELLS = 700_000                   # one subject reported again and again: the next batch's grid estimate is 1 subject
 
 
+_WORLD = {}
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _free_worlds():
+    """the worlds (a 170,000-id view on the device, the oracle's, the cell arrays) live as long as this module's tests"""
+    yield
+    _WORLD.clear()
+
+
 @pytest.fixture(scope="module")
-def world(orc):
+def world(orc, _free_worlds):
+    return _world(orc, 10)
+
+
+def _world(orc, K):
+    """the view, its joiners and the batches at K rings, built once per K"""
+    if K not in _WORLD:
+        _WORLD[K] = _build_world(orc, K)
+    return _WORLD[K]
+
+
+def _build_world(orc, K):
     import rapid_b200 as rb
+    H, L = KHL[K]
     w = OracleWorld(orc, N_MEMBERS, K, n_joiners=N_WIDE + 1)
     v = rb.MembershipView.from_packed(K, *w.member_packed())
     v.registerJoiners(*w.joiner_endpoints())
@@ -44,7 +69,7 @@ def world(orc):
     extra = N_MEMBERS + N_WIDE                                       # the one subject of the duplicate-heavy batches
     dup = (np.full(DUP_CELLS, jobs[N_WIDE, 0], np.int32), np.full(DUP_CELLS, extra, np.int32),
            np.zeros(DUP_CELLS, np.uint8), np.full(DUP_CELLS, W.UP, np.uint8))
-    return dict(rb=rb, w=w, v=v, cfg=cfg, subjects=subjects, low=cells(range(L)), high=cells(range(L, H)), dup=dup)
+    return dict(rb=rb, w=w, v=v, K=K, H=H, L=L, cfg=cfg, subjects=subjects, low=cells(range(L)), high=cells(range(L, H)), dup=dup)
 
 
 def _bitmap(A, n_recv, base, gets):
@@ -65,9 +90,9 @@ class Case:
     def __init__(self, d, bitmap=False):
         rb = d["rb"]
         self.d, self.rb, self.bitmap = d, rb, bitmap
-        self.cl = rb.VirtualCluster(d["v"], H, L, n_receivers=R, receiver_begin=BEGIN, kernel="bucketed",
+        self.cl = rb.VirtualCluster(d["v"], d["H"], d["L"], n_receivers=R, receiver_begin=BEGIN, kernel="bucketed",
                                     max_subjects=N_WIDE + 64)
-        self.sim = d["w"].orc.ClusterSim(d["w"].view, K, H, L, WINDOW, receiver_base=BEGIN + W0)
+        self.sim = d["w"].orc.ClusterSim(d["w"].view, d["K"], d["H"], d["L"], WINDOW, receiver_base=BEGIN + W0)
         self.want = rb.proposal_fingerprint(d["subjects"])
 
     def batch(self, arrays, oracle=True):
@@ -120,15 +145,41 @@ class Case:
 
 def test_wide_batch_default_grid(world):
     """(a) 70,000 fresh subjects reach L in one batch (the batch-wide fresh totals), then all of them reach H"""
-    c = Case(world)
-    c.check_in_band(c.batch(world["low"]))
-    c.check_announced(c.batch(world["high"]))
+    _default_grid(world)
 
 
 def test_wide_batch_in_one_chunk(world):
     """(b) a duplicate-heavy batch first makes the host's estimate 1 subject, so the wide batches run in ONE subject chunk: the
     chunk record sums 70,000 fresh L-crossings, and the carried subjects of the H batch sum 70,000 H-crossings in every
     receiver's partials"""
+    _in_one_chunk(world)
+
+
+@pytest.mark.parametrize("one_chunk", [False, True])
+def test_wide_sequence_prefix(world, one_chunk):
+    """(c) one sequence call: the prefix moves 70,000 subjects into the band, the last batch moves them to H (one pass)"""
+    _sequence_prefix(world, one_chunk)
+
+
+def test_wide_batch_bitmap_delivery(world):
+    """(d) per-receiver delivery bitmaps (the generic kernel) in one subject chunk: one receiver in five gets no cell"""
+    _bitmap_delivery(world)
+
+
+@pytest.mark.parametrize("case", ["default", "one-chunk"])
+def test_wide_batches_at_fourteen_rings(orc, case):
+    """(a) and (b) at K = 14, where the rows hold a hi byte per receiver"""
+    d = _world(orc, 14)
+    {"default": _default_grid, "one-chunk": _in_one_chunk}[case](d)
+
+
+def _default_grid(world):
+    c = Case(world)
+    c.check_in_band(c.batch(world["low"]))
+    c.check_announced(c.batch(world["high"]))
+
+
+def _in_one_chunk(world):
     c = Case(world)
     c.batch(world["dup"], oracle=False)                             # (uniform delivery, seen by the handle only)
     res = c.batch(world["low"])
@@ -140,9 +191,7 @@ def test_wide_batch_in_one_chunk(world):
     c.check_announced(res)
 
 
-@pytest.mark.parametrize("one_chunk", [False, True])
-def test_wide_sequence_prefix(world, one_chunk):
-    """(c) one sequence call: the prefix moves 70,000 subjects into the band, the last batch moves them to H (one pass)"""
+def _sequence_prefix(world, one_chunk):
     rb = world["rb"]
     c = Case(world)
     if one_chunk:
@@ -166,8 +215,7 @@ def test_wide_sequence_prefix(world, one_chunk):
     assert rb.proposal_fingerprint(o_ids[o_off[0]: o_off[1]]) == c.want
 
 
-def test_wide_batch_bitmap_delivery(world):
-    """(d) per-receiver delivery bitmaps (the generic kernel) in one subject chunk: one receiver in five gets no cell"""
+def _bitmap_delivery(world):
     c = Case(world, bitmap=True)
     c.batch(world["dup"], oracle=False)                             # (uniform delivery, seen by the handle only)
     res = c.batch(world["low"])

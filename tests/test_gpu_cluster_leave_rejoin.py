@@ -231,6 +231,24 @@ def test_ten_thousand_nodes_leaves_rejoins_and_crashes(orc, rb):
     same_run(*sims)
 
 
+@pytest.mark.parametrize("K,H,L", [(3, 3, 1), (11, 10, 4), (14, 12, 5)], ids=["K3", "K11", "K14"])
+def test_leave_and_rejoin_wave_at_other_ring_counts(orc, rb, K, H, L):
+    """a wave of graceful leaves and a crash, then every one of them rejoins with a new NodeId, at other ring counts and
+    watermarks"""
+    n = 40
+    sims = make(orc, rb, n, 44, K=K, H=H, L=L)
+    gone, crashed = [3, 17, 29], [11]
+    leave(sims, gone)
+    flags(sims, crashed, CRASHED)
+    run(sims)
+    assert sorted(sims[1].members()) == [t for t in range(n) if t not in gone + crashed]
+    for j, t in enumerate(gone + crashed):
+        rejoin(sims, t, S.fresh_id(200 + j))
+    run(sims)
+    assert sorted(sims[1].members()) == list(range(n))
+    same_run(*sims)
+
+
 # ---- at scale ----------------------------------------------------------------------------------------------------------------------
 def apart(rb, n, count, seed):
     """count members, in pick_smallest order of the seed, none of which observes another"""

@@ -101,6 +101,30 @@ def test_a_stalling_draw_is_reported(orc, rb):
     same_run(ref, dev)
 
 
+# three of ClusterTest's scenarios at other ring counts and watermarks (the smallest K; K = 11 and 14, where the detector's rows hold a
+# hi byte per receiver)
+OTHER_KHL = [(3, 3, 1), (11, 10, 4), (14, 12, 5)]
+
+
+@pytest.mark.parametrize("scenario", ["one-of-five", "failures-of-fifty", "joins-and-fails"])
+@pytest.mark.parametrize("K,H,L", OTHER_KHL, ids=["K%d" % k for k, _, _ in OTHER_KHL])
+def test_scenarios_at_other_ring_counts(orc, rb, K, H, L, scenario):
+    if scenario == "one-of-five":
+        n, seed, nj, failing = 5, 1, 0, [2]
+    elif scenario == "failures-of-fifty":
+        # 12 of 50 as in ClusterTest; at K = 3 with H = 3 that many crashes leave some crashed node without enough live
+        # observers to be cut, so 6
+        n, seed, nj, failing = 50, 3, 0, random_hosts(50, 12 if K > 3 else 6, 3)
+    else:
+        n, seed, nj, failing = 30, 13, 10, list(range(2, 7))
+    ref, dev = sims = make(orc, rb, n, seed, n_joiners=nj, K=K, H=H, L=L)
+    join(sims, range(n, n + nj))
+    flags(sims, failing, CRASHED)
+    run(sims)
+    same_run(ref, dev)
+    assert sorted(dev.members()) == sorted([m for m in range(n) if m not in failing] + list(range(n, n + nj)))
+
+
 # ---- the primitives ------------------------------------------------------------------------------------------------------------
 def _view_with_joiners(rb, n, nj, K=10):
     v = rb.MembershipView.from_packed(K, *W.packed_endpoints(0, n))

@@ -125,13 +125,13 @@ def test_ctor_validation_and_bad_cells(rb, view30):        # MultiNodeCutDetecto
 KERNELS = ["sweep", "bucketed"]
 
 
-def _worlds(orc, rb, n, n_joiners=0, Hh=9, Ll=4, kernel="sweep", R=None, begin=0):
-    w = OracleWorld(orc, n, K, n_joiners=n_joiners)
-    v = rb.MembershipView.from_packed(K, *w.member_packed())
+def _worlds(orc, rb, n, n_joiners=0, Hh=9, Ll=4, kernel="sweep", R=None, begin=0, Kx=K):
+    w = OracleWorld(orc, n, Kx, n_joiners=n_joiners)
+    v = rb.MembershipView.from_packed(Kx, *w.member_packed())
     if n_joiners:
         v.registerJoiners(*w.joiner_endpoints())
     R = n if R is None else R
-    sim = orc.ClusterSim(w.view, K, Hh, Ll, R, receiver_base=begin)
+    sim = orc.ClusterSim(w.view, Kx, Hh, Ll, R, receiver_base=begin)
     cl = rb.VirtualCluster(v, Hh, Ll, n_receivers=R, receiver_begin=begin, kernel=kernel)
     return w, v, sim, cl
 
@@ -538,23 +538,38 @@ def test_fuzz_all_delivery_modes_combined(orc, rb, seed):
             cl.clear(); sim.reset()
 
 
-@pytest.mark.parametrize("seed", range(3))
-def test_fuzz_mid_scale_shards(orc, rb, seed):
+# (K, kernel, seed): the K = 10 bucketed seeds with H = 9, L = 4, then every K from 3 to 14 on both kernels with (H, L) drawn per
+# case; (K + kernel index) % 4 picks the draw, so each kernel meets (K, K), (K, 1), (1, 1) and a random pair at several K
+MID_SCALE = [(10, "bucketed", s) for s in range(3)] + \
+    [(Kx, kernel, 0) for Kx in range(3, 15) for kernel in KERNELS if (Kx, kernel) != (10, "bucketed")]
+
+
+@pytest.mark.parametrize("Kx,kernel,seed", MID_SCALE,
+                         ids=[str(s) if (Kx, k) == (10, "bucketed") else "%d-%s-K%d" % (s, k, Kx) for Kx, k, s in MID_SCALE])
+def test_fuzz_mid_scale_shards(orc, rb, Kx, kernel, seed):
     """the same fuzz at a size where a shard spans several 1024-receiver row tiles and chunks: 2,500-4,000 nodes, a
-    receiver shard that starts mid-tile, several hundred cells per batch over a few dozen subjects, every delivery mode"""
-    rng = np.random.default_rng(9000 + seed)
+    receiver shard that starts mid-tile, several hundred cells per batch over a few dozen subjects, every delivery mode (the
+    sweep kernel takes every one but per-receiver orders)"""
+    if (Kx, kernel) == (10, "bucketed"):
+        rng = np.random.default_rng(9000 + seed)
+        Hx, Lx = 9, 4
+    else:
+        ki = KERNELS.index(kernel)
+        rng = np.random.default_rng((9000, Kx, ki, seed))
+        Hx = [Kx, Kx, 1, int(rng.integers(1, Kx + 1))][(Kx + ki) % 4]
+        Lx = [Hx, 1, 1, int(rng.integers(1, Hx + 1))][(Kx + ki) % 4]
     n, nj = int(rng.integers(2500, 4000)), int(rng.integers(0, 20))
     R = int(rng.integers(1100, n))
     begin = int(rng.integers(0, n - R + 1))
-    w = OracleWorld(orc, n, K, n_joiners=nj)
-    v = rb.MembershipView.from_packed(K, *w.member_packed())
+    w = OracleWorld(orc, n, Kx, n_joiners=nj)
+    v = rb.MembershipView.from_packed(Kx, *w.member_packed())
     if nj:
         v.registerJoiners(*w.joiner_endpoints())
-    sim = orc.ClusterSim(w.view, K, 9, 4, R, receiver_base=begin)
-    cl = rb.VirtualCluster(v, 9, 4, n_receivers=R, receiver_begin=begin, kernel="bucketed")
+    sim = orc.ClusterSim(w.view, Kx, Hx, Lx, R, receiver_base=begin)
+    cl = rb.VirtualCluster(v, Hx, Lx, n_receivers=R, receiver_begin=begin, kernel=kernel)
     words = (R + 31) // 32
     for t in range(4):
-        src, dst, ring, status = random_batch(rng, n + nj, K, int(rng.integers(5, 40)), int(rng.integers(100, 500)), n)
+        src, dst, ring, status = random_batch(rng, n + nj, Kx, int(rng.integers(5, 40)), int(rng.integers(100, 500)), n)
         kw = {}
         if t != 1:
             kw["blocked"] = (rng.random(R) < 0.1).astype(np.uint8)
@@ -563,7 +578,9 @@ def test_fuzz_mid_scale_shards(orc, rb, seed):
             bm |= rng.integers(0, 2**32, size=(len(dst), words), dtype=np.uint64).astype(np.uint32)
             kw["bitmap"] = bm
         if t % 2 == 1:
-            kw["perm_seed"] = int(rng.integers(1, 2**62))
+            perm = int(rng.integers(1, 2**62))
+            if kernel == "bucketed":
+                kw["perm_seed"] = perm
         compare_batch(rb, w, sim, cl, None, (src, dst, ring, status), **kw)
 
 
@@ -611,18 +628,30 @@ def _check_sequence(rb, cl, sim, res, ain, want_in, want_len, want_ids, o_ann, c
             assert cl.debugCounters(int(r))[0] == sim.updatesInProgress(int(r))
 
 
-@pytest.mark.parametrize("kernel", KERNELS)
-@pytest.mark.parametrize("seed", range(8))
-def test_sequence_of_per_sender_batches_matches_sequential_handling(orc, rb, seed, kernel):
+# the sequence tests at other ring counts: (H, L) by seed parity, one pair with H = K; at these K the views are larger (900 to
+# 3,000 nodes), so some cases span several 1024-receiver tiles
+SEQ_K = (3, 8, 11, 14)
+SEQ_HL = {3: ((3, 1), (2, 1)), 8: ((8, 3), (7, 2)), 11: ((10, 4), (11, 5)), 14: ((13, 5), (14, 6))}
+PER_SENDER = [(10, kernel, s) for kernel in KERNELS for s in range(8)] + \
+    [(Kx, kernel, s) for Kx in SEQ_K for kernel in KERNELS for s in range(2)]
+
+
+@pytest.mark.parametrize("Kx,kernel,seed", PER_SENDER, ids=["%d-%s%s" % (s, k, "" if Kx == 10 else "-K%d" % Kx) for Kx, k, s in PER_SENDER])
+def test_sequence_of_per_sender_batches_matches_sequential_handling(orc, rb, Kx, seed, kernel):
     """the reference's AlertBatcher sends one BatchedAlertMessage per observer; a receiver handles them one by one and stops
     at the first that yields a proposal.  One rapid_cd_apply_batches call == the oracle handling the batches one by one."""
-    rng = np.random.default_rng(12000 + seed)
-    n, nj = int(rng.integers(30, 400)), int(rng.integers(0, 5))
-    Hh, Ll = (9, 4) if seed % 2 else (8, 3)
-    w, v, sim, cl = _worlds(orc, rb, n, n_joiners=nj, Hh=Hh, Ll=Ll, kernel=kernel)
+    if Kx == 10:
+        rng = np.random.default_rng(12000 + seed)
+        n, nj = int(rng.integers(30, 400)), int(rng.integers(0, 5))
+        Hh, Ll = (9, 4) if seed % 2 else (8, 3)
+    else:
+        rng = np.random.default_rng((12000, Kx, seed))
+        n, nj = int(rng.integers(900, 3000)), int(rng.integers(0, 5))
+        Hh, Ll = SEQ_HL[Kx][seed % 2]
+    w, v, sim, cl = _worlds(orc, rb, n, n_joiners=nj, Hh=Hh, Ll=Ll, kernel=kernel, Kx=Kx)
     cfg = w.view.getCurrentConfigurationId()
     for call in range(3):
-        src, dst, ring, status = random_batch(rng, n + nj, K, int(rng.integers(1, 6)), int(rng.integers(5, 120)), n)
+        src, dst, ring, status = random_batch(rng, n + nj, Kx, int(rng.integers(1, 6)), int(rng.integers(5, 120)), n)
         src, dst, ring, status, off = _per_sender(src, dst, ring, status)
         blocked = (rng.random(n) < 0.1).astype(np.uint8) if call == 1 else None
         want = _oracle_sequence(sim, cfg, src, dst, ring, status, off, n, blocked=blocked)
@@ -651,17 +680,25 @@ def test_per_sender_batches_can_differ_from_one_merged_batch(orc, rb):
     assert bk.sequenceStats() == (0, 1)
 
 
-@pytest.mark.parametrize("mode", ["uniform", "permuted"])
-@pytest.mark.parametrize("seed", range(10))
-def test_sequences_on_the_bucketed_path_fuzz(orc, rb, seed, mode):
+SEQ_FUZZ = [(10, mode, s) for s in range(10) for mode in ("uniform", "permuted")] + \
+    [(Kx, mode, s) for Kx in SEQ_K for s in range(3) for mode in ("uniform", "permuted")]
+
+
+@pytest.mark.parametrize("Kx,mode,seed", SEQ_FUZZ, ids=["%d-%s%s" % (s, m, "" if Kx == 10 else "-K%d" % Kx) for Kx, m, s in SEQ_FUZZ])
+def test_sequences_on_the_bucketed_path_fuzz(orc, rb, Kx, seed, mode):
     """rapid_cd_apply_batches on bucketed handles: random streams cut into random batches (a few long ones, many tiny ones,
     empty ones), uniform or per-receiver permuted delivery, blocked receivers, state carried from call to call — against the
     oracle handling every batch on its own.  Both outcomes of the one-pass attempt occur (served in one pass / refused and
-    replayed) and must be indistinguishable."""
-    rng = np.random.default_rng(77000 + seed)
-    n, nj = int(rng.integers(60, 1500)), int(rng.integers(0, 6))
-    Hh, Ll = (9, 4) if seed % 3 else (8, 2)
-    w, v, sim, cl = _worlds(orc, rb, n, n_joiners=nj, Hh=Hh, Ll=Ll, kernel="bucketed")
+    replayed) and must be indistinguishable; past K = 10 (a hi byte per receiver) every case takes both."""
+    if Kx == 10:
+        rng = np.random.default_rng(77000 + seed)
+        n, nj = int(rng.integers(60, 1500)), int(rng.integers(0, 6))
+        Hh, Ll = (9, 4) if seed % 3 else (8, 2)
+    else:
+        rng = np.random.default_rng((77000, Kx, seed, mode == "permuted"))
+        n, nj = int(rng.integers(900, 3000)), int(rng.integers(0, 6))
+        Hh, Ll = SEQ_HL[Kx][seed % 2]
+    w, v, sim, cl = _worlds(orc, rb, n, n_joiners=nj, Hh=Hh, Ll=Ll, kernel="bucketed", Kx=Kx)
     cfg = w.view.getCurrentConfigurationId()
     obs = w.tables()[0]
     for call in range(4):
@@ -669,13 +706,13 @@ def test_sequences_on_the_bucketed_path_fuzz(orc, rb, seed, mode):
             # crash-shaped: every observer of a few subjects reports, spread over the batches (long unstable intervals: the
             # one-pass premises usually hold)
             subj = rng.choice(n, size=int(rng.integers(2, 12)), replace=False)
-            cells = [(int(obs[s][r]), int(s), r, 1) for s in subj for r in range(K) if rng.random() < 0.95]
+            cells = [(int(obs[s][r]), int(s), r, 1) for s in subj for r in range(Kx) if rng.random() < 0.95]
             order = rng.permutation(len(cells))
             src, dst, ring, status = (np.array(x) for x in zip(*[cells[i] for i in order]))
             src, dst = src.astype(np.int32), dst.astype(np.int32)
             ring, status = ring.astype(np.uint8), status.astype(np.uint8)
         else:
-            src, dst, ring, status = random_batch(rng, n + nj, K, int(rng.integers(1, 8)), int(rng.integers(5, 150)), n)
+            src, dst, ring, status = random_batch(rng, n + nj, Kx, int(rng.integers(1, 8)), int(rng.integers(5, 150)), n)
         A = len(dst)
         nb = int(rng.integers(2, 12))
         cuts = np.sort(rng.integers(0, A + 1, size=nb - 1))
@@ -687,6 +724,22 @@ def test_sequences_on_the_bucketed_path_fuzz(orc, rb, seed, mode):
         _check_sequence(rb, cl, sim, res, ain, *want)
     one_pass, replayed = cl.sequenceStats()
     assert one_pass + replayed >= 1
+    if Kx > 10:
+        assert one_pass >= 1, cl.sequenceRefusal()                     # the random calls were served in one pass
+        # then one call the one-pass attempt must refuse: all of one crashed node's reports, then another's, one batch per cell,
+        # so the first cut is emitted before the last batch; the batch-by-batch replay gives the sequential answer
+        cl.clear(); sim.reset()
+        cells = [(int(obs[x][r]), x, r, 1) for x in (5, 17) for r in range(Kx)]
+        src, dst, ring, status = (np.array(c) for c in zip(*cells))
+        src, dst, ring, status = src.astype(np.int32), dst.astype(np.int32), ring.astype(np.uint8), status.astype(np.uint8)
+        off = np.arange(len(cells) + 1, dtype=np.int64)
+        perm = int(rng.integers(1, 2**60)) if mode == "permuted" else None
+        want = _oracle_sequence(sim, cfg, src, dst, ring, status, off, n, perm_seed=perm)
+        before = cl.sequenceStats()
+        res, ain = cl.handleBatches(cfg, src, dst, ring, status, off, perm_seed=perm)
+        _check_sequence(rb, cl, sim, res, ain, *want)
+        assert (ain >= 0).all() and (ain < len(cells) - 1).all()
+        assert cl.sequenceStats() == (before[0], before[1] + 1)        # this call was refused and replayed
 
 
 def test_sequence_stream_c4_in_one_pass(orc, rb):

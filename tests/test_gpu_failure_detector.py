@@ -16,10 +16,17 @@ def rb():
     return rapid_b200
 
 
-@pytest.mark.parametrize("seed", range(8))
-def test_every_interval_matches_the_oracle(orc, rb, seed):
+# seeds 0-7 draw K from 3..12; three more seeds fix it at the smallest ring count and at the two largest (each draws a
+# 300-node view)
+INTERVAL_CASES = [(s, None) for s in range(8)] + [(13, 3), (9, 13), (10, 14)]
+
+
+@pytest.mark.parametrize("seed,Kx", INTERVAL_CASES, ids=[str(s) if k is None else "%d-K%d" % (s, k) for s, k in INTERVAL_CASES])
+def test_every_interval_matches_the_oracle(orc, rb, seed, Kx):
     rng = np.random.default_rng(seed)
     K = int(rng.integers(3, 13))
+    if Kx is not None:
+        K = Kx
     n = int(rng.choice([2, 3, 5, 8, 40, 300]))                 # tiny views: one subject on several rings
     w = OracleWorld(orc, n, K)
     v = rb.MembershipView.from_packed(K, *w.member_packed())
@@ -98,8 +105,16 @@ def test_detectors_to_per_sender_batches_on_the_device(orc, rb):
     """the same scenario shipped the way the reference ships it: ONE BatchedAlertMessage per sender (AlertBatcher,
     MembershipService.java:613-637), handled one by one with the announcedProposal gating — as a single rapid_cd_apply_batches_dev
     call on the cells in the detectors' buffers.  Checked against the oracle handling every sender's batch on its own."""
+    _per_sender_batches_on_the_device(orc, rb, 4_000, 10, 9, 4)
+
+
+def test_detectors_to_per_sender_batches_at_fourteen_rings(orc, rb):
+    """the same at K = 14, H = 12: the detectors' cells feed the kernels whose rows hold a hi byte per receiver"""
+    _per_sender_batches_on_the_device(orc, rb, 4_000, 14, 12, 5)
+
+
+def _per_sender_batches_on_the_device(orc, rb, n, K, H, L):
     import torch
-    n, K = 4_000, 10
     w = OracleWorld(orc, n, K)
     v = rb.MembershipView.from_packed(K, *w.member_packed())
     obs, _ = v.tables()
@@ -118,12 +133,12 @@ def test_detectors_to_per_sender_batches_on_the_device(orc, rb):
     ring0 = np.asarray(v.getRing(0))
     blocked = np.ascontiguousarray(flags[ring0])
     d_blocked = torch.from_numpy(blocked).cuda()
-    cl = rb.VirtualCluster(v, 9, 4, kernel="bucketed")
+    cl = rb.VirtualCluster(v, H, L, kernel="bucketed")
     p = fd.cellsDevice()
     cl.handleBatchesDevice(cfg, nc, p[1], p[2], p[3], off, cell_cfg_dev=p[4], blocked_dev=d_blocked.data_ptr())
     res, ain = cl.readOutputs(), cl.readAnnouncedIn()
     # the oracle: every sender's batch on its own, in order
-    sim = orc.ClusterSim(w.view, K, 9, 4, n)
+    sim = orc.ClusterSim(w.view, K, H, L, n)
     want_in, want_len = np.full(n, -1, np.int32), np.zeros(n, np.int32)
     for i in range(len(off) - 1):
         sl = slice(int(off[i]), int(off[i + 1]))

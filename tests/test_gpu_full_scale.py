@@ -12,9 +12,9 @@ pytestmark = pytest.mark.gpu
 K, H, L = 10, 9, 4
 
 
-def _view(rb, n, nj=0):
+def _view(rb, n, nj=0, Kx=K):
     hb, off, ports = W.packed_endpoints(0, n + nj)
-    v = rb.MembershipView.from_packed(K, hb[: off[n]], off[: n + 1], ports[:n])
+    v = rb.MembershipView.from_packed(Kx, hb[: off[n]], off[: n + 1], ports[:n])
     if nj:
         hosts, jports = W.endpoints(n, nj)
         v.registerJoiners(hosts, jports)
@@ -24,20 +24,20 @@ def _view(rb, n, nj=0):
 SAMPLE = 256
 
 
-def _oracle_view(orc, n, nj=0):
+def _oracle_view(orc, n, nj=0, Kx=K):
     hb, off, ports = W.packed_endpoints(0, n + nj)
     u = orc.Universe()
     tags = u.add_bulk(hb, off, ports)
     hi, lo = W.node_ids(0, n)
-    return u, orc.MembershipView(u, K, tags[:n], hi, lo)
+    return u, orc.MembershipView(u, Kx, tags[:n], hi, lo)
 
 
-def _sampled_oracle_check(orc, rb, oview, cl, res, window_begin, batch, cfg, blocked, perm_seed=None, sim=None):
+def _sampled_oracle_check(orc, rb, oview, cl, res, window_begin, batch, cfg, blocked, perm_seed=None, sim=None, khl=(K, H, L)):
     """Per-receiver parity AT FULL SCALE: a window of SAMPLE receivers is run through the literal oracle on the same batch and
     compared receiver by receiver (length, both fingerprint words, announced flag, canonical list of one announcer, report
     masks + updatesInProgress of a few receivers that have not announced)."""
     if sim is None:
-        sim = orc.ClusterSim(oview, K, H, L, SAMPLE, receiver_base=cl.receiver_begin + window_begin)
+        sim = orc.ClusterSim(oview, *khl, SAMPLE, receiver_base=cl.receiver_begin + window_begin)
     o_len, o_ann, o_ids, o_off = sim.apply_batch(batch.src, batch.dst, batch.ring, batch.status, np.full(len(batch), cfg, np.int64),
                                                  blocked=blocked[window_begin: window_begin + SAMPLE], perm_seed=perm_seed, threads=8)
     sl = slice(window_begin, window_begin + SAMPLE)
@@ -80,25 +80,25 @@ def _check_converged(rb, v, cl, b, cfg, blocked, perm_seed=None):
     return res, want
 
 
-def test_c5_one_million_nodes(orc):
-    import rapid_b200 as rb
-    n = 1_000_000
+def _c5(orc, rb, n, khl, windows):
+    """the C5 batch (n / 200 crashes, n / 200 joins) over n receivers: converged, the uniform kernel, per-receiver oracle parity on
+    the windows, and the fast round's decision -> (view, batch, cfg, blocked, outputs)"""
+    Kx, Hx, Lx = khl
     nj = n // 200
-    v = _view(rb, n, nj)
+    v = _view(rb, n, nj, Kx)
     obs, _ = v.tables()
     b = W.c5_churn(obs, v.joinerTables(), n, n // 200, nj)
     hi, lo = W.node_ids(0, n)
     cfg = v.getCurrentConfigurationId(hi, lo)
     ring0 = v.getRing(0)
     blocked = W.blocked_by_receiver(b.blocked, ring0, 0, n)
-    cl = rb.VirtualCluster(v, H, L, max_subjects=len(b.expected_cut) + 64)
+    cl = rb.VirtualCluster(v, Hx, Lx, max_subjects=len(b.expected_cut) + 64)
     res, want = _check_converged(rb, v, cl, b, cfg, blocked)
     assert cl.lastPath()[0] == 2                                   # the subject-bucketed uniform kernel served it
-    # per-receiver oracle parity on two windows of the million receivers (one of them straddling a 1024-receiver tile edge)
-    _, oview = _oracle_view(orc, n, nj)
+    _, oview = _oracle_view(orc, n, nj, Kx)
     assert oview.getCurrentConfigurationId() == cfg
-    for w0 in (1024 * 300 - 100, 987_654):
-        _sampled_oracle_check(orc, rb, oview, cl, res, w0, b, cfg, blocked)
+    for w0 in windows:
+        _sampled_oracle_check(orc, rb, oview, cl, res, w0, b, cfg, blocked, khl=khl)
     # fast round: the decision is that cut, taken at the quorum-th vote
     cl.clear()
     cl.handleBatch(cfg, None, b.dst, b.ring, b.status, blocked=blocked, read_outputs=False)
@@ -107,12 +107,28 @@ def test_c5_one_million_nodes(orc):
     assert t.decided and (t.hash, t.hash2, t.length) == (want[0], want[1], len(b.expected_cut))
     assert t.count == rb.quorum(n) == t.votes_received
     del cl
+    return v, b, cfg, blocked, res
+
+
+def test_c5_one_million_nodes(orc):
+    import rapid_b200 as rb
+    n = 1_000_000
+    # per-receiver oracle parity on two windows of the million receivers (one of them straddling a 1024-receiver tile edge)
+    v, b, cfg, blocked, res = _c5(orc, rb, n, (K, H, L), (1024 * 300 - 100, 987_654))
     # the per-cell sweep kernel on a slice of the receivers agrees bit for bit
     lo_r, cnt = 123_456, 4096
     sw = rb.VirtualCluster(v, H, L, n_receivers=cnt, receiver_begin=lo_r, kernel="sweep", max_subjects=len(b.expected_cut) + 64)
     r2 = sw.handleBatch(cfg, None, b.dst, b.ring, b.status, blocked=blocked[lo_r: lo_r + cnt])
     assert (r2.proposal_hash == res.proposal_hash[lo_r: lo_r + cnt]).all()
     assert (r2.proposal_len == res.proposal_len[lo_r: lo_r + cnt]).all()
+
+
+@pytest.mark.parametrize("n,khl", [(100_000, (11, 11, 4)), (150_000, (14, 12, 5))], ids=["K11", "K14"])
+def test_c5_past_ten_rings(orc, n, khl):
+    """the C5 shape where the rows hold a hi byte per receiver (K > 10, 2 B per (subject, receiver)): windows across a tile edge
+    and at the end of the receivers, the same final tally"""
+    import rapid_b200 as rb
+    _c5(orc, rb, n, khl, (1024 * 60 - 100, n - SAMPLE))
 
 
 def test_c3_ten_thousand_nodes_correlated_partition(orc):

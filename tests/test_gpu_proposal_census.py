@@ -23,12 +23,31 @@ def rb():
     return rapid_b200
 
 
+@pytest.fixture(scope="module", autouse=True)
+def _free_worlds():
+    """the views live as long as this module's tests"""
+    yield
+    _WORLD.clear()
+
+
 @pytest.fixture(scope="module")
-def world(orc, rb):
-    w = OracleWorld(orc, N, K, n_joiners=8)
-    v = rb.MembershipView.from_packed(K, *w.member_packed())
-    v.registerJoiners(*w.joiner_endpoints())
-    return dict(w=w, v=v, cfg=w.view.getCurrentConfigurationId(), obs=w.tables()[0], ring0=w.ring0(), jobs=v.joinerTables())
+def world(orc, rb, _free_worlds):
+    return _world(orc, rb, K, H, L)
+
+
+# the census at other ring counts, each with H = K: the smallest K and the largest (a hi byte per receiver in the rows)
+OTHER_KHL = [(3, 3, 1), (14, 14, 6)]
+_WORLD = {}
+
+
+def _world(orc, rb, Kx, Hx, Lx):
+    if Kx not in _WORLD:
+        w = OracleWorld(orc, N, Kx, n_joiners=8)
+        v = rb.MembershipView.from_packed(Kx, *w.member_packed())
+        v.registerJoiners(*w.joiner_endpoints())
+        _WORLD[Kx] = dict(w=w, v=v, K=Kx, H=Hx, L=Lx, cfg=w.view.getCurrentConfigurationId(), obs=w.tables()[0], ring0=w.ring0(),
+                          jobs=v.joinerTables())
+    return _WORLD[Kx]
 
 
 def per_sender(src, dst, ring, status):
@@ -84,7 +103,7 @@ def check(rb, cl, props, cut=None, n_members=None):
 def oracle_sender(world, orc, seq, blocked, seed, R=N, base=0):
     """per-sender batches through the oracle's handlers, batch b with cell order seed + b -> per-receiver proposals of the call"""
     src, dst, ring, st, off = seq
-    sim = orc.ClusterSim(world["w"].view, K, H, L, R, receiver_base=base)
+    sim = orc.ClusterSim(world["w"].view, world["K"], world["H"], world["L"], R, receiver_base=base)
     props = [None] * R
     for b in range(len(off) - 1):
         sl = slice(off[b], off[b + 1])
@@ -102,8 +121,12 @@ def c2(world, frac=0.01, seed=W.SEED):
 
 # ---- against the oracle --------------------------------------------------------------------------------------------------------------
 def test_bucketed_sender_batches_one_call(orc, rb, world):
+    _sender_batches_one_call(orc, rb, world)
+
+
+def _sender_batches_one_call(orc, rb, world):
     seq, blocked = c2(world)
-    cl = rb.VirtualCluster(world["v"], H, L, kernel="bucketed")
+    cl = rb.VirtualCluster(world["v"], world["H"], world["L"], kernel="bucketed")
     cl.handleBatches(world["cfg"], *seq, blocked=blocked, perm_seed=41, read_outputs=False)
     c = check(rb, cl, oracle_sender(world, orc, seq, blocked, 41))
     assert len(c) >= 1 and c.voters.sum() > N // 2
@@ -128,11 +151,15 @@ def test_bucketed_one_batch_per_call(orc, rb, world):
 
 
 def test_joins_and_crashes_with_blocked_receivers(orc, rb, world):
+    _joins_and_crashes(orc, rb, world)
+
+
+def _joins_and_crashes(orc, rb, world):
     b = W.c5_churn(world["obs"], world["jobs"], N, 6, 8, seed=11)
     blocked = W.blocked_by_receiver(b.blocked, world["ring0"], 0, N)
     assert blocked.any()
     seq = per_sender(b.src, b.dst, b.ring, b.status)
-    cl = rb.VirtualCluster(world["v"], H, L, kernel="bucketed")
+    cl = rb.VirtualCluster(world["v"], world["H"], world["L"], kernel="bucketed")
     cl.handleBatches(world["cfg"], *seq, blocked=blocked, perm_seed=3, read_outputs=False)
     c = check(rb, cl, oracle_sender(world, orc, seq, blocked, 3))
     assert (c.status == 0).any() and (c.status == 1).any()                      # UP (joiners) and DOWN entries
@@ -158,13 +185,26 @@ def test_shuffled_c2_many_proposals(orc, rb, world):
 
 
 def test_shard_second_call_and_clear(orc, rb, world):
+    _shard_second_call_and_clear(orc, rb, world)
+
+
+@pytest.mark.parametrize("case", ["sender-batches", "joins-and-crashes", "shard"])
+@pytest.mark.parametrize("Kx,Hx,Lx", OTHER_KHL, ids=["K%d" % k for k, _, _ in OTHER_KHL])
+def test_census_at_other_ring_counts(orc, rb, Kx, Hx, Lx, case):
+    """the sender-batches call, joins and crashes with blocked receivers, and the shard's two calls at K = 3 and K = 14"""
+    world = _world(orc, rb, Kx, Hx, Lx)
+    {"sender-batches": _sender_batches_one_call, "joins-and-crashes": _joins_and_crashes,
+     "shard": _shard_second_call_and_clear}[case](orc, rb, world)
+
+
+def _shard_second_call_and_clear(orc, rb, world):
     (src, dst, ring, st, off), blocked = c2(world, 0.005, seed=5)
     half = len(off) // 2
     first = (src[: off[half]], dst[: off[half]], ring[: off[half]], st[: off[half]], off[: half + 1])
     second = (src[off[half]:], dst[off[half]:], ring[off[half]:], st[off[half]:], off[half:] - off[half])
     base, R = 700, 500
-    cl = rb.VirtualCluster(world["v"], H, L, n_receivers=R, receiver_begin=base, kernel="sweep")
-    sim = orc.ClusterSim(world["w"].view, K, H, L, R, receiver_base=base)
+    cl = rb.VirtualCluster(world["v"], world["H"], world["L"], n_receivers=R, receiver_begin=base, kernel="sweep")
+    sim = orc.ClusterSim(world["w"].view, world["K"], world["H"], world["L"], R, receiver_base=base)
     bl = blocked[base: base + R]
     announced = 0
     for i, part in enumerate((first, second)):

@@ -23,10 +23,14 @@ def rb():
 
 
 # ---------------------------------------------------------------- the reference itself, against the oracle (CPU) ------------------
-@pytest.mark.parametrize("seed", range(16))
-def test_plain_view_change_matches_oracle(orc, seed):
+# seeds 0-15 draw K from {3, 7, 10}; seeds 16-17 fix it at the largest ring count
+@pytest.mark.parametrize("seed,K14", [(s, False) for s in range(16)] + [(16, True), (17, True)],
+                         ids=[str(s) for s in range(16)] + ["16-K14", "17-K14"])
+def test_plain_view_change_matches_oracle(orc, seed, K14):
     rng = np.random.default_rng(900 + seed)
     Kx = int(rng.choice([3, 7, 10]))
+    if K14:
+        Kx = 14
     n = int(rng.integers(0, 60))
     nj = int(rng.integers(0, 20))
     w = OracleWorld(orc, n, Kx, n_joiners=nj)
@@ -70,11 +74,11 @@ class Tracked:
     """A device view plus what the tests know about it: the endpoint (index into a pool of synthetic endpoints) and NodeId of
     every id, and identifiersSeen."""
 
-    def __init__(self, rb, n, pool):
-        self.rb = rb
+    def __init__(self, rb, n, pool, K=K):
+        self.rb, self.K = rb, K
         self.hb, self.off, self.ports = W.packed_endpoints(0, pool)
         self.pool_hi, self.pool_lo = W.node_ids(0, pool)
-        self.v = rb.MembershipView.from_packed(K, *self.packed(np.arange(n)))
+        self.v = rb.MembershipView.from_packed(self.K, *self.packed(np.arange(n)))
         self.ep = np.arange(n)
         self.hi, self.lo = self.pool_hi[:n].copy(), self.pool_lo[:n].copy()
         self.v.setNodeIds(self.hi, self.lo)
@@ -112,8 +116,8 @@ class Tracked:
         """everything a refused cut must leave as it was"""
         v = self.v
         obs, subj = v.tables()
-        return (v.getMembershipSize(), v.numJoiners(), [v.getRing(k).tolist() for k in range(K)],
-                [v.keys(k).tolist() for k in range(K)], obs.tolist(), subj.tolist(), v.joinerTables().tolist(),
+        return (v.getMembershipSize(), v.numJoiners(), [v.getRing(k).tolist() for k in range(self.K)],
+                [v.keys(k).tolist() for k in range(self.K)], obs.tolist(), subj.tolist(), v.joinerTables().tolist(),
                 v.currentConfigurationId())
 
     def refused(self, cut, exc):
@@ -124,7 +128,7 @@ class Tracked:
 
     def apply(self, cut):
         """apply `cut` on the device and compare the result with both references"""
-        v = self.v
+        v, K = self.v, self.K
         n = v.getMembershipSize()
         assert n + v.numJoiners() == len(self.ep)
         keys = np.stack([v.keys(k) for k in range(K)]) if len(self.ep) else np.zeros((K, 0), np.int64)
@@ -168,6 +172,18 @@ def test_cut_admits_m_joiners(rb, members, m):
     ref = t.apply(rng.permutation(np.concatenate([leave, join])))
     assert int((ref.kept >= members).sum()) == m            # m > RANK_LIMIT: the joiners were ranked by the radix sorts
     assert len(ref.kept) == members - members // 100 + m
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("m", [100, RANK_LIMIT + 1])
+def test_cut_at_fourteen_rings(rb, m):
+    """the same cut at K = 14 on both sides of the rank / radix edge: 1 % of 5,000 members leave, m joiners come in"""
+    rng = np.random.default_rng(14 + m)
+    t = Tracked(rb, 5000, 5000 + m + 3, K=14)
+    jids = t.register(t.fresh_endpoints(m + 3))
+    join = np.sort(rng.choice(jids, size=m, replace=False))
+    ref = t.apply(rng.permutation(np.concatenate([rng.choice(5000, size=50, replace=False), join])))
+    assert int((ref.kept >= 5000).sum()) == m and len(ref.kept) == 5000 - 50 + m
 
 
 @pytest.mark.gpu

@@ -61,10 +61,15 @@ def set_msg(field, value):
     field.MergeFrom(value)
 
 
+# (H, L) of the detectors whose votes are encoded, by ring count
+HL = {3: (3, 1), 10: (9, 4), 14: (12, 5)}
+
+
 class Cluster:
-    def __init__(self, rb, n, n_joiners, seed):
+    def __init__(self, rb, n, n_joiners, seed, K=K):
         hosts, ports = endpoints(n + n_joiners, seed)
         self.hosts, self.ports = hosts, ports
+        self.K, (self.H, self.L) = K, HL[K]
         self.view = rb.MembershipView(K, hosts[:n], ports[:n])
         self.hi, self.lo = node_ids(0, n + n_joiners)
         self.view.setNodeIds(self.hi[:n], self.lo[:n])
@@ -121,16 +126,28 @@ def wrap(pb, case, msg):
     return r
 
 
-@pytest.mark.parametrize("seed,as_request,tick_cfg,merge_cfg", [(0, False, 0, 0), (1, True, -5, -5), (2, False, 7, -(1 << 62)),
-                                                                 (3, True, 1 << 40, 3)])
-def test_alert_batches_are_byte_identical_and_decode_back(rb, pb, seed, as_request, tick_cfg, merge_cfg):
-    c = Cluster(rb, [60, 400, 2000, 300][seed], 4, seed)
-    fd = interval(rb, c, seed, 0.05, tick_cfg, merge_cfg, n_leavers=3)
+def _ids(cases):
+    """the ids pytest gives the cases at K = 10, with the ring count appended at the others"""
+    return ["-".join(str(x) for x in c[:-1]) + ("" if c[-1] == K else "-K%d" % c[-1]) for c in cases]
+
+
+# K = 3 and 14; seed 4 is a two-member view at K = 14, where the live member observes the crashed one on every ring and its
+# DOWN alert lists all 14 ring numbers
+ALERT_CASES = [(0, False, 0, 0, K), (1, True, -5, -5, K), (2, False, 7, -(1 << 62), K), (3, True, 1 << 40, 3, K),
+               (0, False, 0, 0, 3), (1, True, -5, -5, 3), (0, False, 0, 0, 14), (1, True, -5, -5, 14), (4, False, 9, 9, 14)]
+
+
+@pytest.mark.parametrize("seed,as_request,tick_cfg,merge_cfg,Kx", ALERT_CASES, ids=_ids(ALERT_CASES))
+def test_alert_batches_are_byte_identical_and_decode_back(rb, pb, seed, as_request, tick_cfg, merge_cfg, Kx):
+    c = Cluster(rb, [60, 400, 2000, 300, 2][seed], 4, seed, Kx)
+    fd = interval(rb, c, seed, 0.05, tick_cfg, merge_cfg, n_leavers=3 if c.n > 2 else 0)
     dec = rb.WireDecoder(c.view)
     enc = dec.encodeAlertBatches(fd, as_request=as_request)
     want = expected_batches(pb, c, fd)
     assert len(enc) == len(want) > 0
     assert any(m.edgeStatus == 0 for _, b in want for m in b.messages)          # join alerts present
+    if seed == 4:
+        assert max(len(m.ringNumber) for _, b in want for m in b.messages) == Kx     # one alert lists every ring
     assert (enc.body_ids == -1).all() and len(enc.body_off) == 1
     for i, (_, b) in enumerate(want):
         w = wrap(pb, "batchedAlertMessage", b) if as_request else b
@@ -151,7 +168,7 @@ def run_votes(rb, c, seed, split):
     receivers, so receivers announce different subsets of the crashed nodes"""
     fd = interval(rb, c, seed, 0.04, 11, 11, n_leavers=0)
     src, dst, ring, status, cfg = fd.cells()
-    vc = rb.VirtualCluster(c.view, 9, 4, kernel="sweep" if split else "auto")
+    vc = rb.VirtualCluster(c.view, c.H, c.L, kernel="sweep" if split else "auto")
     bitmap = None
     if split:
         rng = np.random.default_rng(seed)
@@ -163,10 +180,13 @@ def run_votes(rb, c, seed, split):
     return vc, res
 
 
-@pytest.mark.parametrize("seed,as_request,cfg,split", [(0, False, 11, False), (1, True, -3, False), (2, False, 0, True),
-                                                       (3, True, 1 << 50, True)])
-def test_votes_are_byte_identical_share_bodies_and_decode_back(rb, pb, seed, as_request, cfg, split):
-    c = Cluster(rb, [300, 1000, 200, 500][seed], 0, seed)
+VOTE_CASES = [(0, False, 11, False, K), (1, True, -3, False, K), (2, False, 0, True, K), (3, True, 1 << 50, True, K),
+              (0, False, 11, False, 3), (2, False, 0, True, 3), (1, True, -3, False, 14), (3, True, 1 << 50, True, 14)]
+
+
+@pytest.mark.parametrize("seed,as_request,cfg,split,Kx", VOTE_CASES, ids=_ids(VOTE_CASES))
+def test_votes_are_byte_identical_share_bodies_and_decode_back(rb, pb, seed, as_request, cfg, split, Kx):
+    c = Cluster(rb, [300, 1000, 200, 500][seed], 0, seed, Kx)
     vc, res = run_votes(rb, c, seed, split)
     voters = np.nonzero(res.proposal_len > 0)[0]
     assert len(voters) > 0
