@@ -2,8 +2,8 @@
 // its voters, its lowest receiver, its list in canonical ring-0 order with a status per entry (VIEW_CHANGE_PROPOSAL's
 // NodeStatusChange list, MembershipService.java:336-345, :586-593) and, given a cut, how many of its entries the cut holds.
 //
-//   claim     one thread per receiver: every announcer inserts its (h1, h2, len) into an open-addressing table (fp_table_claim,
-//             the wire encoder's scheme); a slot keeps the lowest receiver and counts its voters
+//   claim     one thread per receiver: every announcer inserts its (h1, h2, len) into an open-addressing table (fp_table_claim);
+//             a slot keeps the lowest receiver and counts its voters
 //   classes   representatives (the lowest receiver of a fingerprint) marked and scanned: class c is the c-th representative in
 //             receiver order; cls[r] = class of receiver r, -1 if r did not announce; list offsets are the scan of the
 //             representatives' lengths
@@ -12,9 +12,11 @@
 //             ring-0 key, by class — give every list get_proposal's order
 //   status    DOWN for a member id, UP for a registered joiner (createNodeStatusChangeList :586-593)
 //   in_cut    one block per class counts its entries in a device bitmap of the cut
-// One host synchronisation per census: the class and entry counts the caller gets back, which also size the sorts.  The lists
-// are enqueued after it on the handle's stream; the reads wait for them.  Outputs are double-buffered: a census writes the spare
-// set and swaps on success, so a refused or failed census leaves the previous one as it was.
+// Claim and classes (group_proposals) and the lists (list_proposals) are also the wire encoder's (wire_encode.cu): it groups its
+// votes' and answers' lists with them, in storage of its own.  One host synchronisation per census: the class and entry counts
+// the caller gets back, which also size the per-class arrays and the sorts.  The lists are enqueued after it on the handle's
+// stream; the reads wait for them.  Outputs are double-buffered: a census writes the spare set and swaps on success, so a
+// refused or failed census leaves the previous one as it was.
 #include <algorithm>
 #include <vector>
 
@@ -23,11 +25,6 @@
 #include "scan.cuh"
 
 namespace rapid {
-
-struct CensusScal {
-    int32_t n_ann, n_classes, n_entries, T;
-    unsigned long long entries64;      // the representatives' lengths summed in 64 bits (the int32 scan must not wrap)
-};
 
 struct CensusOut {
     bool valid = false;
@@ -43,18 +40,19 @@ struct CensusOut {
 struct Census {
     CensusOut out[2];
     int cur = 0;                       // out[cur] holds the last census
-    DevBuf<int32_t> table, tcnt;       // [T cap] open-addressing table: lowest receiver, voters
-    DevBuf<int32_t> slot, rep, rpos, loff, scan_sums;                 // [R]
-    DevBuf<uint64_t> c_h1, c_h2;                                      // [R] per class (n_classes <= announcers <= R)
-    DevBuf<int32_t> c_rep, c_len, c_voters, c_off, c_rule, c_fill;
+    ProposalGroups g;
+    DevBuf<int32_t> cut_ids;
+    DevBuf<uint32_t> cut_bits;
+};
+
+// the lists stage's scratch: per entry, and the sorts'
+struct ListScratch {
     DevBuf<int32_t> e_id, e_cls, idx, k32, k32s, perm;                // [n_entries]
     DevBuf<uint64_t> e_key, k64, k64s;
     RadixScratch rs;
-    DevBuf<int32_t> cut_ids;
-    DevBuf<uint32_t> cut_bits;
-    DevBuf<CensusScal> sc;
-    PinnedBuf<CensusScal> h_sc;
 };
+
+ProposalGroups::~ProposalGroups() { delete ls; }
 
 void census_destroy(CD* cd) {
     delete cd->census;
@@ -67,92 +65,87 @@ constexpr int CEN_TABLE_MIN = 1024;
 constexpr uint64_t KEY_SIGN = 0x8000000000000000ULL;   // signed ring-0 key -> unsigned order
 
 // ------------------------------------------------------------------ claim and classes
-__global__ void k_cen_count(int64_t R, const uint32_t* __restrict__ rflags, CensusScal* __restrict__ sc) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool ann = r < R && (rflags[r] & RF_ANN_NOW);
-    const unsigned b = __ballot_sync(0xffffffffu, ann);
-    if ((threadIdx.x & 31) == 0 && b) atomicAdd(&sc->n_ann, __popc(b));
+template <typename Src>
+__global__ void k_cen_count(int64_t n, Src src, GroupScal* __restrict__ sc) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool part = i < n && src.part((int32_t)i);
+    const unsigned b = __ballot_sync(0xffffffffu, part);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(&sc->n_part, __popc(b));
 }
 
-// T = the smallest power of two >= 2 x announcers (at least CEN_TABLE_MIN), chosen on the device; grid-stride fill of T slots
-__global__ void k_cen_table_init(CensusScal* __restrict__ sc, int32_t* __restrict__ table, int32_t* __restrict__ tcnt) {
+// T = the smallest power of two >= 2 x items taking part (at least CEN_TABLE_MIN), chosen on the device; grid-stride fill of T slots
+__global__ void k_cen_table_init(GroupScal* __restrict__ sc, int32_t* __restrict__ table, int32_t* __restrict__ tcnt) {
     uint32_t T = CEN_TABLE_MIN;
-    while ((int64_t)T < 2 * (int64_t)sc->n_ann) T <<= 1;
+    while ((int64_t)T < 2 * (int64_t)sc->n_part) T <<= 1;
     if (blockIdx.x == 0 && threadIdx.x == 0) sc->T = (int32_t)T;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < T; i += gridDim.x * blockDim.x) { table[i] = -1; tcnt[i] = 0; }
 }
 
-struct OutFp {
-    const uint64_t* h1;
-    const uint64_t* h2;
-    const int32_t* len;
-    __device__ __forceinline__ void operator()(int32_t i, uint64_t* a, uint64_t* b, int32_t* l) const { *a = h1[i]; *b = h2[i]; *l = len[i]; }
-};
-
-__global__ void k_cen_claim(int64_t R, const uint32_t* __restrict__ rflags, OutFp fp, const CensusScal* __restrict__ sc,
-                            int32_t* __restrict__ table, int32_t* __restrict__ tcnt, int32_t* __restrict__ slot) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= R) return;
-    if (!(rflags[r] & RF_ANN_NOW)) { slot[r] = -1; return; }
+template <typename Src>
+__global__ void k_cen_claim(int64_t n, Src src, const GroupScal* __restrict__ sc, int32_t* __restrict__ table,
+                            int32_t* __restrict__ tcnt, int32_t* __restrict__ slot) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (!src.part((int32_t)i)) { slot[i] = -1; return; }
     uint64_t a, b; int32_t l;
-    fp((int32_t)r, &a, &b, &l);
-    const uint32_t pos = fp_table_claim(table, (uint32_t)sc->T, (int32_t)r, a, b, l, fp);
+    src((int32_t)i, &a, &b, &l);
+    const uint32_t pos = fp_table_claim(table, (uint32_t)sc->T, (int32_t)i, a, b, l, src);
     atomicAdd(&tcnt[pos], 1);
-    slot[r] = (int32_t)pos;
+    slot[i] = (int32_t)pos;
 }
 
-// rep[r]: r is its fingerprint's lowest receiver; loff[r]: its list length if so (scanned into list offsets)
-__global__ void k_cen_rep(int64_t R, const int32_t* __restrict__ slot, const int32_t* __restrict__ table, const int32_t* __restrict__ len,
-                          int32_t* __restrict__ rep, int32_t* __restrict__ loff, CensusScal* __restrict__ sc) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= R) return;
-    const bool is = slot[r] >= 0 && table[slot[r]] == (int32_t)r;
-    rep[r] = is ? 1 : 0;
-    loff[r] = is ? len[r] : 0;
-    if (is) atomicAdd(&sc->entries64, (unsigned long long)len[r]);
+// rep[i]: i is its fingerprint's lowest item; loff[i]: its list length if so (scanned into list offsets)
+template <typename Src>
+__global__ void k_cen_rep(int64_t n, Src src, const int32_t* __restrict__ slot, const int32_t* __restrict__ table,
+                          int32_t* __restrict__ rep, int32_t* __restrict__ loff, GroupScal* __restrict__ sc) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const bool is = slot[i] >= 0 && table[slot[i]] == (int32_t)i;
+    const int32_t l = is ? src.length((int32_t)i) : 0;
+    rep[i] = is ? 1 : 0;
+    loff[i] = l;
+    if (is) atomicAdd(&sc->entries64, (unsigned long long)l);
 }
 
+template <typename Src>
 struct ClassArgs {
-    int64_t R;
+    int64_t n;
     const int32_t* slot;
     const int32_t* table;
     const int32_t* tcnt;
     const int32_t* rep;
     const int32_t* rpos;
     const int32_t* loff;
-    const uint32_t* rflags;
-    OutFp fp;
+    Src src;
     int32_t* cls;
     uint64_t* c_h1;
     uint64_t* c_h2;
-    int32_t *c_rep, *c_len, *c_voters, *c_off, *c_rule;
+    int32_t *c_rep, *c_len, *c_voters, *c_off;
 };
-__global__ void k_cen_classes(ClassArgs a) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= a.R) return;
-    const int32_t sl = a.slot[r];
-    a.cls[r] = sl >= 0 ? a.rpos[a.table[sl]] : -1;
-    if (!a.rep[r]) return;
-    const int32_t c = a.rpos[r];
-    a.fp((int32_t)r, &a.c_h1[c], &a.c_h2[c], &a.c_len[c]);
-    a.c_rep[c] = (int32_t)r;
+template <typename Src>
+__global__ void k_cen_classes(ClassArgs<Src> a) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n) return;
+    const int32_t sl = a.slot[i];
+    a.cls[i] = sl >= 0 ? a.rpos[a.table[sl]] : -1;
+    if (!a.rep[i]) return;
+    const int32_t c = a.rpos[i];
+    a.src((int32_t)i, &a.c_h1[c], &a.c_h2[c], &a.c_len[c]);
+    a.c_rep[c] = (int32_t)i;
     a.c_voters[c] = a.tcnt[sl];
-    a.c_off[c] = a.loff[r];
-    a.c_rule[c] = (a.rflags[r] & RF_RULE_GE_H) ? 1 : 0;
+    a.c_off[c] = a.loff[i];
 }
 
 // ------------------------------------------------------------------ lists
 __global__ void k_cen_class_out(int32_t nc, int32_t ne, const uint64_t* __restrict__ c_h1, const uint64_t* __restrict__ c_h2,
                                 const int32_t* __restrict__ c_len, const int32_t* __restrict__ c_voters, const int32_t* __restrict__ c_rep,
                                 const int32_t* __restrict__ c_off, uint64_t* __restrict__ h1, uint64_t* __restrict__ h2,
-                                int32_t* __restrict__ len, int32_t* __restrict__ voters, int32_t* __restrict__ rep, int64_t* __restrict__ off,
-                                int32_t* __restrict__ fill) {
+                                int32_t* __restrict__ len, int32_t* __restrict__ voters, int32_t* __restrict__ rep, int64_t* __restrict__ off) {
     const int32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c == nc) off[c] = ne;
     if (c >= nc) return;
     h1[c] = c_h1[c]; h2[c] = c_h2[c]; len[c] = c_len[c]; voters[c] = c_voters[c]; rep[c] = c_rep[c];
     off[c] = c_off[c];
-    fill[c] = 0;
 }
 
 // one thread per (class, subject slot): the slot's subject joins the class's list if its representative announced it.  Lanes of a
@@ -163,8 +156,8 @@ struct GatherArgs {
     uint32_t RM;
     RowRef rows;
     MarkPlane emit;
+    const uint32_t* rflags;
     const int32_t* c_rep;
-    const int32_t* c_rule;
     const int32_t* c_off;
     const int32_t* c_len;
     int32_t* c_fill;
@@ -179,7 +172,8 @@ __global__ void k_cen_gather(GatherArgs a) {
     const int64_t n = (int64_t)a.nc * a.S;
     const int32_t c = i < n ? (int32_t)(i / a.S) : -1;
     const int32_t s = i < n ? (int32_t)(i - (int64_t)c * a.S) : 0;
-    const bool in = i < n && in_announced_proposal(a.rows, a.emit, s, a.c_rep[c], a.H, a.RM, a.c_rule[c]);
+    const int32_t r = i < n ? a.c_rep[c] : 0;
+    const bool in = i < n && in_announced_proposal(a.rows, a.emit, s, r, a.H, a.RM, (a.rflags[r] & RF_RULE_GE_H) ? 1 : 0);
     const unsigned act = __ballot_sync(0xffffffffu, in);
     if (!in) return;
     const unsigned peers = __match_any_sync(act, c);
@@ -215,7 +209,7 @@ __global__ void k_cen_entries(int32_t n, int64_t members, const int32_t* __restr
     if (j >= n) return;
     const int32_t id = e_id[perm[j]];
     ids[j] = id;
-    status[j] = id < members ? RAPID_EDGE_DOWN : RAPID_EDGE_UP;
+    if (status) status[j] = id < members ? RAPID_EDGE_DOWN : RAPID_EDGE_UP;
 }
 
 // ------------------------------------------------------------------ distance from a cut
@@ -236,16 +230,35 @@ __global__ void __launch_bounds__(TB) k_cen_in_cut(const int64_t* __restrict__ o
 }
 
 // ------------------------------------------------------------------ host side
-static int32_t census_get(CD* cd, Census** out) {
-    if (!cd->census) {
-        Census* c = new Census();
-        int32_t rc;
-        if ((rc = c->sc.reserve(1)) || (rc = c->h_sc.reserve(1))) { delete c; return rc; }
-        cd->census = c;
-    }
-    *out = cd->census;
+template <typename Src>
+int32_t group_proposals(cudaStream_t s, int64_t n, const Src& src, ProposalGroups& g, int32_t* cls) {
+    const size_t N = (size_t)std::max<int64_t>(n, 1);
+    uint32_t Tcap = CEN_TABLE_MIN;
+    while ((int64_t)Tcap < 2 * n) Tcap <<= 1;
+    RAPID_CHECK(g.sc.reserve(1)); RAPID_CHECK(g.h_sc.reserve(1));
+    RAPID_CHECK(g.table.reserve(Tcap)); RAPID_CHECK(g.tcnt.reserve(Tcap));
+    RAPID_CHECK(g.slot.reserve(N)); RAPID_CHECK(g.rep.reserve(N)); RAPID_CHECK(g.rpos.reserve(N)); RAPID_CHECK(g.loff.reserve(N));
+    RAPID_CUDA(cudaMemsetAsync(g.sc.p, 0, sizeof(GroupScal), s));
+    k_cen_count<<<grid_for(n), TB, 0, s>>>(n, src, g.sc.p);
+    k_cen_table_init<<<(unsigned)std::min<int64_t>(ceil_div<int64_t>(Tcap, TB), 4 * TARGET_SMS), TB, 0, s>>>(g.sc.p, g.table.p, g.tcnt.p);
+    k_cen_claim<<<grid_for(n), TB, 0, s>>>(n, src, g.sc.p, g.table.p, g.tcnt.p, g.slot.p);
+    k_cen_rep<<<grid_for(n), TB, 0, s>>>(n, src, g.slot.p, g.table.p, g.rep.p, g.loff.p, g.sc.p);
+    RAPID_KERNEL_CHECK();
+    RAPID_CHECK(exclusive_scan_i32(g.rpos.p, n, g.scan_sums, &g.sc.p->n_classes, s, nullptr, g.rep.p));
+    RAPID_CHECK(exclusive_scan_i32(g.loff.p, n, g.scan_sums, &g.sc.p->n_entries, s, nullptr));
+    RAPID_CUDA(cudaMemcpyAsync(g.h_sc.p, g.sc.p, sizeof(GroupScal), cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    const size_t C = (size_t)std::max(g.h_sc.p->n_classes, 1);
+    RAPID_CHECK(g.c_h1.reserve(C)); RAPID_CHECK(g.c_h2.reserve(C)); RAPID_CHECK(g.c_rep.reserve(C)); RAPID_CHECK(g.c_len.reserve(C));
+    RAPID_CHECK(g.c_voters.reserve(C)); RAPID_CHECK(g.c_off.reserve(C)); RAPID_CHECK(g.c_fill.reserve(C));
+    ClassArgs<Src> ca{n, g.slot.p, g.table.p, g.tcnt.p, g.rep.p, g.rpos.p, g.loff.p, src, cls,
+                      g.c_h1.p, g.c_h2.p, g.c_rep.p, g.c_len.p, g.c_voters.p, g.c_off.p};
+    k_cen_classes<<<grid_for(n), TB, 0, s>>>(ca);
+    RAPID_KERNEL_CHECK();
     return RAPID_OK;
 }
+template int32_t group_proposals<AnnouncedFp>(cudaStream_t, int64_t, const AnnouncedFp&, ProposalGroups&, int32_t*);
+template int32_t group_proposals<AnswerFp>(cudaStream_t, int64_t, const AnswerFp&, ProposalGroups&, int32_t*);
 
 static int bits_for(int64_t n) {                  // bits of the largest value below n (at least 1)
     int b = 1;
@@ -253,33 +266,46 @@ static int bits_for(int64_t n) {                  // bits of the largest value b
     return b;
 }
 
+int32_t list_proposals(cudaStream_t s, const CD* cd, ProposalGroups& g, int32_t* ids, uint8_t* status) {
+    const int32_t nc = g.h_sc.p->n_classes, ne = g.h_sc.p->n_entries;
+    if (ne <= 0) return RAPID_OK;
+    if (!g.ls) g.ls = new ListScratch();
+    ListScratch& e = *g.ls;
+    const size_t E = (size_t)ne;
+    RAPID_CHECK(e.e_id.reserve(E)); RAPID_CHECK(e.e_cls.reserve(E)); RAPID_CHECK(e.e_key.reserve(E));
+    RAPID_CHECK(e.idx.reserve(E)); RAPID_CHECK(e.perm.reserve(E)); RAPID_CHECK(e.k32.reserve(E)); RAPID_CHECK(e.k32s.reserve(E));
+    RAPID_CHECK(e.k64.reserve(E)); RAPID_CHECK(e.k64s.reserve(E));
+    RAPID_CUDA(cudaMemsetAsync(g.c_fill.p, 0, (size_t)nc * sizeof(int32_t), s));
+    const int32_t S = cd->S;
+    GatherArgs ga{nc, S, cd->H, (1u << cd->K) - 1u, rowref(cd), emit_plane(cd), cd->rflags.p, g.c_rep.p, g.c_off.p, g.c_len.p,
+                  g.c_fill.p, cd->slot_subject.p, cd->view->key.p /* ring 0 row */, e.e_id.p, e.e_cls.p, e.e_key.p};
+    k_cen_gather<<<grid_for((int64_t)nc * S), TB, 0, s>>>(ga);
+    // stable LSD: by id, then by signed ring-0 key, then by class
+    k_cen_iota<<<grid_for(ne), TB, 0, s>>>(ne, e.e_id.p, e.k32.p, e.idx.p);
+    RAPID_KERNEL_CHECK();
+    uint32_t* k32 = reinterpret_cast<uint32_t*>(e.k32.p);
+    uint32_t* k32s = reinterpret_cast<uint32_t*>(e.k32s.p);
+    RAPID_CHECK(radix_sort_pairs<uint32_t>(e.rs, k32, e.idx.p, k32s, e.perm.p, ne, 0, bits_for(cd->view->n + cd->view->nj), s));
+    k_cen_key64<<<grid_for(ne), TB, 0, s>>>(ne, e.perm.p, e.e_key.p, e.k64.p);
+    RAPID_KERNEL_CHECK();
+    RAPID_CHECK(radix_sort_pairs<uint64_t>(e.rs, e.k64.p, e.perm.p, e.k64s.p, e.idx.p, ne, 0, 64, s));
+    int32_t* order = e.idx.p;
+    if (nc > 1) {
+        k_cen_key32<<<grid_for(ne), TB, 0, s>>>(ne, e.idx.p, e.e_cls.p, e.k32.p);
+        RAPID_KERNEL_CHECK();
+        RAPID_CHECK(radix_sort_pairs<uint32_t>(e.rs, k32, e.idx.p, k32s, e.perm.p, ne, 0, bits_for(nc), s));
+        order = e.perm.p;
+    }
+    k_cen_entries<<<grid_for(ne), TB, 0, s>>>(ne, cd->view->n, order, e.e_id.p, ids, status);
+    RAPID_KERNEL_CHECK();
+    return RAPID_OK;
+}
+
 static int32_t census_run(CD* cd, Census* e, const int32_t* cut_ids, int32_t cut_len) {
     cudaStream_t s = cd->stream;
     CensusOut& o = e->out[1 - e->cur];
     const int64_t R = cd->R;
-    const size_t RN = (size_t)R;
     const int64_t ntot = cd->view->n + cd->view->nj;
-    // ---- claim and classes
-    uint32_t Tcap = CEN_TABLE_MIN;
-    while ((int64_t)Tcap < 2 * R) Tcap <<= 1;
-    RAPID_CHECK(e->table.reserve(Tcap)); RAPID_CHECK(e->tcnt.reserve(Tcap));
-    RAPID_CHECK(e->slot.reserve(RN)); RAPID_CHECK(e->rep.reserve(RN)); RAPID_CHECK(e->rpos.reserve(RN)); RAPID_CHECK(e->loff.reserve(RN));
-    RAPID_CHECK(e->c_h1.reserve(RN)); RAPID_CHECK(e->c_h2.reserve(RN)); RAPID_CHECK(e->c_rep.reserve(RN)); RAPID_CHECK(e->c_len.reserve(RN));
-    RAPID_CHECK(e->c_voters.reserve(RN)); RAPID_CHECK(e->c_off.reserve(RN)); RAPID_CHECK(e->c_rule.reserve(RN)); RAPID_CHECK(e->c_fill.reserve(RN));
-    RAPID_CHECK(o.cls.reserve(RN));
-    RAPID_CUDA(cudaMemsetAsync(e->sc.p, 0, sizeof(CensusScal), s));
-    const OutFp fp{cd->out_h1.p, cd->out_h2.p, cd->out_len.p};
-    k_cen_count<<<grid_for(R), TB, 0, s>>>(R, cd->rflags.p, e->sc.p);
-    k_cen_table_init<<<(unsigned)std::min<int64_t>(ceil_div<int64_t>(Tcap, TB), 4 * TARGET_SMS), TB, 0, s>>>(e->sc.p, e->table.p, e->tcnt.p);
-    k_cen_claim<<<grid_for(R), TB, 0, s>>>(R, cd->rflags.p, fp, e->sc.p, e->table.p, e->tcnt.p, e->slot.p);
-    k_cen_rep<<<grid_for(R), TB, 0, s>>>(R, e->slot.p, e->table.p, cd->out_len.p, e->rep.p, e->loff.p, e->sc.p);
-    RAPID_KERNEL_CHECK();
-    RAPID_CHECK(exclusive_scan_i32(e->rpos.p, R, e->scan_sums, &e->sc.p->n_classes, s, nullptr, e->rep.p));
-    RAPID_CHECK(exclusive_scan_i32(e->loff.p, R, e->scan_sums, &e->sc.p->n_entries, s, nullptr));
-    ClassArgs ca{R, e->slot.p, e->table.p, e->tcnt.p, e->rep.p, e->rpos.p, e->loff.p, cd->rflags.p, fp, o.cls.p,
-                 e->c_h1.p, e->c_h2.p, e->c_rep.p, e->c_len.p, e->c_voters.p, e->c_off.p, e->c_rule.p};
-    k_cen_classes<<<grid_for(R), TB, 0, s>>>(ca);
-    RAPID_KERNEL_CHECK();
     // the cut's bitmap (ids checked by the caller)
     if (cut_ids) {
         const size_t words = (size_t)ceil_div<int64_t>(std::max<int64_t>(ntot, 1), 32);
@@ -291,10 +317,11 @@ static int32_t census_run(CD* cd, Census* e, const int32_t* cut_ids, int32_t cut
             RAPID_KERNEL_CHECK();
         }
     }
-    // the one synchronisation: the counts the caller gets back, which size the lists
-    RAPID_CUDA(cudaMemcpyAsync(e->h_sc.p, e->sc.p, sizeof(CensusScal), cudaMemcpyDeviceToHost, s));
-    RAPID_CUDA(cudaStreamSynchronize(s));
-    const CensusScal h = *e->h_sc.p;
+    // ---- claim and classes; the one synchronisation: the counts the caller gets back, which size the lists
+    RAPID_CHECK(o.cls.reserve((size_t)R));
+    const AnnouncedFp fp{cd->rflags.p, cd->out_h1.p, cd->out_h2.p, cd->out_len.p, 0};
+    RAPID_CHECK(group_proposals(s, R, fp, e->g, o.cls.p));
+    const GroupScal h = *e->g.h_sc.p;
     if (h.entries64 >= (1ULL << 30)) { set_error("the census would list %llu entries (at most 2^30)", h.entries64); return RAPID_ENOMEM; }
     const int32_t nc = h.n_classes, ne = h.n_entries;
     // ---- lists
@@ -303,37 +330,11 @@ static int32_t census_run(CD* cd, Census* e, const int32_t* cut_ids, int32_t cut
     RAPID_CHECK(o.rep.reserve((size_t)std::max(nc, 1))); RAPID_CHECK(o.in_cut.reserve((size_t)std::max(nc, 1)));
     RAPID_CHECK(o.off.reserve((size_t)nc + 1));
     RAPID_CHECK(o.ids.reserve((size_t)std::max(ne, 1))); RAPID_CHECK(o.status.reserve((size_t)std::max(ne, 1)));
-    k_cen_class_out<<<grid_for((int64_t)nc + 1), TB, 0, s>>>(nc, ne, e->c_h1.p, e->c_h2.p, e->c_len.p, e->c_voters.p, e->c_rep.p,
-                                                             e->c_off.p, o.h1.p, o.h2.p, o.len.p, o.voters.p, o.rep.p, o.off.p, e->c_fill.p);
+    const ProposalGroups& g = e->g;
+    k_cen_class_out<<<grid_for((int64_t)nc + 1), TB, 0, s>>>(nc, ne, g.c_h1.p, g.c_h2.p, g.c_len.p, g.c_voters.p, g.c_rep.p,
+                                                             g.c_off.p, o.h1.p, o.h2.p, o.len.p, o.voters.p, o.rep.p, o.off.p);
     RAPID_KERNEL_CHECK();
-    if (ne > 0) {
-        const size_t E = (size_t)ne;
-        RAPID_CHECK(e->e_id.reserve(E)); RAPID_CHECK(e->e_cls.reserve(E)); RAPID_CHECK(e->e_key.reserve(E));
-        RAPID_CHECK(e->idx.reserve(E)); RAPID_CHECK(e->perm.reserve(E)); RAPID_CHECK(e->k32.reserve(E)); RAPID_CHECK(e->k32s.reserve(E));
-        RAPID_CHECK(e->k64.reserve(E)); RAPID_CHECK(e->k64s.reserve(E));
-        const int32_t S = cd->S;
-        GatherArgs ga{nc, S, cd->H, (1u << cd->K) - 1u, rowref(cd), emit_plane(cd), e->c_rep.p, e->c_rule.p, e->c_off.p, e->c_len.p,
-                      e->c_fill.p, cd->slot_subject.p, cd->view->key.p /* ring 0 row */, e->e_id.p, e->e_cls.p, e->e_key.p};
-        k_cen_gather<<<grid_for((int64_t)nc * S), TB, 0, s>>>(ga);
-        // stable LSD: by id, then by signed ring-0 key, then by class
-        k_cen_iota<<<grid_for(ne), TB, 0, s>>>(ne, e->e_id.p, e->k32.p, e->idx.p);
-        RAPID_KERNEL_CHECK();
-        uint32_t* k32 = reinterpret_cast<uint32_t*>(e->k32.p);
-        uint32_t* k32s = reinterpret_cast<uint32_t*>(e->k32s.p);
-        RAPID_CHECK(radix_sort_pairs<uint32_t>(e->rs, k32, e->idx.p, k32s, e->perm.p, ne, 0, bits_for(ntot), s));
-        k_cen_key64<<<grid_for(ne), TB, 0, s>>>(ne, e->perm.p, e->e_key.p, e->k64.p);
-        RAPID_KERNEL_CHECK();
-        RAPID_CHECK(radix_sort_pairs<uint64_t>(e->rs, e->k64.p, e->perm.p, e->k64s.p, e->idx.p, ne, 0, 64, s));
-        int32_t* order = e->idx.p;
-        if (nc > 1) {
-            k_cen_key32<<<grid_for(ne), TB, 0, s>>>(ne, e->idx.p, e->e_cls.p, e->k32.p);
-            RAPID_KERNEL_CHECK();
-            RAPID_CHECK(radix_sort_pairs<uint32_t>(e->rs, k32, e->idx.p, k32s, e->perm.p, ne, 0, bits_for(nc), s));
-            order = e->perm.p;
-        }
-        k_cen_entries<<<grid_for(ne), TB, 0, s>>>(ne, cd->view->n, order, e->e_id.p, o.ids.p, o.status.p);
-        RAPID_KERNEL_CHECK();
-    }
+    RAPID_CHECK(list_proposals(s, cd, e->g, o.ids.p, o.status.p));
     if (nc > 0) {
         if (cut_ids) k_cen_in_cut<<<(unsigned)nc, TB, 0, s>>>(o.off.p, o.ids.p, e->cut_bits.p, o.in_cut.p);
         else RAPID_CUDA(cudaMemsetAsync(o.in_cut.p, 0xff, (size_t)nc * sizeof(int32_t), s));
@@ -376,8 +377,8 @@ int32_t rapid_cd_proposal_census(rapid_cd* cd, const int32_t* cut_ids, int32_t c
     }
     DeviceGuard g(cd->device);
     RAPID_CHECK(cd_wait(cd, false));      // asynchronous batches still in flight on the handle's stream
-    Census* e = nullptr;
-    RAPID_CHECK(census_get(cd, &e));
+    if (!cd->census) cd->census = new Census();
+    Census* e = cd->census;
     RAPID_CHECK(census_run(cd, e, cut_ids, cut_len));
     const CensusOut& o = e->out[e->cur];
     if (n_classes) *n_classes = o.n_classes;

@@ -433,6 +433,60 @@ int32_t cd_wait(const CD* cd, bool take_status);
 // implemented in cd_census.cu
 void census_destroy(CD* cd);
 
+// ---- grouping announced proposals (cd_census.cu): the proposal census and the wire encoder's list-carrying messages ---------
+// Fingerprint sources: item i takes part iff part(i); fp(i, &h1, &h2, &len) reads its fingerprint (the fp of fp_table_claim).
+struct AnnouncedFp {                  // a detector's receivers that announced in its last call with at least min_len entries
+    const uint32_t* rflags;
+    const uint64_t* h1;
+    const uint64_t* h2;
+    const int32_t* len;
+    int32_t min_len;
+    __device__ __forceinline__ int32_t length(int32_t i) const { return len[i]; }
+    __device__ __forceinline__ bool part(int32_t i) const { return (rflags[i] & RF_ANN_NOW) && (min_len <= 0 || len[i] >= min_len); }
+    __device__ __forceinline__ void operator()(int32_t i, uint64_t* a, uint64_t* b, int32_t* l) const { *a = h1[i]; *b = h2[i]; *l = len[i]; }
+};
+struct AnswerFp {                     // acceptors' answers with a non-empty list: per answer, or (h1 == NULL) the constant (c1, c2, clen)
+    const uint64_t* h1;
+    const uint64_t* h2;
+    const int32_t* len;
+    uint64_t c1, c2;
+    int32_t clen;
+    __device__ __forceinline__ int32_t length(int32_t i) const { return h1 ? len[i] : clen; }
+    __device__ __forceinline__ bool part(int32_t i) const { return length(i) > 0; }
+    __device__ __forceinline__ void operator()(int32_t i, uint64_t* a, uint64_t* b, int32_t* l) const {
+        if (h1) { *a = h1[i]; *b = h2[i]; *l = len[i]; } else { *a = c1; *b = c2; *l = clen; }
+    }
+};
+
+struct GroupScal {
+    int32_t n_part, n_classes, n_entries, T;
+    unsigned long long entries64;     // the representatives' lengths summed in 64 bits (the int32 scan must not wrap)
+};
+
+// A grouping's scratch and per-class outputs.  Class c is the c-th representative (the lowest item of a fingerprint) in item
+// order: c_h1/c_h2/c_len its fingerprint, c_rep its representative, c_voters the items that hold it, c_off the exclusive scan of
+// the lengths.  The per-item arrays slot, rep, rpos and loff are free for the caller's use once group_proposals returns.
+struct ProposalGroups {
+    DevBuf<int32_t> table, tcnt;                                      // [T cap] open-addressing table: lowest item, voters
+    DevBuf<int32_t> slot, rep, rpos, loff, scan_sums;                 // [n]
+    DevBuf<uint64_t> c_h1, c_h2;                                      // [n_classes]
+    DevBuf<int32_t> c_rep, c_len, c_voters, c_off, c_fill;
+    DevBuf<GroupScal> sc;
+    PinnedBuf<GroupScal> h_sc;                                        // the counts, on the host once group_proposals returns
+    struct ListScratch* ls = nullptr;                                 // list_proposals' entry and sort scratch
+    ProposalGroups() = default;
+    ~ProposalGroups();
+};
+
+// Groups items [0, n) by fingerprint on stream s: cls[i] = class of item i (-1: it does not take part), and the per-class
+// outputs.  One host synchronisation, before the per-class outputs are written (they are sized by the class count).
+template <typename Src>
+int32_t group_proposals(cudaStream_t s, int64_t n, const Src& src, ProposalGroups& g, int32_t* cls);
+// The list of every class of a grouping of cd's receivers, by rapid_cd_get_proposal's rule and in its order: class c's entries
+// at ids[c_off[c] ..], the status of each (DOWN: a member, UP: a registered joiner) to `status` unless it is NULL.  c_fill[c]
+// counts the subjects the rule found; a class never takes more than c_len[c] of them.
+int32_t list_proposals(cudaStream_t s, const CD* cd, ProposalGroups& g, int32_t* ids, uint8_t* status);
+
 }  // namespace rapid
 
 struct rapid_cd : rapid::CD {};

@@ -152,8 +152,8 @@ RAPID_HD uint64_t fp_mix2(int32_t id) { return splitmix64(((uint64_t)(uint32_t)i
 #ifdef __CUDACC__
 // Open addressing over proposal fingerprints (a, b, l) = (h1, h2, len) in a table of T (a power of two) slots, empty slots -1:
 // item s claims the slot of its fingerprint, and the slot keeps the LOWEST item holding it (atomicCAS, then atomicMin).
-// fp(i, &a, &b, &l) reads item i's fingerprint.  Returns the slot.  The wire encoder numbers its bodies and the proposal census
-// its classes this way.
+// fp(i, &a, &b, &l) reads item i's fingerprint.  Returns the slot.  The proposal grouping (group_proposals, cd_census.cu) numbers
+// the census's classes and the wire encoder's bodies this way.
 template <typename FP>
 __device__ __forceinline__ uint32_t fp_table_claim(int32_t* table, uint32_t T, int32_t s, uint64_t a, uint64_t b, int32_t l, const FP& fp) {
     uint32_t pos = (uint32_t)(splitmix64(a ^ (b * 0x9E3779B97F4A7C15ULL) ^ (uint64_t)l) >> 32) & (T - 1);

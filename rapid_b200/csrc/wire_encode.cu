@@ -3,15 +3,15 @@
 //
 // A message is a HEADER plus, for the kinds whose last field is a list, a BODY shared by every message that carries the same
 // list: canonical bytes = header ++ body, because fields are serialized in field-number order and the list is the highest.
-// Bodies are the distinct (h1, h2, len) fingerprints of the lists (the identity the tally already counts votes by), found on the
-// device with an open-addressing table; each is encoded once, one thread per list ENTRY, from the canonical list of its lowest
-// receiver.  Every kind is count -> exclusive scan -> emit, the scheme of the decoder (wire.cu), with the int32 scans of scan.cuh.
+// Bodies are the distinct (h1, h2, len) fingerprints of the lists (the identity the tally already counts votes by), grouped on the
+// device by the proposal census's grouping (group_proposals, cd_census.cu); each is encoded once, one thread per list ENTRY, from
+// the canonical list of its lowest sender.  Every kind is count -> exclusive scan -> emit, the scheme of the decoder (wire.cu),
+// with the int32 scans of scan.cuh.
 // Outputs are double-buffered: an encode writes the spare set and swaps on success, so a refused or failed encode leaves the
 // previous outputs as they were.
 #include <limits.h>
 
 #include <algorithm>
-#include <functional>
 #include <map>
 #include <tuple>
 #include <vector>
@@ -193,17 +193,9 @@ struct ListIn {
     const int32_t* acc;                 // answers: the sender's acceptor index, a ring-0 position; NULL: rbegin + slot
     int64_t rbegin;
     const int32_t* ring0;
-    const uint64_t* h1;                 // the slot's list fingerprint; NULL: the constant (c1, c2, clen) of a Phase2a value
-    const uint64_t* h2;
-    const int32_t* len;
-    uint64_t c1, c2;
-    int32_t clen;
     const int64_t* vrnd;                // Phase1b: per slot
     int64_t rank;                       // Phase1b / Phase2b: rnd (packed, see pack_rank)
 };
-__device__ __forceinline__ void list_fp(const ListIn& L, int32_t s, uint64_t* a, uint64_t* b, int32_t* l) {
-    if (L.h1) { *a = L.h1[s]; *b = L.h2[s]; *l = L.len[s]; } else { *a = L.c1; *b = L.c2; *l = L.clen; }
-}
 __device__ __forceinline__ bool list_sends(const ListIn& L, int32_t s) { return !L.rflags || (L.rflags[s] & RF_ANN_NOW); }
 __device__ __forceinline__ int32_t list_sender(const ListIn& L, int32_t s) { return L.ring0[L.acc ? L.acc[s] : L.rbegin + s]; }
 // Rank {round = 1, nodeIndex = 2}, int32 fields
@@ -223,39 +215,9 @@ RAPID_HD uint8_t list_tag(int32_t kind) {                                  // en
     return kind == RAPID_WIRE_FAST_ROUND_PHASE2B ? 0x1A : kind == RAPID_WIRE_PHASE1B ? 0x2A : 0x22;
 }
 
-// every slot with a non-empty list claims the table slot of the list's fingerprint (fp_table_claim); the slot keeps the LOWEST
-// such slot (the body's representative)
-__global__ void k_enc_list_claim(ListIn L, uint32_t T, int32_t* __restrict__ table, int32_t* __restrict__ slot, int32_t* __restrict__ send) {
+__global__ void k_enc_send(ListIn L, int32_t* __restrict__ send) {
     const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= L.n) return;
-    const bool v = list_sends(L, s);
-    send[s] = v ? 1 : 0;
-    uint64_t a, b; int32_t l;
-    list_fp(L, s, &a, &b, &l);
-    if (!v || l <= 0) { slot[s] = -1; return; }
-    const auto fp = [&](int32_t i, uint64_t* ca, uint64_t* cb, int32_t* cl) { list_fp(L, i, ca, cb, cl); };
-    slot[s] = (int32_t)fp_table_claim(table, T, s, a, b, l, fp);
-}
-__global__ void k_enc_list_rep(int32_t n, const int32_t* __restrict__ slot, const int32_t* __restrict__ table, int32_t* __restrict__ rep) {
-    const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s < n) rep[s] = (slot[s] >= 0 && table[slot[s]] == s) ? 1 : 0;
-}
-// body id of every slot (bodies numbered by ascending representative, -1: no list), and the representatives in body order
-__global__ void k_enc_list_bodies(int32_t n, const int32_t* __restrict__ slot, const int32_t* __restrict__ table,
-                                  const int32_t* __restrict__ rep, const int32_t* __restrict__ rpos, int32_t* __restrict__ bid_s,
-                                  int32_t* __restrict__ reps) {
-    const int32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    bid_s[s] = slot[s] >= 0 ? rpos[table[slot[s]]] : -1;
-    if (rep[s]) reps[rpos[s]] = s;
-}
-__global__ void k_enc_gather_fp(int32_t nb, ListIn L, const int32_t* __restrict__ reps, uint64_t* __restrict__ g1, uint64_t* __restrict__ g2,
-                                int32_t* __restrict__ gl, int32_t* __restrict__ gacc) {
-    const int32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= nb) return;
-    const int32_t s = reps[b];
-    list_fp(L, s, &g1[b], &g2[b], &gl[b]);
-    gacc[b] = L.acc ? L.acc[s] : (int32_t)(L.rbegin + s);
+    if (s < L.n) send[s] = list_sends(L, s) ? 1 : 0;
 }
 // one thread per list entry: its size as a repeated Endpoint field
 __global__ void k_enc_entry_sizes(int32_t n, const int32_t* __restrict__ ids, EpTab t, int32_t* __restrict__ sz, EncScal* __restrict__ sc) {
@@ -270,13 +232,12 @@ __global__ void k_enc_entry_emit(int32_t n, const int32_t* __restrict__ ids, EpT
     const int32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j < n) put_ep_field(out + pos[j], tag, t, ids[j]);
 }
-// body b = entries [first[b], first[b + 1]): its byte range
-__global__ void k_enc_body_off(int32_t nb, int32_t n_entries, const int32_t* __restrict__ first, const int32_t* __restrict__ pos,
+// body b = entries [first[b], first[b] + len[b]), len[b] > 0: its byte range
+__global__ void k_enc_body_off(int32_t nb, const int32_t* __restrict__ first, const int32_t* __restrict__ pos,
                                const EncScal* __restrict__ sc, int64_t* __restrict__ boff) {
     const int32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b > nb) return;
-    const int32_t e = first[b];
-    boff[b] = e < n_entries ? pos[e] : sc->body_bytes;
+    boff[b] = b < nb ? pos[first[b]] : sc->body_bytes;
 }
 // per sending slot: header = [RapidRequest tag, length] sender, configurationId (omitted when 0), and the kind's ranks (Phase1b:
 // rnd, vrnd; Phase2b: rnd; both set, so written even when (0, 0))
@@ -347,9 +308,10 @@ struct WireEnc {
     EncOut out[2];
     int cur = 0;                       // out[cur] holds the last successful encode
     DevBuf<int32_t> a, b, c, d, e, f, g, scan_sums;
-    DevBuf<int32_t> table, ids, ids2, epos, gl, gacc;
-    DevBuf<uint64_t> g1, g2;
+    DevBuf<int32_t> ids, epos;
     DevBuf<int64_t> sizes;
+    ProposalGroups grp;                // the bodies of list-carrying messages (group_bodies), never a detector's census
+    DevBuf<int32_t> cls;               // [n]: body of every slot, -1 for none
     DevBuf<EncScal> sc;
     PinnedBuf<EncScal> h_sc;
     // the lists already fetched as ids, by (h1, h2, len), for the view's member_epoch `lists_epoch`: a vval or Phase2a value is
@@ -451,98 +413,61 @@ static int32_t encode_alerts(WireEnc* e, const WireEncCtx& ctx, const FdetInterv
 }
 
 
-// The list of every distinct body: fetch(representative's acceptor / receiver index, fingerprint, ids) -> RAPID_OK with the ids.
-using ListFetch = std::function<int32_t(int64_t, uint64_t, uint64_t, int32_t, std::vector<int32_t>&)>;
+// Groups the slots' lists (group_proposals): the body of slot s is cls[s], bodies numbered by their lowest slot.  Every entry is
+// >= 2 bytes: an encode whose bodies would list more than ENC_LIMIT / 2 entries is refused before they are listed.
+template <typename Src>
+static int32_t group_bodies(WireEnc* e, cudaStream_t s, int64_t n, const Src& src) {
+    RAPID_CHECK(e->cls.reserve((size_t)std::max<int64_t>(n, 1)));
+    RAPID_CHECK(group_proposals(s, n, src, e->grp, e->cls.p));
+    if ((int64_t)e->grp.h_sc.p->entries64 > ENC_LIMIT / 2) return too_big();
+    return RAPID_OK;
+}
 
-// The messages of the sending slots of L, in slot order: bodies first (distinct fingerprints on the device, each list fetched
-// once on the host and encoded one thread per entry), then one header per message.
-static int32_t encode_lists(WireEnc* e, const WireEncCtx& ctx, const ListIn& L0, const ListFetch& fetch) {
+// The messages of the sending slots of L, in slot order, once group_bodies has run and every body's list is in e->ids at its
+// class's offset: bodies first (one thread per entry), then one header per message.
+static int32_t encode_lists(WireEnc* e, const WireEncCtx& ctx, const ListIn& L) {
     cudaStream_t s = ctx.stream;
     EncOut& o = e->out[1 - e->cur];
-    ListIn L = L0;
     const int32_t n = L.n;
     const EpTab t = ep_tab(ctx.view);
+    const ProposalGroups& g = e->grp;
+    const int32_t nb = g.h_sc.p->n_classes, nE = g.h_sc.p->n_entries;
+    int32_t *send = g.rep.p, *mpos = g.rpos.p, *hsz = g.loff.p, *hpos = g.slot.p;   // the grouping's per-slot scratch is free
     RAPID_CUDA(cudaMemsetAsync(e->sc.p, 0, sizeof(EncScal), s));
-    int64_t nm = 0, nb = 0, hbytes = 0, bbytes = 0;
-    if (n > 0) {
-        const size_t N = (size_t)n;
-        uint32_t T = 1024;
-        while ((int64_t)T < 2 * (int64_t)n) T <<= 1;
-        RAPID_CHECK(e->table.reserve(T));
-        RAPID_CHECK(e->a.reserve(N)); RAPID_CHECK(e->b.reserve(N)); RAPID_CHECK(e->c.reserve(N)); RAPID_CHECK(e->d.reserve(N));
-        RAPID_CHECK(e->f.reserve(N)); RAPID_CHECK(e->g.reserve(N));
-        int32_t *slot = e->a.p, *send = e->b.p, *rep = e->c.p, *rpos = e->d.p, *bid_s = e->f.p, *reps = e->g.p;
-        RAPID_CUDA(cudaMemsetAsync(e->table.p, 0xff, (size_t)T * sizeof(int32_t), s));
-        k_enc_list_claim<<<grid_for(n), TB, 0, s>>>(L, T, e->table.p, slot, send);
-        k_enc_list_rep<<<grid_for(n), TB, 0, s>>>(n, slot, e->table.p, rep);
+    k_enc_send<<<grid_for(n), TB, 0, s>>>(L, send);
+    RAPID_KERNEL_CHECK();
+    RAPID_CHECK(exclusive_scan_i32(mpos, n, e->scan_sums, &e->sc.p->n_msgs, s, nullptr, send));
+    if (nb > 0) {
+        RAPID_CHECK(e->epos.reserve((size_t)nE));
+        k_enc_entry_sizes<<<grid_for(nE), TB, 0, s>>>(nE, e->ids.p, t, e->epos.p, e->sc.p);
         RAPID_KERNEL_CHECK();
-        RAPID_CHECK(exclusive_scan_i32(rpos, n, e->scan_sums, &e->sc.p->n_bodies, s, nullptr, rep));
-        k_enc_list_bodies<<<grid_for(n), TB, 0, s>>>(n, slot, e->table.p, rep, rpos, bid_s, reps);
+    }
+    RAPID_CHECK(enc_read_scal(e, s));
+    if ((int64_t)e->h_sc.p->bytes64 > ENC_LIMIT) return too_big();
+    const int64_t nm = e->h_sc.p->n_msgs, bbytes = (int64_t)e->h_sc.p->bytes64;
+    int64_t hbytes = 0;
+    if (nb > 0) {
+        RAPID_CHECK(exclusive_scan_i32(e->epos.p, nE, e->scan_sums, &e->sc.p->body_bytes, s, nullptr));
+        RAPID_CHECK(o.bodies.reserve((size_t)std::max<int64_t>(bbytes, 1))); RAPID_CHECK(o.boff.reserve((size_t)nb + 1));
+        k_enc_entry_emit<<<grid_for(nE), TB, 0, s>>>(nE, e->ids.p, t, list_tag(L.kind), e->epos.p, o.bodies.p);
+        k_enc_body_off<<<grid_for(nb + 1), TB, 0, s>>>(nb, g.c_off.p, e->epos.p, e->sc.p, o.boff.p);
         RAPID_KERNEL_CHECK();
-        int32_t* mpos = rep;                                                 // rep and rpos are consumed: reuse them
-        int32_t* hsz = rpos;
-        RAPID_CHECK(exclusive_scan_i32(mpos, n, e->scan_sums, &e->sc.p->n_msgs, s, nullptr, send));
+    } else {
+        RAPID_CUDA(cudaMemsetAsync(o.boff.p, 0, sizeof(int64_t), s));
+    }
+    if (nm > 0) {
+        RAPID_CHECK(o.hoff.reserve((size_t)nm + 1)); RAPID_CHECK(o.bid.reserve((size_t)nm)); RAPID_CHECK(o.snd.reserve((size_t)nm));
+        k_enc_list_sizes<<<grid_for(n), TB, 0, s>>>(L, t, send, mpos, e->cls.p, o.boff.p, hsz);
+        RAPID_KERNEL_CHECK();
+        RAPID_CHECK(exclusive_scan_i32(hpos, nm, e->scan_sums, &e->sc.p->hdr_bytes, s, nullptr, hsz));
         RAPID_CHECK(enc_read_scal(e, s));
-        nm = e->h_sc.p->n_msgs; nb = e->h_sc.p->n_bodies;
-        if (nb > 0) {
-            const size_t B = (size_t)nb;
-            RAPID_CHECK(e->g1.reserve(B)); RAPID_CHECK(e->g2.reserve(B)); RAPID_CHECK(e->gl.reserve(B)); RAPID_CHECK(e->gacc.reserve(B));
-            k_enc_gather_fp<<<grid_for(nb), TB, 0, s>>>((int32_t)nb, L, reps, e->g1.p, e->g2.p, e->gl.p, e->gacc.p);
-            RAPID_KERNEL_CHECK();
-            std::vector<uint64_t> f1(B), f2(B);
-            std::vector<int32_t> fl(B), facc(B), first(B + 1, 0), ids;
-            RAPID_CUDA(cudaMemcpyAsync(f1.data(), e->g1.p, B * 8, cudaMemcpyDeviceToHost, s));
-            RAPID_CUDA(cudaMemcpyAsync(f2.data(), e->g2.p, B * 8, cudaMemcpyDeviceToHost, s));
-            RAPID_CUDA(cudaMemcpyAsync(fl.data(), e->gl.p, B * 4, cudaMemcpyDeviceToHost, s));
-            RAPID_CUDA(cudaMemcpyAsync(facc.data(), e->gacc.p, B * 4, cudaMemcpyDeviceToHost, s));
-            RAPID_CUDA(cudaStreamSynchronize(s));
-            int64_t tot = 0;
-            for (size_t b = 0; b < B; ++b) tot += fl[b];
-            if (tot > ENC_LIMIT / 2) return too_big();                      // every entry is >= 2 bytes
-            ids.reserve((size_t)tot);
-            std::vector<int32_t> one;
-            for (size_t b = 0; b < B; ++b) {
-                RAPID_CHECK(fetch(facc[b], f1[b], f2[b], fl[b], one));
-                ids.insert(ids.end(), one.begin(), one.end());
-                first[b + 1] = (int32_t)ids.size();
-            }
-            const int32_t nE = first[B];
-            RAPID_CHECK(e->ids.reserve((size_t)std::max(nE, 1))); RAPID_CHECK(e->e.reserve(B + 1));
-            RAPID_CHECK(e->epos.reserve((size_t)std::max(nE, 1)));
-            RAPID_CUDA(cudaMemcpyAsync(e->ids.p, ids.data(), (size_t)nE * 4, cudaMemcpyHostToDevice, s));
-            RAPID_CUDA(cudaMemcpyAsync(e->e.p, first.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
-            k_enc_entry_sizes<<<grid_for(nE), TB, 0, s>>>(nE, e->ids.p, t, e->epos.p, e->sc.p);
-            RAPID_KERNEL_CHECK();
-            RAPID_CHECK(enc_read_scal(e, s));
-            if ((int64_t)e->h_sc.p->bytes64 > ENC_LIMIT) return too_big();
-            RAPID_CHECK(exclusive_scan_i32(e->epos.p, nE, e->scan_sums, &e->sc.p->body_bytes, s, nullptr));
-            bbytes = (int64_t)e->h_sc.p->bytes64;
-            RAPID_CHECK(o.bodies.reserve((size_t)std::max<int64_t>(bbytes, 1))); RAPID_CHECK(o.boff.reserve(B + 1));
-            k_enc_entry_emit<<<grid_for(nE), TB, 0, s>>>(nE, e->ids.p, t, list_tag(L.kind), e->epos.p, o.bodies.p);
-            k_enc_body_off<<<grid_for(nb + 1), TB, 0, s>>>((int32_t)nb, nE, e->e.p, e->epos.p, e->sc.p, o.boff.p);
-            RAPID_KERNEL_CHECK();
-        } else {
-            RAPID_CUDA(cudaMemsetAsync(o.boff.p, 0, sizeof(int64_t), s));
-        }
-        if (nm > 0) {
-            RAPID_CHECK(o.hoff.reserve((size_t)nm + 1)); RAPID_CHECK(o.bid.reserve((size_t)nm)); RAPID_CHECK(o.snd.reserve((size_t)nm));
-            RAPID_CHECK(e->ids2.reserve((size_t)nm));
-            k_enc_list_sizes<<<grid_for(n), TB, 0, s>>>(L, t, send, mpos, bid_s, o.boff.p, hsz);
-            RAPID_KERNEL_CHECK();
-            int32_t* hpos = e->ids2.p;
-            RAPID_CHECK(exclusive_scan_i32(hpos, nm, e->scan_sums, &e->sc.p->hdr_bytes, s, nullptr, hsz));
-            RAPID_CHECK(enc_read_scal(e, s));
-            hbytes = e->h_sc.p->hdr_bytes;
-            RAPID_CHECK(o.hdr.reserve((size_t)std::max<int64_t>(hbytes, 1)));
-            k_enc_list_emit<<<grid_for(n), TB, 0, s>>>(L, t, send, mpos, bid_s, o.boff.p, hpos, o.bid.p, o.snd.p, o.hdr.p);
-            k_enc_off64<<<grid_for(nm + 1), TB, 0, s>>>((int32_t)nm, hpos, &e->sc.p->hdr_bytes, o.hoff.p);
-            RAPID_KERNEL_CHECK();
-        } else {
-            RAPID_CUDA(cudaMemsetAsync(o.hoff.p, 0, sizeof(int64_t), s));
-        }
+        hbytes = e->h_sc.p->hdr_bytes;
+        RAPID_CHECK(o.hdr.reserve((size_t)std::max<int64_t>(hbytes, 1)));
+        k_enc_list_emit<<<grid_for(n), TB, 0, s>>>(L, t, send, mpos, e->cls.p, o.boff.p, hpos, o.bid.p, o.snd.p, o.hdr.p);
+        k_enc_off64<<<grid_for(nm + 1), TB, 0, s>>>((int32_t)nm, hpos, &e->sc.p->hdr_bytes, o.hoff.p);
+        RAPID_KERNEL_CHECK();
     } else {
         RAPID_CUDA(cudaMemsetAsync(o.hoff.p, 0, sizeof(int64_t), s));
-        RAPID_CUDA(cudaMemsetAsync(o.boff.p, 0, sizeof(int64_t), s));
     }
     RAPID_CUDA(cudaStreamSynchronize(s));
     o.n = nm; o.n_bodies = nb; o.hdr_bytes = hbytes; o.body_bytes = bbytes;
@@ -567,6 +492,71 @@ static int32_t cd_list(const rapid_cd* cd, int64_t receiver, uint64_t h1, uint64
     return RAPID_OK;
 }
 
+// The votes' bodies: the detector's lists of the grouped proposals (list_proposals, into the encoder's storage: the handle's
+// census stays as it was), each checked against its fingerprint and kept in the list cache for the answers.
+static int32_t vote_lists(WireEnc* e, cudaStream_t s, const rapid_cd* cd) {
+    const ProposalGroups& g = e->grp;
+    const int32_t nb = g.h_sc.p->n_classes, nE = g.h_sc.p->n_entries;
+    if (nb == 0) return RAPID_OK;
+    RAPID_CHECK(e->ids.reserve((size_t)nE));
+    RAPID_CHECK(list_proposals(s, cd, e->grp, e->ids.p, nullptr));
+    const size_t B = (size_t)nb;
+    std::vector<uint64_t> h1(B), h2(B);
+    std::vector<int32_t> len(B), fill(B), rep(B), off(B), ids((size_t)nE);
+    RAPID_CUDA(cudaMemcpyAsync(h1.data(), g.c_h1.p, B * 8, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaMemcpyAsync(h2.data(), g.c_h2.p, B * 8, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaMemcpyAsync(len.data(), g.c_len.p, B * 4, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaMemcpyAsync(fill.data(), g.c_fill.p, B * 4, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaMemcpyAsync(rep.data(), g.c_rep.p, B * 4, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaMemcpyAsync(off.data(), g.c_off.p, B * 4, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaMemcpyAsync(ids.data(), e->ids.p, (size_t)nE * 4, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    for (size_t b = 0; b < B; ++b) {
+        const int32_t* l = ids.data() + off[b];
+        uint64_t a = 0, c = 0;
+        if (fill[b] == len[b]) RAPID_CHECK(rapid_proposal_fingerprint(l, len[b], &a, &c));
+        if (fill[b] != len[b] || a != h1[b] || c != h2[b]) { set_error("receiver %d's proposal does not match its fingerprint", rep[b]); return RAPID_EINVAL; }
+        e->lists[std::make_tuple(h1[b], h2[b], len[b])].assign(l, l + len[b]);
+    }
+    return RAPID_OK;
+}
+
+// The answers' bodies: each distinct list from the cache, else from the detector receiver with the representative's index
+static int32_t answer_lists(WireEnc* e, cudaStream_t s, const ListIn& L, const rapid_cd* cd) {
+    const ProposalGroups& g = e->grp;
+    const int32_t nb = g.h_sc.p->n_classes, nE = g.h_sc.p->n_entries;
+    if (nb == 0) return RAPID_OK;
+    const size_t B = (size_t)nb;
+    std::vector<uint64_t> h1(B), h2(B);
+    std::vector<int32_t> len(B), rep(B), ids, one;
+    RAPID_CUDA(cudaMemcpyAsync(h1.data(), g.c_h1.p, B * 8, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaMemcpyAsync(h2.data(), g.c_h2.p, B * 8, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaMemcpyAsync(len.data(), g.c_len.p, B * 4, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaMemcpyAsync(rep.data(), g.c_rep.p, B * 4, cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
+    ids.reserve((size_t)nE);
+    for (size_t b = 0; b < B; ++b) {
+        const auto key = std::make_tuple(h1[b], h2[b], len[b]);
+        auto it = e->lists.find(key);
+        if (it == e->lists.end()) {
+            int32_t acc = 0;
+            RAPID_CUDA(cudaMemcpyAsync(&acc, L.acc + rep[b], sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+            RAPID_CUDA(cudaStreamSynchronize(s));
+            const int64_t r = cd ? acc - cd->rbegin : -1;
+            if (!cd || r < 0 || r >= cd->R || cd_list(cd, r, h1[b], h2[b], len[b], one) != RAPID_OK) {
+                set_error("the %d-endpoint list held by acceptor %lld is not known: encode the votes that carried it first, or pass the "
+                          "detector whose receiver announced it", len[b], (long long)acc);
+                return RAPID_EINVAL;
+            }
+            it = e->lists.emplace(key, one).first;
+        }
+        ids.insert(ids.end(), it->second.begin(), it->second.end());
+    }
+    RAPID_CHECK(e->ids.reserve((size_t)nE));
+    RAPID_CUDA(cudaMemcpyAsync(e->ids.p, ids.data(), (size_t)nE * 4, cudaMemcpyHostToDevice, s));
+    return RAPID_OK;
+}
+
 static int32_t check_cd(const WireEncCtx& ctx, const rapid_cd* cd) {
     if (cd->view != ctx.view || cd->device != ctx.device) { set_error("the detector was created on another view or device"); return RAPID_EINVAL; }
     if (cd->raw) { set_error("RAW detectors do not announce proposals"); return RAPID_EINVAL; }
@@ -574,8 +564,7 @@ static int32_t check_cd(const WireEncCtx& ctx, const rapid_cd* cd) {
     return RAPID_OK;
 }
 
-// Phase1b (want = 1) / Phase2b (want = 2) answers of the acceptors; each distinct list from the cache, else from the detector
-// receiver with the representative's index
+// Phase1b (want = 1) / Phase2b (want = 2) answers of the acceptors
 static int32_t encode_answers(rapid_wire* w, const rapid_pxa* pxa, const rapid_cd* cd, uint32_t flags, int want, int64_t* n_messages,
                               int64_t* n_bodies) {
     if (!w || !pxa || (flags & ~RAPID_WIRE_REQUEST)) { set_error("bad arguments"); return RAPID_EINVAL; }
@@ -598,19 +587,11 @@ static int32_t encode_answers(rapid_wire* w, const rapid_pxa* pxa, const rapid_c
     ListIn L{};
     L.n = (int32_t)in.n; L.kind = want == 1 ? RAPID_WIRE_PHASE1B : RAPID_WIRE_PHASE2B; L.wrap = (flags & RAPID_WIRE_REQUEST) ? 1 : 0;
     L.cfg = in.cfg; L.acc = in.sender; L.ring0 = ctx.view->ring.p; L.rank = in.rank;
-    if (want == 1) { L.h1 = in.h1; L.h2 = in.h2; L.len = in.len; L.vrnd = in.vrnd; }
-    else { L.c1 = in.v_h1; L.c2 = in.v_h2; L.clen = in.v_len; }
-    const ListFetch fetch = [&](int64_t acc, uint64_t h1, uint64_t h2, int32_t len, std::vector<int32_t>& ids) -> int32_t {
-        const auto key = std::make_tuple(h1, h2, len);
-        auto it = e->lists.find(key);
-        if (it != e->lists.end()) { ids = it->second; return RAPID_OK; }
-        const int64_t r = cd ? acc - cd->rbegin : -1;
-        if (cd && r >= 0 && r < cd->R && cd_list(cd, r, h1, h2, len, ids) == RAPID_OK) { e->lists[key] = ids; return RAPID_OK; }
-        set_error("the %d-endpoint list held by acceptor %lld is not known: encode the votes that carried it first, or pass the "
-                  "detector whose receiver announced it", len, (long long)acc);
-        return RAPID_EINVAL;
-    };
-    RAPID_CHECK(encode_lists(e, ctx, L, fetch));
+    if (want == 1) L.vrnd = in.vrnd;
+    const AnswerFp fp = want == 1 ? AnswerFp{in.h1, in.h2, in.len, 0, 0, 0} : AnswerFp{nullptr, nullptr, nullptr, in.v_h1, in.v_h2, in.v_len};
+    RAPID_CHECK(group_bodies(e, ctx.stream, L.n, fp));
+    RAPID_CHECK(answer_lists(e, ctx.stream, L, cd));
+    RAPID_CHECK(encode_lists(e, ctx, L));
     const EncOut& o = e->out[e->cur];
     if (n_messages) *n_messages = o.n;
     if (n_bodies) *n_bodies = o.n_bodies;
@@ -655,15 +636,9 @@ int32_t rapid_wire_encode_votes(rapid_wire* w, const rapid_cd* cd, int64_t cfg_i
     ListIn L{};
     L.n = (int32_t)cd->R; L.kind = RAPID_WIRE_FAST_ROUND_PHASE2B; L.wrap = (flags & RAPID_WIRE_REQUEST) ? 1 : 0; L.cfg = cfg_id;
     L.rflags = cd->rflags.p; L.rbegin = cd->rbegin; L.ring0 = ctx.view->ring.p;
-    L.h1 = cd->out_h1.p; L.h2 = cd->out_h2.p; L.len = cd->out_len.p;
-    const ListFetch fetch = [&](int64_t pos, uint64_t h1, uint64_t h2, int32_t len, std::vector<int32_t>& ids) -> int32_t {
-        if (cd_list(cd, pos - cd->rbegin, h1, h2, len, ids) != RAPID_OK) {
-            set_error("receiver %lld's proposal does not match its fingerprint", (long long)(pos - cd->rbegin)); return RAPID_EINVAL;
-        }
-        e->lists[std::make_tuple(h1, h2, len)] = ids;
-        return RAPID_OK;
-    };
-    RAPID_CHECK(encode_lists(e, ctx, L, fetch));
+    RAPID_CHECK(group_bodies(e, ctx.stream, L.n, AnnouncedFp{cd->rflags.p, cd->out_h1.p, cd->out_h2.p, cd->out_len.p, 1}));
+    RAPID_CHECK(vote_lists(e, ctx.stream, cd));
+    RAPID_CHECK(encode_lists(e, ctx, L));
     const EncOut& o = e->out[e->cur];
     if (n_messages) *n_messages = o.n;
     if (n_bodies) *n_bodies = o.n_bodies;

@@ -192,6 +192,20 @@ def test_votes_are_byte_identical_share_bodies_and_decode_back(rb, pb, seed, as_
     assert len(voters) > 0
     dec = rb.WireDecoder(c.view)
     enc = dec.encodeVotes(vc, cfg, as_request=as_request)
+    proposals = check_votes(pb, c, vc, voters, enc, cfg, as_request)
+    if split:
+        assert len(proposals) > 1
+    # round trip: senders, configuration and fingerprints as the detector's outputs
+    ring0 = c.view.getRing(0)
+    s, cf, h1, h2, ln = dec.decodeFastRoundPhase2bMessages([enc.message(i) for i in range(len(enc))], is_request=as_request)
+    assert s.tolist() == [int(ring0[r]) for r in voters]
+    assert (cf == cfg).all()
+    assert np.array_equal(h1, res.proposal_hash[voters]) and np.array_equal(h2, res.proposal_hash2[voters])
+    assert np.array_equal(ln, res.proposal_len[voters])
+
+
+def check_votes(pb, c, vc, voters, enc, cfg, as_request):
+    """every vote byte-identical to the runtime's -> {proposal: its body}"""
     assert len(enc) == len(voters)
     ring0 = c.view.getRing(0)
     proposals = {}
@@ -208,17 +222,34 @@ def test_votes_are_byte_identical_share_bodies_and_decode_back(rb, pb, seed, as_
     # one body per distinct proposal, numbered by its lowest receiver, each the encoding of that proposal's list
     assert len(enc.body_off) - 1 == len(proposals) == len(set(proposals.values()))
     assert sorted(proposals.values()) == list(range(len(proposals)))
-    if split:
-        assert len(proposals) > 1
     for ids, b in proposals.items():
         assert enc.body(b) == b"".join(wire_proto.field(3, 2, c.ep(pb, j).SerializeToString(deterministic=True)) for j in ids)
     assert enc.sizes().sum() == sum(len(enc.message(i)) for i in range(len(enc)))
-    # round trip: senders, configuration and fingerprints as the detector's outputs
-    s, cf, h1, h2, ln = dec.decodeFastRoundPhase2bMessages([enc.message(i) for i in range(len(enc))], is_request=as_request)
-    assert s.tolist() == [int(ring0[r]) for r in voters]
-    assert (cf == cfg).all()
-    assert np.array_equal(h1, res.proposal_hash[voters]) and np.array_equal(h2, res.proposal_hash2[voters])
-    assert np.array_equal(ln, res.proposal_len[voters])
+    return proposals
+
+
+def census_state(vc, census, cut_len):
+    """what a user reads of the detector's last census"""
+    from rapid_b200.cut_detector import ProposalCensus
+    c = ProposalCensus(vc, len(census), len(census.ids), cut_len)
+    return ([a.tobytes() for a in (c.hash, c.hash2, c.length, c.voters, c.representative, c.in_cut, c.list_off, c.ids, c.status,
+                                   c.classes())], c.classes_dev)
+
+
+@pytest.mark.parametrize("as_request", [False, True])
+def test_encoding_votes_leaves_the_detectors_census(rb, pb, as_request):
+    """the vote encode lists the proposals in storage of its own: the census taken before it reads back unchanged after it"""
+    c = Cluster(rb, 1000, 0, 1)
+    vc, res = run_votes(rb, c, 1, True)
+    voters = np.nonzero(res.proposal_len > 0)[0]
+    cut = np.unique(np.concatenate([vc.getProposal(int(r)) for r in voters[:3]]))
+    census = vc.proposalCensus(cut)
+    assert len(census) > 1 and (census.in_cut >= 0).all()
+    before = census_state(vc, census, len(cut))
+    enc = rb.WireDecoder(c.view).encodeVotes(vc, 5, as_request=as_request)
+    assert census_state(vc, census, len(cut)) == before
+    proposals = check_votes(pb, c, vc, voters, enc, 5, as_request)
+    assert len(proposals) == len(census)
 
 
 def snapshot(dec):
