@@ -276,9 +276,9 @@ int32_t rapid_cd_read_census(const rapid_cd* cd, uint64_t* hash, uint64_t* hash2
 int32_t rapid_cd_census_classes_dev(const rapid_cd* cd, const int32_t** cls_dev);
 int32_t rapid_cd_read_census_classes(const rapid_cd* cd, int32_t* cls);
 /* getNumProposals :62-66 (the reference's tests are its only caller).  Sweep handles count while they walk the cells.
- * Subject-bucketed handles never see a receiver's cells in order, so they answer by REPLAYING that one receiver through the
- * literal per-cell rule over the epoch's cell log — exact; needs RAPID_CD_LOG at creation (RAPID_EUNSUPPORTED otherwise, or once
- * the epoch held a per-receiver BITMAP delivery or more than 2^24 cells). */
+ * Subject-bucketed handles never see a receiver's cells in order, so they answer by REPLAYING that one receiver's cells from the
+ * epoch's cell log, in its own order, through the sweep kernel — exact; needs RAPID_CD_LOG at creation (RAPID_EUNSUPPORTED
+ * otherwise, or once the epoch held a per-receiver BITMAP delivery or more than 2^24 cells). */
 int32_t rapid_cd_num_proposals(const rapid_cd* cd, int64_t receiver, int32_t* out);
 /* clear() :169-178 + announcedProposal = false (MembershipService.java:425-426) for every receiver. */
 int32_t rapid_cd_clear(rapid_cd* cd);

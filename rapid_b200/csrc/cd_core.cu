@@ -372,9 +372,9 @@ int32_t cd_wait(const CD* ccd, bool take_status) {
     return rc;
 }
 
-static int32_t launch_sweep(CD* cd, int64_t A, const uint8_t* ring_dev, const uint8_t* status_dev, const DeliveryDev& dl,
-                            bool do_cells, bool do_inval, const int64_t* batch_off_dev = nullptr, int32_t n_batches = 0,
-                            int32_t* out_batch_dev = nullptr) {
+// the sweep over the handle's receivers, rows and last prepared cells
+static SweepArgs sweep_args(const CD* cd, int64_t A, const uint8_t* ring_dev, const uint8_t* status_dev, const DeliveryDev& dl,
+                            bool do_cells, bool do_inval, const int64_t* batch_off_dev, int32_t n_batches, int32_t* out_batch_dev) {
     SweepArgs a;
     a.batch_off = batch_off_dev; a.n_batches = n_batches; a.out_batch = out_batch_dev;
     a.K = cd->K; a.H = cd->H; a.L = cd->L; a.raw = cd->raw ? 1 : 0;
@@ -393,6 +393,13 @@ static int32_t launch_sweep(CD* cd, int64_t A, const uint8_t* ring_dev, const ui
     a.n_pre = cd->n_pre.p; a.n_prop = cd->n_prop.p; a.rflags = cd->rflags.p;
     a.out_h1 = cd->out_h1.p; a.out_h2 = cd->out_h2.p; a.out_len = cd->out_len.p; a.out_ann = cd->out_ann.p;
     a.rbegin = cd->rbegin;
+    return a;
+}
+
+static int32_t launch_sweep(CD* cd, int64_t A, const uint8_t* ring_dev, const uint8_t* status_dev, const DeliveryDev& dl,
+                            bool do_cells, bool do_inval, const int64_t* batch_off_dev = nullptr, int32_t n_batches = 0,
+                            int32_t* out_batch_dev = nullptr) {
+    const SweepArgs a = sweep_args(cd, A, ring_dev, status_dev, dl, do_cells, do_inval, batch_off_dev, n_batches, out_batch_dev);
     const int TB = 128;
     RAPID_CUDA(cudaEventRecord(cd->evk0, cd->stream));
     if (dl.flags & RAPID_DELIVERY_SHUFFLED_BATCHES) k_sweep<true><<<(unsigned)ceil_div<int64_t>(cd->R, TB), TB, 0, cd->stream>>>(a);
@@ -486,87 +493,20 @@ static int32_t log_append(CD* cd, int64_t A, const uint8_t* ring_dev, const uint
     return RAPID_OK;
 }
 
-struct ReplayBatch { int64_t c0, c1; int32_t permuted, blocked; uint64_t rs; };
-// ONE receiver, the literal rule (MultiNodeCutDetector.java:84-128, :137-164, MembershipService.java:300-354) over the logged
-// batches in order.  Thread 0 walks the cells; the invalidation pass (order-independent, SURVEY §7) runs across the block.
-__global__ void __launch_bounds__(256) k_replay_receiver(int n_batches, const ReplayBatch* __restrict__ rb, const int32_t* __restrict__ cslot,
-                                                         const uint8_t* __restrict__ cring, const uint8_t* __restrict__ cstatus,
-                                                         const int32_t* __restrict__ order /* permuted batches: cell order of this receiver */,
-                                                         int32_t S, int K, int H, int L, const int32_t* __restrict__ slot_subject,
-                                                         const int32_t* __restrict__ slot_of, const int32_t* __restrict__ obs,
-                                                         uint16_t* __restrict__ m /* [S] zeroed */, uint16_t* __restrict__ tmp /* [S] */,
-                                                         int32_t* __restrict__ out /* [0] numProposals, [1] announced in batch (-1) */) {
-    __shared__ int s_npre, s_seen, s_nprop, s_emitted, s_raised;
-    const uint32_t RM = (1u << K) - 1u;
-    const int t = threadIdx.x;
-    if (t == 0) { s_npre = 0; s_seen = 0; s_nprop = 0; s_emitted = 0; out[1] = -1; }
-    __syncthreads();
-    for (int b = 0; b < n_batches; ++b) {
-        if (rb[b].blocked) continue;                       // nothing delivered to this receiver
-        if (t == 0) {
-            auto emit = [&]() {
-                for (int32_t s = 0; s < S; ++s) { const uint32_t w = m[s]; if (!(w & CD_BIT_EMIT) && __popc(w & RM) >= H) m[s] = (uint16_t)(w | CD_BIT_EMIT); }
-                ++s_nprop; s_emitted = 1;
-            };
-            for (int64_t q = rb[b].c0; q < rb[b].c1; ++q) {
-                const int64_t i = rb[b].permuted ? (int64_t)order[q] : q;
-                const int32_t slot = cslot[i];
-                if (slot < 0) continue;
-                if (cstatus[i] == RAPID_EDGE_DOWN) s_seen = 1;
-                uint32_t w = m[slot];
-                const uint32_t bit = 1u << cring[i];
-                if (w & bit) continue;
-                w |= bit; m[slot] = (uint16_t)w;
-                const int c = __popc(w & RM);
-                if (c == L) ++s_npre;
-                if (c == H) { --s_npre; if (s_npre == 0) emit(); }
-            }
-        }
-        __syncthreads();
-        if (s_seen && s_npre > 0) {                         // invalidateFailingEdges: implicit reports from observers in proposal U preProposal
-            if (t == 0) s_raised = 0;
-            __syncthreads();
-            for (int32_t s = t; s < S; s += 256) {
-                const uint32_t w0 = m[s];
-                uint32_t w = w0;
-                const int c0 = __popc(w0 & RM);
-                if (c0 >= L && c0 < H) {
-                    const int32_t subject = slot_subject[s];
-                    for (int k = 0; k < K; ++k) {
-                        const int32_t o = obs[(size_t)subject * K + k];
-                        const int32_t so = o >= 0 ? slot_of[o] : -1;
-                        if (so < 0 || so >= S) continue;
-                        const uint32_t wo = m[so];
-                        if ((wo & CD_BIT_EMIT) || __popc(wo & RM) < L) continue;
-                        w |= 1u << k;
-                    }
-                    if (__popc(w & RM) >= H) atomicAdd(&s_raised, 1);
-                }
-                tmp[s] = (uint16_t)w;
-            }
-            __syncthreads();
-            for (int32_t s = t; s < S; s += 256) m[s] = tmp[s];
-            __syncthreads();
-            if (t == 0 && s_raised > 0) {
-                s_npre -= s_raised;
-                if (s_npre == 0) {
-                    for (int32_t s = 0; s < S; ++s) { const uint32_t w = m[s]; if (!(w & CD_BIT_EMIT) && __popc(w & RM) >= H) m[s] = (uint16_t)(w | CD_BIT_EMIT); }
-                    ++s_nprop; s_emitted = 1;
-                }
-            }
-            __syncthreads();
-        }
-        if (s_emitted) { if (t == 0) out[1] = b; break; }   // announcedProposal: every later batch is ignored (:318-319)
-    }
-    __syncthreads();
-    if (t == 0) out[0] = s_nprop;
-}
-
 __global__ void k_replay_keys(int64_t c0, int64_t c1, uint64_t rs, uint64_t* __restrict__ key, int32_t* __restrict__ idx) {
     const int64_t i = c0 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= c1) return;
     key[i - c0] = splitmix64(rs ^ (uint64_t)(i - c0));
     idx[i - c0] = (int32_t)i;
+}
+
+__global__ void k_replay_gather(int64_t n, const int32_t* __restrict__ idx, const int32_t* __restrict__ slot, const uint8_t* __restrict__ ring,
+                                const uint8_t* __restrict__ status, int32_t* __restrict__ out_slot, uint8_t* __restrict__ out_ring,
+                                uint8_t* __restrict__ out_status) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const int32_t i = idx[j];
+    out_slot[j] = slot[i]; out_ring[j] = ring[i]; out_status[j] = status[i];
 }
 
 // ---- bucketed handles: one batch (or a whole sequence of batches in one pass: batch_off_dev != nullptr) -----------------------
@@ -809,51 +749,73 @@ static int32_t apply_entry(rapid_cd* cd, int64_t cfg, int64_t n, const int32_t* 
                         sequence ? cd->out_batch.p : nullptr, async, sequence ? batch_off : nullptr);
 }
 
-// getNumProposals of ONE receiver of a bucketed handle: replay its epoch through the literal per-cell rule (the bucketed kernels
-// never see a receiver's cells in order, so they cannot count emissions; the log can)
+// getNumProposals of ONE receiver of a bucketed handle: the sweep kernel on that receiver alone, over the epoch's logged cells in
+// the receiver's own order (the bucketed kernels never see a receiver's cells in order, so they cannot count emissions; the log can)
 static int32_t replay_num_proposals(CD* cd, int64_t receiver, int32_t* out) {
     if (!cd->log_on) { set_error("getNumProposals on the subject-bucketed kernels replays the epoch's cell log: create the handle with RAPID_CD_LOG (or use a RAPID_CD_SWEEP handle)"); return RAPID_EUNSUPPORTED; }
     if (!cd->log_complete) { set_error("the epoch's cell log is incomplete (a per-receiver BITMAP delivery, more than 2^24 cells, or a batch that was not applied)"); return RAPID_EUNSUPPORTED; }
     cudaStream_t s = cd->stream;
-    const size_t nb = cd->log_batches.size();
     const int32_t S = cd->S;
-    if (nb == 0 || S == 0) { *out = 0; return RAPID_OK; }
-    std::vector<ReplayBatch> rb(nb);
-    std::vector<uint8_t> blk(1);
-    DevBuf<int32_t> order, idx, d_out;
-    DevBuf<uint64_t> key, skey;
-    DevBuf<uint16_t> m, tmp;
-    DevBuf<ReplayBatch> d_rb;
-    RadixScratch rs;
-    RAPID_CHECK(order.reserve(std::max<size_t>(cd->log_cells, 1))); RAPID_CHECK(d_out.reserve(2)); RAPID_CHECK(d_rb.reserve(nb));
-    RAPID_CHECK(m.reserve((size_t)S)); RAPID_CHECK(tmp.reserve((size_t)S));
-    RAPID_CUDA(cudaMemsetAsync(m.p, 0, (size_t)S * sizeof(uint16_t), s));
-    for (size_t b = 0; b < nb; ++b) {
-        const CD::LogRec& r = cd->log_batches[b];
-        rb[b].c0 = r.c0; rb[b].c1 = r.c1; rb[b].permuted = (r.flags & RAPID_DELIVERY_PERMUTED) ? 1 : 0; rb[b].blocked = 0;
-        rb[b].rs = splitmix64(r.perm_seed + (uint64_t)(cd->rbegin + receiver));
-        if (r.blocked_off >= 0) {
-            RAPID_CUDA(cudaMemcpyAsync(blk.data(), cd->log_blocked.p + r.blocked_off + receiver, 1, cudaMemcpyDeviceToHost, s));
-            RAPID_CUDA(cudaStreamSynchronize(s));
-            rb[b].blocked = blk[0] ? 1 : 0;
-        }
-        if (rb[b].permuted && !rb[b].blocked && r.c1 > r.c0) {
-            // this receiver's own order of the batch: ascending splitmix64(rs ^ index inside the batch)
-            const int64_t n = r.c1 - r.c0;
-            RAPID_CHECK(key.reserve((size_t)n)); RAPID_CHECK(skey.reserve((size_t)n)); RAPID_CHECK(idx.reserve((size_t)n));
-            k_replay_keys<<<(unsigned)ceil_div<int64_t>(n, 256), 256, 0, s>>>(r.c0, r.c1, rb[b].rs, key.p, idx.p);
-            RAPID_KERNEL_CHECK();
-            RAPID_CHECK(radix_sort_pairs<uint64_t>(rs, key.p, idx.p, skey.p, order.p + r.c0, n, 0, 64, s));
-        }
-    }
-    RAPID_CUDA(cudaMemcpyAsync(d_rb.p, rb.data(), nb * sizeof(ReplayBatch), cudaMemcpyHostToDevice, s));
-    k_replay_receiver<<<1, 256, 0, s>>>((int)nb, d_rb.p, cd->log_slot.p, cd->log_ring.p, cd->log_status.p, order.p, S, cd->K, cd->H, cd->L,
-                                        cd->slot_subject.p, cd->slot_of.p, cd->view->obs.p, m.p, tmp.p, d_out.p);
-    RAPID_KERNEL_CHECK();
-    int32_t h[2] = {0, -1};
-    RAPID_CUDA(cudaMemcpyAsync(h, d_out.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+    if (cd->log_batches.empty() || S == 0) { *out = 0; return RAPID_OK; }
+    // the receiver's byte of every logged blocked array
+    const size_t R = (size_t)cd->R;
+    std::vector<uint8_t> blk(cd->log_blocked_bytes / R);
+    if (!blk.empty()) RAPID_CUDA(cudaMemcpy2DAsync(blk.data(), 1, cd->log_blocked.p + receiver, R, 1, blk.size(), cudaMemcpyDeviceToHost, s));
     RAPID_CUDA(cudaStreamSynchronize(s));
-    *out = h[0];
+    // the batches delivered to the receiver, their cells concatenated in log order (a blocked batch never reaches handleMessage,
+    // so it has no invalidation pass either)
+    std::vector<const CD::LogRec*> kept;
+    std::vector<int64_t> off(1, 0);
+    std::vector<int32_t> idx;
+    for (const CD::LogRec& r : cd->log_batches) {
+        if (r.blocked_off >= 0 && blk[(size_t)r.blocked_off / R]) continue;
+        kept.push_back(&r);
+        for (int64_t i = r.c0; i < r.c1; ++i) idx.push_back((int32_t)i);
+        off.push_back((int64_t)idx.size());
+    }
+    const size_t n = idx.size(), nk = kept.size();
+    struct Receiver { int32_t n_pre, n_prop, len; uint32_t rflags; uint64_t h1, h2; };
+    DevBuf<int32_t> d_idx, kidx, g_slot;
+    DevBuf<uint8_t> g_ring, g_status;
+    DevBuf<int64_t> d_off;
+    DevBuf<uint64_t> key, skey;
+    DevBuf<uint16_t> rows;
+    DevBuf<Receiver> one;
+    RadixScratch sc;
+    RAPID_CHECK(d_idx.reserve(std::max<size_t>(n, 1))); RAPID_CHECK(g_slot.reserve(std::max<size_t>(n, 1)));
+    RAPID_CHECK(g_ring.reserve(std::max<size_t>(n, 1))); RAPID_CHECK(g_status.reserve(std::max<size_t>(n, 1)));
+    RAPID_CHECK(d_off.reserve(nk + 1)); RAPID_CHECK(rows.reserve((size_t)S)); RAPID_CHECK(one.reserve(1));
+    if (n) RAPID_CUDA(cudaMemcpyAsync(d_idx.p, idx.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    for (size_t b = 0; b < nk; ++b) {
+        const CD::LogRec& r = *kept[b];
+        if (!(r.flags & RAPID_DELIVERY_PERMUTED) || r.c1 == r.c0) continue;
+        // this receiver's own order of the batch: ascending splitmix64(rs ^ index inside the batch)
+        const int64_t nc = r.c1 - r.c0;
+        RAPID_CHECK(key.reserve((size_t)nc)); RAPID_CHECK(skey.reserve((size_t)nc)); RAPID_CHECK(kidx.reserve((size_t)nc));
+        k_replay_keys<<<(unsigned)ceil_div<int64_t>(nc, 256), 256, 0, s>>>(r.c0, r.c1, splitmix64(r.perm_seed + (uint64_t)(cd->rbegin + receiver)),
+                                                                          key.p, kidx.p);
+        RAPID_KERNEL_CHECK();
+        RAPID_CHECK(radix_sort_pairs<uint64_t>(sc, key.p, kidx.p, skey.p, d_idx.p + off[b], nc, 0, 64, s));
+    }
+    if (n) {
+        k_replay_gather<<<(unsigned)ceil_div<int64_t>((int64_t)n, 256), 256, 0, s>>>((int64_t)n, d_idx.p, cd->log_slot.p, cd->log_ring.p,
+                                                                                    cd->log_status.p, g_slot.p, g_ring.p, g_status.p);
+        RAPID_KERNEL_CHECK();
+    }
+    RAPID_CUDA(cudaMemcpyAsync(d_off.p, off.data(), (nk + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    RAPID_CUDA(cudaMemsetAsync(rows.p, 0, (size_t)S * sizeof(uint16_t), s));
+    RAPID_CUDA(cudaMemsetAsync(one.p, 0, sizeof(Receiver), s));
+    // the batches of one launch: the sweep stops at the batch in which the receiver announces (MembershipService.java:318-319)
+    SweepArgs a = sweep_args(cd, (int64_t)n, g_ring.p, g_status.p, DeliveryDev(), true, true, d_off.p, (int32_t)nk, nullptr);
+    a.R = 1;
+    a.rows = RowRef{reinterpret_cast<uint8_t*>(rows.p), nullptr, 1, sizeof(uint16_t), 1, 0};
+    a.cell_slot = g_slot.p;
+    a.n_pre = &one.p->n_pre; a.n_prop = &one.p->n_prop; a.rflags = &one.p->rflags;
+    a.out_h1 = &one.p->h1; a.out_h2 = &one.p->h2; a.out_len = &one.p->len; a.out_ann = nullptr;
+    k_sweep<false><<<1, 1, 0, s>>>(a);
+    RAPID_KERNEL_CHECK();
+    RAPID_CUDA(cudaMemcpyAsync(out, &one.p->n_prop, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    RAPID_CUDA(cudaStreamSynchronize(s));
     return RAPID_OK;
 }
 
@@ -1092,15 +1054,28 @@ int32_t rapid_cd_sequence_stats(const rapid_cd* cd, int32_t* one_pass, int32_t* 
     return RAPID_OK;
 }
 
-static int32_t gather_sorted(const rapid_cd* cd, int32_t n, std::vector<int32_t>& ids, std::vector<int64_t>* keys,
-                             const DevBuf<int32_t>& d_ids, const DevBuf<int64_t>* d_keys) {
-    ids.resize((size_t)n);
-    if (n) RAPID_CUDA(cudaMemcpy(ids.data(), d_ids.p, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    if (keys) {
-        keys->resize((size_t)n);
-        if (n) RAPID_CUDA(cudaMemcpy(keys->data(), d_keys->p, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost));
+// RAW mode, after a sweep: what the call emitted for `receiver` (ascending; at most cap ids, *out_len = all of them), then the
+// call marks of every receiver cleared
+static int32_t take_call_marks(rapid_cd* cd, int64_t receiver, int32_t* out_ids, int32_t cap, int32_t* out_len) {
+    DevBuf<int32_t> d_ids, d_cnt;
+    const int32_t S = cd->S;
+    RAPID_CHECK(d_ids.reserve((size_t)std::max(S, 1)));
+    RAPID_CHECK(d_cnt.reserve(1));
+    RAPID_CUDA(cudaMemsetAsync(d_cnt.p, 0, sizeof(int32_t), cd->stream));
+    int32_t n = 0;
+    if (S > 0) {
+        k_gather_call<<<(unsigned)ceil_div<int32_t>(S, 256), 256, 0, cd->stream>>>(rowref(cd), S, receiver, cd->slot_subject.p, d_ids.p, S, d_cnt.p);
+        dim3 grid((unsigned)ceil_div<int64_t>(cd->R, 256), (unsigned)S);
+        k_clear_call<<<grid, 256, 0, cd->stream>>>(rowref(cd), S, cd->R);
+        RAPID_KERNEL_CHECK();
+        RAPID_CUDA(cudaMemcpyAsync(&n, d_cnt.p, sizeof(int32_t), cudaMemcpyDeviceToHost, cd->stream));
     }
-    (void)cd;
+    RAPID_CUDA(cudaStreamSynchronize(cd->stream));
+    std::vector<int32_t> ids((size_t)n);
+    if (n) RAPID_CUDA(cudaMemcpy(ids.data(), d_ids.p, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    std::sort(ids.begin(), ids.end());
+    *out_len = n;
+    for (int32_t i = 0; i < n && i < cap; ++i) out_ids[i] = ids[(size_t)i];
     return RAPID_OK;
 }
 
@@ -1114,27 +1089,7 @@ int32_t rapid_cd_aggregate(rapid_cd* cd, int64_t n_cells, const int32_t* src, co
     Staged st;
     RAPID_CHECK(stage_cells(cd, n_cells, dst, ring, status, nullptr, nullptr, &st));
     RAPID_CHECK(apply_common(cd, 0, n_cells, st.dst, st.ring, st.status, nullptr, DeliveryDev()));
-    // collect what this call emitted for `receiver`, then clear the call marks of every receiver
-    DevBuf<int32_t> d_ids, d_cnt;
-    const int32_t S = cd->S;
-    RAPID_CHECK(d_ids.reserve((size_t)std::max(S, 1)));
-    RAPID_CHECK(d_cnt.reserve(1));
-    RAPID_CUDA(cudaMemsetAsync(d_cnt.p, 0, sizeof(int32_t), cd->stream));
-    int32_t n = 0;
-    if (S > 0) {
-        k_gather_call<<<(unsigned)ceil_div<int32_t>(S, 256), 256, 0, cd->stream>>>(rowref(cd), S, receiver, cd->slot_subject.p, d_ids.p, S, d_cnt.p);
-        dim3 grid((unsigned)ceil_div<int64_t>(cd->R, 256), (unsigned)S);
-        k_clear_call<<<grid, 256, 0, cd->stream>>>(rowref(cd), S, cd->R);
-        RAPID_KERNEL_CHECK();
-        RAPID_CUDA(cudaMemcpyAsync(&n, d_cnt.p, sizeof(int32_t), cudaMemcpyDeviceToHost, cd->stream));
-    }
-    RAPID_CUDA(cudaStreamSynchronize(cd->stream));
-    std::vector<int32_t> ids;
-    RAPID_CHECK(gather_sorted(cd, n, ids, nullptr, d_ids, nullptr));
-    std::sort(ids.begin(), ids.end());
-    *out_len = n;
-    for (int32_t i = 0; i < n && i < cap; ++i) out_ids[i] = ids[(size_t)i];
-    return RAPID_OK;
+    return take_call_marks(cd, receiver, out_ids, cap, out_len);
 }
 
 int32_t rapid_cd_invalidate(rapid_cd* cd, int64_t receiver, int32_t* out_ids, int32_t cap, int32_t* out_len) {
@@ -1145,26 +1100,7 @@ int32_t rapid_cd_invalidate(rapid_cd* cd, int64_t receiver, int32_t* out_ids, in
     cd->last_launches = 0;
     RAPID_CHECK(ensure_id_capacity(cd));
     RAPID_CHECK(launch_sweep(cd, 0, nullptr, nullptr, DeliveryDev(), false, true));
-    DevBuf<int32_t> d_ids, d_cnt;
-    const int32_t S = cd->S;
-    RAPID_CHECK(d_ids.reserve((size_t)std::max(S, 1)));
-    RAPID_CHECK(d_cnt.reserve(1));
-    RAPID_CUDA(cudaMemsetAsync(d_cnt.p, 0, sizeof(int32_t), cd->stream));
-    int32_t n = 0;
-    if (S > 0) {
-        k_gather_call<<<(unsigned)ceil_div<int32_t>(S, 256), 256, 0, cd->stream>>>(rowref(cd), S, receiver, cd->slot_subject.p, d_ids.p, S, d_cnt.p);
-        dim3 grid((unsigned)ceil_div<int64_t>(cd->R, 256), (unsigned)S);
-        k_clear_call<<<grid, 256, 0, cd->stream>>>(rowref(cd), S, cd->R);
-        RAPID_KERNEL_CHECK();
-        RAPID_CUDA(cudaMemcpyAsync(&n, d_cnt.p, sizeof(int32_t), cudaMemcpyDeviceToHost, cd->stream));
-    }
-    RAPID_CUDA(cudaStreamSynchronize(cd->stream));
-    std::vector<int32_t> ids;
-    RAPID_CHECK(gather_sorted(cd, n, ids, nullptr, d_ids, nullptr));
-    std::sort(ids.begin(), ids.end());
-    *out_len = n;
-    for (int32_t i = 0; i < n && i < cap; ++i) out_ids[i] = ids[(size_t)i];
-    return RAPID_OK;
+    return take_call_marks(cd, receiver, out_ids, cap, out_len);
 }
 
 int32_t rapid_cd_get_proposal(const rapid_cd* cd, int64_t receiver, int32_t* out_ids, int32_t cap, int32_t* out_len) {
@@ -1189,9 +1125,12 @@ int32_t rapid_cd_get_proposal(const rapid_cd* cd, int64_t receiver, int32_t* out
     int32_t n = 0;
     RAPID_CUDA(cudaMemcpyAsync(&n, d_cnt.p, sizeof(int32_t), cudaMemcpyDeviceToHost, cd->stream));
     RAPID_CUDA(cudaStreamSynchronize(cd->stream));
-    std::vector<int32_t> ids;
-    std::vector<int64_t> keys;
-    RAPID_CHECK(gather_sorted(cd, n, ids, &keys, d_ids, &d_keys));
+    std::vector<int32_t> ids((size_t)n);
+    std::vector<int64_t> keys((size_t)n);
+    if (n) {
+        RAPID_CUDA(cudaMemcpy(ids.data(), d_ids.p, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost));
+        RAPID_CUDA(cudaMemcpy(keys.data(), d_keys.p, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost));
+    }
     std::vector<int32_t> order((size_t)n);
     for (int32_t i = 0; i < n; ++i) order[(size_t)i] = i;
     // sorted(membershipView.getRingZeroComparator())  MembershipService.java:346-348 (signed key; id breaks exact ties)

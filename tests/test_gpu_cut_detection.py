@@ -273,22 +273,28 @@ def test_num_proposals_sweep(orc, rb):
         assert cl.getNumProposals(r) == sim.numProposals(r)
 
 
-@pytest.mark.parametrize("seed", range(6))
-def test_num_proposals_on_the_bucketed_kernels_by_replay(orc, rb, seed):
+# (K, seed): the K = 10 seeds, then K = 3 and K = 14, so the replay meets both bucketed row formats.  (H, L) by seed % 3, with H = K
+# among them; at K = 3 and 14 every case emits in some epoch.
+NUM_PROP = [(10, s) for s in range(6)] + [(Kx, s) for Kx in (3, 14) for s in range(3)]
+NUM_PROP_HL = {10: ((8, 2), (9, 4), (3, 1)), 3: ((3, 3), (3, 2), (2, 2)), 14: ((14, 6), (14, 14), (5, 2))}
+
+
+@pytest.mark.parametrize("Kx,seed", NUM_PROP, ids=["%d%s" % (s, "" if Kx == 10 else "-K%d" % Kx) for Kx, s in NUM_PROP])
+def test_num_proposals_on_the_bucketed_kernels_by_replay(orc, rb, Kx, seed):
     """getNumProposals (MultiNodeCutDetector.java:62-66) on a bucketed handle created with RAPID_CD_LOG: the receiver asked about is
     replayed through the per-cell rule over the epoch's cell log — several batches, blocked receivers, permuted delivery, a
     sequence call, several emissions inside one batch (small H / L); after clear() the count starts over."""
-    rng = np.random.default_rng(4100 + seed)
+    rng = np.random.default_rng(4100 + seed if Kx == 10 else (4100, Kx, seed))
     n = int(rng.integers(40, 600))
-    Hh, Ll = [(8, 2), (9, 4), (3, 1)][seed % 3]
-    w = OracleWorld(orc, n, K)
-    v = rb.MembershipView.from_packed(K, *w.member_packed())
-    sim = orc.ClusterSim(w.view, K, Hh, Ll, n)
+    Hh, Ll = NUM_PROP_HL[Kx][seed % 3]
+    w = OracleWorld(orc, n, Kx)
+    v = rb.MembershipView.from_packed(Kx, *w.member_packed())
+    sim = orc.ClusterSim(w.view, Kx, Hh, Ll, n)
     cl = rb.VirtualCluster(v, Hh, Ll, kernel="bucketed", log=True)
     cfg = w.view.getCurrentConfigurationId()
     for epoch in range(2):
         for call in range(3):
-            src, dst, ring, status = random_batch(rng, n, K, int(rng.integers(1, 7)), int(rng.integers(10, 90)), n)
+            src, dst, ring, status = random_batch(rng, n, Kx, int(rng.integers(1, 7)), int(rng.integers(10, 90)), n)
             blocked = (rng.random(n) < 0.15).astype(np.uint8) if call == 1 else None
             perm = int(rng.integers(1, 2**60)) if (seed + call) % 2 else None
             if call == 2:
